@@ -2,7 +2,10 @@
 """Benchmark of the hot path: SD1.5 LoRA (rank 8, every attn1/attn2 Linear) training step, 512x512 (64x64 latents),
 batch 4 per GPU, bf16 kernels / fp32 master weights -- BASELINE.json `configs[1]`, metric "LoRA-train images/sec".
 
-  python bench.py [--gpus N] [--steps K] [--warmup W]            product arm (B200 kernels)
+  python bench.py [--gpus N] [--steps K] [--warmup W]            product arm (H100 kernels)
+  python bench.py ... --dump-outputs DIR                         also write, after the K timed steps, what the last of them computed
+                                                                 (the step's loss, noise prediction and trained fp32 parameters) as
+                                                                 DIR/<name>.npy
   python bench.py --impl reference [--gpus N] ...                CPU arm: the oracle restatement of the reference path
                                                                  (diffusers UNet semantics + hcpdiff LoRA operator + train_ac
                                                                  step order) on the host cores -- the reference itself cannot
@@ -31,12 +34,19 @@ PER_GPU_BATCH = 4
 LORA_RANK = 8
 
 
+# H100 SXM data sheet (700 W): dense BF16 989 TFLOP/s, HBM3 3.35 TB/s.  A denominator, never a value this run reached.
+H100_BF16_TFLOPS = 989.0
+H100_HBM_GBS = 3350.0
+DUMP_MAX_ELEMS = 8 << 20         # elements of one array written by --dump-outputs before a seeded sample is taken (32 MB in fp32)
+
+
 def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("bf16_tflops_sustained", 1423.3), d.get("bf16_tflops", 1713.4), d.get("hbm_gbs", 6567.7), "measured"
-    return 1400.0, 1590.0, 6650.0, "fallback"
+        return (d.get("bf16_tflops_sustained", H100_BF16_TFLOPS), d.get("bf16_tflops", H100_BF16_TFLOPS), d.get("hbm_gbs", H100_HBM_GBS),
+                "measured")
+    return H100_BF16_TFLOPS, H100_BF16_TFLOPS, H100_HBM_GBS, "H100 SXM data sheet"
 
 
 def usable_cores() -> int:
@@ -182,28 +192,6 @@ def time_kernel(fn, iters=10):
     return e0.elapsed_time(e1) / iters
 
 
-def ncu_dram_traffic(summary=None):
-    """DRAM bytes (read + write) of ONE launch of the dominant kernel, from the committed `ncu --set full` summary of the same
-    kernel at the same shape (attention backward, B=4 H=8 L=4096 d=40).  None when the file is absent."""
-    import csv
-    here = os.path.dirname(os.path.abspath(__file__))
-    if summary is None:          # the newest committed capture of the kernel
-        summary = next((n for n in ("profiles/r02_ncu_attn_bwd.summary.csv", "profiles/r01_ncu_attn_bwd_v23.summary.csv")
-                        if os.path.exists(os.path.join(here, n))), "profiles/r01_ncu_attn_bwd_v23.summary.csv")
-    path = os.path.join(here, summary)
-    try:
-        rows = list(csv.reader(open(path)))
-        hdr, unit, val = rows[0], rows[1], rows[2]
-        scale = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-        tot = 0.0
-        for name in ("dram__bytes_read.sum", "dram__bytes_write.sum"):
-            i = hdr.index(name)
-            tot += float(val[i]) * scale[unit[i]]
-        return {"bytes_per_launch": tot, "kernel": "attn_bwd_kernel B4 H8 L4096 d40", "source": summary}
-    except (OSError, ValueError, KeyError, IndexError):
-        return None
-
-
 def dominant_kernel_roofline(peak_tflops):
     """Live CUDA-event timing of the kernels that dominate the step, at their benchmark shapes (B=4)."""
     from hcp_diffusion_b200 import ops
@@ -271,29 +259,25 @@ def count_step_flops(step, host):
     return total[0] / 3.0
 
 
-def attn_tensor_pipe_pct():
-    """BASELINE.json's second metric, "attn tensor-pipe % of peak": sm__pipe_tensor... pct of peak of the attention kernels at the
-    benchmark shape (B=4, H=8, L=4096, d=40), read from the committed `ncu --set full` summaries (a number taken under a profiler is
-    never a bench value: this is evidence attached to the line, not something measured by this run)."""
-    import csv
-    out = {}
-    for key, names in (("fwd", ("profiles/r02_ncu_attn_fwd.summary.csv", "profiles/r01_ncu_attn_fwd_v23.summary.csv")),
-                       ("bwd", ("profiles/r02_ncu_attn_bwd.summary.csv", "profiles/r01_ncu_attn_bwd_v23.summary.csv"))):
-        for name in names:
-            path = os.path.join(ROOT, name)
-            try:
-                rows = list(csv.reader(open(path)))
-                hdr, val = rows[0], rows[2]
-                # the SM-average over the kernel's whole duration (not the busiest SM, not "while active")
-                pref = "sm__pipe_tensor_cycles_active.avg.pct_of_peak_sustained_elapsed"
-                cols = [i for i, h in enumerate(hdr) if h == pref] or \
-                       [i for i, h in enumerate(hdr) if h.startswith("sm__pipe_tensor") and "avg.pct_of_peak_sustained_elapsed" in h]
-                if cols:
-                    out[key] = {"pct": float(val[cols[0]]), "metric": hdr[cols[0]], "source": name}
-                    break
-            except (OSError, ValueError, IndexError):
-                continue
-    return out or None
+def dump_outputs(out_dir, step):
+    """What the timed path hands its caller after its last step: the step's loss, its noise prediction (the UNet output, fp32) and the
+    trained fp32 parameters (the flat master buffer, in parameter order).  An array above DUMP_MAX_ELEMS elements is written as a fixed
+    sample: the elements at DUMP_MAX_ELEMS sorted indices drawn with torch.randint from a generator seeded with 0, the same on every run
+    and build."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+
+    def save(name, t):
+        flat = t.detach().reshape(-1)
+        if flat.numel() > DUMP_MAX_ELEMS:
+            idx = torch.randint(flat.numel(), (DUMP_MAX_ELEMS,), generator=torch.Generator().manual_seed(0)).sort().values
+            flat = flat[idx.to(flat.device)]
+        np.save(os.path.join(out_dir, name + ".npy"), flat.float().cpu().numpy())
+
+    save("loss", step.loss)
+    save("noise_pred", step.noise_pred)
+    save("params", step.flat.data)
 
 
 def run_product_arm(args, rank, world, local_rank):
@@ -306,6 +290,7 @@ def run_product_arm(args, rank, world, local_rank):
 
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
+    torch.manual_seed(0)             # adapter initialisation: the same inputs and weights on every run with the same arguments
     _lib.check(_lib.lib().hcp_device_check(), "hcp_device_check")
     sustained, burst, hbm, peak_src = measured_peaks()
 
@@ -415,6 +400,8 @@ def run_product_arm(args, rank, world, local_rank):
     sampler.start()
     ms_resident = timed(resident_step, args.steps)
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, step)
     ms_e2e = timed(e2e_step, args.steps)
     # sustained leg: at least 3 s of back-to-back steps (the short timed region above runs at boost clocks; a training job does not)
     n_sus = max(args.steps, int(3200.0 / max(ms_resident / args.steps, 1e-3)) + 1)
@@ -444,7 +431,7 @@ def run_product_arm(args, rank, world, local_rank):
         "config": {"workload": (what % n_train) + ", " + res_txt + "; step = add_noise + UNet fwd + MSE + bwd + grad all-reduce + clip + AdamW",
                    "baseline_config": args.config, "global_batch": world * B, "per_gpu_batch": B, "lora_rank": {2: LORA_RANK, 3: 0, 4: 16}[args.config],
                    "parallelism": f"dp{world}",
-                   "l2": "working set (1.7 GB bf16 weights + activations) is far larger than the 126 MB L2; no explicit flush",
+                   "l2": "working set (1.7 GB bf16 weights + activations) is far larger than the 50 MB L2; no explicit flush",
                    "cuda_graph": use_graph, "grad_checkpointing": False,
                    "side_stream": os.environ.get("HCP_SIDE_STREAM", "1") != "0", "pdl": os.environ.get("HCP_PDL", "1") != "0"},
         "clocks": clocks,
@@ -454,10 +441,9 @@ def run_product_arm(args, rank, world, local_rank):
         "gpu_launches": launches_per_step * args.steps,
         "roofline": {"bound": "tensor", "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
                      "frac_vs_burst": achieved / burst, "frac_vs_sustained": achieved / sustained,
-                     "traffic": ncu_dram_traffic(),
                      "peak_source": f"{peak_src} {'bf16_tflops (burst: the timed region ran at boost clocks)' if boosted else 'bf16_tflops_sustained'}; "
                                     f"burst {burst}, sustained {sustained}",
-                     "flop_per_image": f_step, "kernels": kern, "attn_tensor_pipe_pct": attn_tensor_pipe_pct()},
+                     "flop_per_image": f_step, "kernels": kern},
         "final_loss": losses[-1],
     }
     if world == 1 and not args.no_cpu_baseline and args.config == 2:
@@ -475,6 +461,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="hcpb200", choices=["hcpb200", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's loss, noise prediction and trained fp32 parameters as DIR/<name>.npy")
     ap.add_argument("--config", type=int, default=2, choices=[2, 3, 4],
                     help="BASELINE.json config: 2 = SD1.5 LoRA r8 bs 4/GPU (the headline, default); 3 = SD1.5 full fine-tune bs 16/GPU; "
                          "4 = SDXL-base LoRA r16 attn + Conv2d bs 2/GPU, 1024x1024")

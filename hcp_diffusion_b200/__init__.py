@@ -1,4 +1,4 @@
-"""hcp_diffusion_b200 -- B200-native (sm_100a) UNet denoising hot path behind HCP-Diffusion's plugin surface.
+"""hcp_diffusion_b200 -- H100-native (sm_90a) UNet denoising hot path behind HCP-Diffusion's plugin surface.
 
 Only the hot path of the reference (IrisRainbowNeko/HCP-Diffusion) is provided: the SD1.x `UNet2DConditionModel`
 forward/backward with layer-wise LoRA adapters, the cfg-driven layer selection (`make_hcpdiff`, `re:` patterns), the LoRA

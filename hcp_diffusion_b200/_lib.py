@@ -18,7 +18,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("HCP_LIB", os.path.join(_HERE, "lib", "libhcpb200.so"))     # HCP_LIB: an alternative build (A/B experiments)
 CSRC = os.path.join(_HERE, "csrc")
 SOURCES = ["gemm.cu", "host_util.cu", "attention.cu", "norms.cu", "misc.cu", "step.cu", "wgrad.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "--shared", "-Xcompiler", "-fPIC"]
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "--shared", "-Xcompiler", "-fPIC"]
 
 MAX_SEG = 3
 
@@ -28,14 +28,14 @@ class HcpError(RuntimeError):
 
 
 def build(verbose: bool = False) -> str:
-    """Compile the CUDA sources for sm_100a into lib/libhcpb200.so (nvcc cross-compiles without a GPU)."""
+    """Compile the CUDA sources for sm_90a into lib/libhcpb200.so (nvcc cross-compiles without a GPU)."""
     os.makedirs(os.path.dirname(LIB_PATH), exist_ok=True)
     srcs = [os.path.join(CSRC, s) for s in SOURCES]
-    newest = max(os.path.getmtime(p) for p in srcs + [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "host_util.h"),
-                                                      os.path.join(_HERE, "..", "include", "hcp_b200.h")])
+    newest = max(os.path.getmtime(p) for p in srcs + [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "wgmma.cuh"),
+                                                      os.path.join(CSRC, "host_util.h"), os.path.join(_HERE, "..", "include", "hcp_b200.h")])
     if os.path.exists(LIB_PATH) and os.path.getmtime(LIB_PATH) >= newest:
         return LIB_PATH
-    cmd = ["nvcc", *NVCC_FLAGS, *os.environ.get("HCP_EXTRA_NVCC_FLAGS", "").split(), "-o", LIB_PATH, *srcs, "-lcudart"]   # e.g. -DHCP_ATTN_TRACE
+    cmd = ["nvcc", *NVCC_FLAGS, *os.environ.get("HCP_EXTRA_NVCC_FLAGS", "").split(), "-o", LIB_PATH, *srcs, "-lcudart"]
     if verbose:
         print(" ".join(cmd))
     subprocess.run(cmd, check=True)

@@ -1,5 +1,5 @@
 // SPDX-License-Identifier: Apache-2.0
-// Fused scaled-dot-product attention for sm_100a (tcgen05 + TMA), forward and backward.
+// Fused scaled-dot-product attention for sm_90a (wgmma + TMA), forward and backward.
 //
 // Replaces: diffusers Attention (AttnProcessor2_0 -> F.scaled_dot_product_attention, or xFormers when
 // `enable_xformers`, reference hcpdiff/train_ac.py:258-263) inside BasicTransformerBlock.attn1/attn2
@@ -7,18 +7,20 @@
 //
 // Layout: Q/K/V/O are token-major bf16 matrices [B, L, ld] in which head h occupies columns [h*d, (h+1)*d) -- the
 // layout the (fused) projection GEMMs write and the out-projection GEMM reads, so no head permute ever exists in
-// HBM.  A 4D TMA map (d, H, L, B) with box (64, 1, 128, 1) lands a [128 x 64] K-major SWIZZLE_128B tile of one head
+// HBM.  A 4D TMA map (d, H, L, B) with box (64, 1, rows, 1) lands a [rows x 64] K-major SWIZZLE_128B tile of one head
 // in shared memory; columns >= d and rows >= L are zero-filled by the TMA unit.
 //
-// Forward, one CTA per (128 query rows, head, image), 4 softmax warps + 1 control warp:
-//   S = Q K^T            tcgen05.mma SS, fp32 S in TMEM columns [0,128)
-//   online softmax       thread == row (tcgen05.ld 32x32b); exp2 with folded scale; running max is only refreshed
-//                        (and O rescaled in TMEM) when it grows by > 2^8, so the rescale is rare
-//   P (bf16)             written back to TMEM over the S columns (tcgen05.st) and fed as the A operand from TMEM
-//   O += P V             tcgen05.mma TS; V tile is used straight from its row-major TMA box as an MN-major operand
-// Backward, one CTA per (128 kv rows, head, image) looping over query tiles:
-//   S = Q K^T, dP = dO V^T (TMEM) -> P, dS (bf16, smem) -> dV += P^T dO, dK += dS^T Q (TMEM accumulators,
-//   MN-major A operands), dQ_i = dS K (TMEM) reduced into an fp32 buffer with vector red.global.
+// Forward, one CTA per (128 query rows, head, image): two MMA warpgroups of 64 query rows each + one TMA warp.
+//   S = Q K^T            wgmma SS, fp32 S in registers
+//   online softmax       on the accumulator fragments (a row lives in the four lanes of a quad); exp2 with folded scale
+//   O += P V             wgmma RS: P (bf16) goes from the S registers straight into the A operand; V is used from its
+//                        row-major TMA box as an MN-major operand
+// Backward, one CTA per (128 kv rows, head, image, output column slice of 64) looping over 64-row query tiles; warpgroup g owns
+// kv rows [64g, 64g+64):
+//   S^T = K Q^T, dP^T = V dO^T (registers) -> P^T, dS^T -> dV += P^T dO, dK += dS^T Q (wgmma RS, accumulators in registers),
+//   dQ_i += dS K over all 128 kv rows of the CTA (dS^T of both warpgroups staged in shared memory as one MN-major operand; the
+//   warpgroups take turns per query tile), reduced into an fp32 buffer with vector red.global: one contribution per CTA, so a
+//   short kv range (<= 2 tiles) sums dQ in an order-independent way.
 #include <stdlib.h>
 #include "common.cuh"
 #include "host_util.h"
@@ -26,28 +28,29 @@
 
 namespace hcp {
 
-constexpr int kAttnThreads = 160;          // fwd: warps 0-3: softmax/epilogue rows, warp 4: TMA + MMA control
-constexpr int kBwdParts = 4;               // bwd: softmax warps per TMEM lane quarter (each owns 128/kBwdParts kv columns): 16 warps hide
-                                           // the TMEM-load / MUFU latencies that 8 warps (2 per scheduler) left exposed (ncu: 2.25 active warps,
-                                           // issue slot used every 3.1 cycles); 16-column register chunks keep them under the 120-register cap
-constexpr int kBwdSoftmaxThreads = 4 * kBwdParts * 32;
-constexpr int kAttnBwdThreads = kBwdSoftmaxThreads + 3 * 32;   // + three single-thread warps: S/dP issue (+ TMA), dV/dK/dQ issue, Q/dO refill
-constexpr int TILE_BYTES = 128 * 128;      // one [128 rows x 64 cols] bf16 box
+constexpr int kAttnThreads = 288;          // warps 0-7: two MMA warpgroups, warp 8: TMA
+constexpr int BOX_BYTES = 128 * 128;       // one [128 rows x 64 cols] bf16 box
 constexpr float kLog2e = 1.4426950408889634f;
 constexpr float kLn2 = 0.6931471805599453f;
 
-__device__ __forceinline__ uint32_t lane_base(int warp) { return static_cast<uint32_t>(warp * 32) << 16; }
+// offset (in 16-byte units) of k-step ks inside a K-major operand made of 64-column SWIZZLE_128B boxes of `box_bytes` each
+__device__ __forceinline__ uint32_t kmajor_off(int ks, int box_bytes) { return (uint32_t)((ks >> 2) * (box_bytes >> 4) + (ks & 3) * 2); }
+__device__ __forceinline__ float quad_max(float v) {
+    v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+    return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+__device__ __forceinline__ float quad_sum(float v) {
+    v += __shfl_xor_sync(0xffffffffu, v, 1);
+    return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
 
 // =============================================================================================
 // forward
 // =============================================================================================
 struct alignas(64) AttnFwdParams {
-    CUtensorMap tmQ, tmK, tmV;
+    CUtensorMap tmQ, tmK, tmV;   // Q: boxes of 128 rows; K / V: boxes of KVT rows
     int B, H, Lq, Lkv, d;
-    int nbox;            // ceil(d / 64)
-    int dn;              // d rounded up to a multiple of 16
-    int tmem_cols;
-    int kv_stages;       // 2, or 1 when the tiles are too large (d > 128)
+    int nks;             // 16-wide k-steps of Q K^T: ceil(d / 16)
     float scale_log2;    // softmax scale * log2(e)
     const float* kv_bias;   // [B, Lkv] additive bias (natural-log units) or nullptr
     __nv_bfloat16* O;
@@ -55,1142 +58,377 @@ struct alignas(64) AttnFwdParams {
     float* lse;          // [B, H, Lq], natural log
 };
 
-__global__ void __launch_bounds__(kAttnThreads, 1) attn_fwd_kernel(const __grid_constant__ AttnFwdParams p) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    const int tile_bytes = p.nbox * TILE_BYTES;
-    uint8_t* sQ = smem;
-    uint8_t* sK = sQ + tile_bytes;           // kv_stages
-    uint8_t* sV = sK + p.kv_stages * tile_bytes;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sV + p.kv_stages * tile_bytes);
-    uint64_t* q_full = bars + 0;
-    uint64_t* kv_full = bars + 1;    // [2]
-    uint64_t* s_full = bars + 3;
-    uint64_t* p_ready = bars + 4;
-    uint64_t* pv_done = bars + 5;    // [2]
-    uint64_t* o_full = bars + 7;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 8);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
-    const int nkv = (p.Lkv + 127) / 128;
-
-    if (threadIdx.x == 0) {
-        mbar_init(q_full, 1);
-        mbar_init(&kv_full[0], 1);
-        mbar_init(&kv_full[1], 1);
-        mbar_init(s_full, 1);
-        mbar_init(p_ready, 128);
-        mbar_init(&pv_done[0], 1);
-        mbar_init(&pv_done[1], 1);
-        mbar_init(o_full, 1);
-        fence_mbar_init();
-    }
-    if (warp == 4) {
-        tmem_alloc(tmem_slot, p.tmem_cols);
-        tmem_relinquish();
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
-    pdl_trigger();
-    pdl_wait();
-    const uint32_t tS = tmem;            // S fp32 [128 cols]; P bf16 packed aliases columns [0,64)
-    const uint32_t tO = tmem + 128;
-
-    if (warp == 4) {
-        if (elect_one()) {
-            auto load_kv = [&](int j) {
-                const int st = (p.kv_stages == 2) ? (j & 1) : 0;
-                mbar_arrive_expect_tx(&kv_full[st], 2 * tile_bytes);
-                for (int bx = 0; bx < p.nbox; ++bx) {
-                    tma_load_4d(sK + st * tile_bytes + bx * TILE_BYTES, &p.tmK, &kv_full[st], bx * 64, h, j * 128, b);
-                    tma_load_4d(sV + st * tile_bytes + bx * TILE_BYTES, &p.tmV, &kv_full[st], bx * 64, h, j * 128, b);
-                }
-            };
-            mbar_arrive_expect_tx(q_full, tile_bytes);
-            for (int bx = 0; bx < p.nbox; ++bx)
-                tma_load_4d(sQ + bx * TILE_BYTES, &p.tmQ, q_full, bx * 64, h, qt * 128, b);
-            load_kv(0);
-            if (p.kv_stages == 2 && nkv > 1) load_kv(1);
-            mbar_wait(q_full, 0);
-            for (int j = 0; j < nkv; ++j) {
-                const int st = (p.kv_stages == 2) ? (j & 1) : 0;
-                const uint32_t ph = (p.kv_stages == 2) ? ((j >> 1) & 1) : (j & 1);
-                const int ncols = min(128, p.Lkv - j * 128);
-                const int n16 = (ncols + 15) & ~15;
-                mbar_wait(&kv_full[st], ph);
-                tc_fence_after();
-                // ---- S = Q K^T
-                const uint32_t idesc_s = make_idesc_bf16(128, n16, 0, 0);
-                const uint32_t kbase = smem_u32(sK + st * tile_bytes);
-                const uint32_t qbase = smem_u32(sQ);
-                for (int ks = 0; ks < p.dn / 16; ++ks) {
-                    const uint32_t off = (ks >> 2) * TILE_BYTES + (ks & 3) * 32;
-                    umma_ss(tS, make_smem_desc(qbase + off, 16, 1024), make_smem_desc(kbase + off, 16, 1024), idesc_s,
-                            ks > 0);
-                }
-                umma_commit(s_full);
-                // while the softmax warps work on tile j: refill the stage tile j-1 used
-                if (p.kv_stages == 2 && j >= 1 && j + 1 < nkv) {
-                    mbar_wait(&pv_done[(j - 1) & 1], ((j - 1) >> 1) & 1);
-                    load_kv(j + 1);
-                }
-                mbar_wait(p_ready, j & 1);
-                tc_fence_after();
-                // ---- O += P V   (A = P from TMEM, B = V tile as MN-major operand)
-                const uint32_t idesc_pv = make_idesc_bf16(128, p.dn, 0, 1);
-                const uint32_t vbase = smem_u32(sV + st * tile_bytes);
-                for (int ks = 0; ks < n16 / 16; ++ks) {
-                    umma_ts(tO, tS + ks * 8, make_smem_desc(vbase + ks * 2048, TILE_BYTES, 1024), idesc_pv,
-                            (j > 0 || ks > 0) ? 1u : 0u);
-                }
-                umma_commit(&pv_done[st]);
-                if (p.kv_stages == 1 && j + 1 < nkv) {
-                    mbar_wait(&pv_done[0], j & 1);
-                    load_kv(j + 1);
-                }
-            }
-            umma_commit(o_full);
-        }
-    } else {
-        // ------------------------------ softmax: thread == query row ------------------------------
-        const int row = warp * 32 + lane;
-        const int qrow = qt * 128 + row;
-        const uint32_t lb = lane_base(warp);
-        float m = -INFINITY, l = 0.f;
-        const float* bias = p.kv_bias ? p.kv_bias + (int64_t)b * p.Lkv : nullptr;
-        for (int j = 0; j < nkv; ++j) {
-            const int kv0 = j * 128;
-            const int ncols = min(128, p.Lkv - kv0);
-            const int nch = (((ncols + 15) & ~15) + 31) >> 5;
-            mbar_wait(s_full, j & 1);
-            tc_fence_after();
-            // pass 1: row max (log2 domain)
-            float mx = -INFINITY;
-            for (int c = 0; c < nch; ++c) {
-                uint32_t v[32];
-                tmem_ld32(tS + lb + c * 32, v);
-                tmem_wait_ld();
-#pragma unroll
-                for (int e = 0; e < 32; ++e) {
-                    const int col = c * 32 + e;
-                    float s = __uint_as_float(v[e]) * p.scale_log2;
-                    if (bias && col < ncols) s += bias[kv0 + col] * kLog2e;
-                    s = (col < ncols) ? s : -INFINITY;
-                    mx = fmaxf(mx, s);
-                }
-            }
-            if (j == 0) {
-                m = (mx == -INFINITY) ? 0.f : mx;
-            } else {
-                const float m_new = fmaxf(m, mx);
-                if (__any_sync(0xffffffffu, m_new - m > 8.f)) {
-                    const float alpha = fast_exp2(m - m_new);
-                    l *= alpha;
-                    for (int c = 0; c < p.dn / 16; ++c) {
-                        uint32_t o[16];
-                        tmem_ld16(tO + lb + c * 16, o);
-                        tmem_wait_ld();
-#pragma unroll
-                        for (int e = 0; e < 16; ++e) o[e] = __float_as_uint(__uint_as_float(o[e]) * alpha);
-                        tmem_st16(tO + lb + c * 16, o);
-                    }
-                    tmem_wait_st();
-                    m = m_new;
-                }
-            }
-            // pass 2: P = exp2(s - m), packed bf16 back into TMEM (aliases the S columns already consumed)
-            for (int c = 0; c < nch; ++c) {
-                uint32_t v[32];
-                tmem_ld32(tS + lb + c * 32, v);
-                tmem_wait_ld();
-                uint32_t pk[16];
-#pragma unroll
-                for (int e = 0; e < 32; e += 2) {
-                    float pe[2];
-#pragma unroll
-                    for (int t = 0; t < 2; ++t) {
-                        const int col = c * 32 + e + t;
-                        float s = __uint_as_float(v[e + t]) * p.scale_log2;
-                        if (bias && col < ncols) s += bias[kv0 + col] * kLog2e;
-                        const float pv = fast_exp2(s - m);
-                        pe[t] = (col < ncols) ? pv : 0.f;
-                    }
-                    // accumulate the row sum from the bf16-rounded values the MMA will actually see
-                    const uint32_t u = pack_bf16x2(pe[0], pe[1]);
-                    const float2 r = unpack_bf16x2(u);
-                    l += r.x + r.y;
-                    pk[e >> 1] = u;
-                }
-                tmem_st16(tS + lb + c * 16, pk);
-            }
-            tmem_wait_st();
-            tc_fence_before();
-            mbar_arrive(p_ready);
-        }
-        mbar_wait(o_full, 0);
-        tc_fence_after();
-        const float inv = 1.f / l;
-        __nv_bfloat16* orow = p.O + ((int64_t)b * p.Lq + qrow) * p.ldo + (int64_t)h * p.d;
-        for (int c = 0; c < p.dn / 16; ++c) {
-            uint32_t o[16];
-            tmem_ld16(tO + lb + c * 16, o);
-            tmem_wait_ld();
-            if (qrow < p.Lq) {
-#pragma unroll
-                for (int g = 0; g < 2; ++g) {
-                    const int col = c * 16 + g * 8;
-                    if (col < p.d) {
-                        uint4 w;
-                        w.x = pack_bf16x2(__uint_as_float(o[g * 8 + 0]) * inv, __uint_as_float(o[g * 8 + 1]) * inv);
-                        w.y = pack_bf16x2(__uint_as_float(o[g * 8 + 2]) * inv, __uint_as_float(o[g * 8 + 3]) * inv);
-                        w.z = pack_bf16x2(__uint_as_float(o[g * 8 + 4]) * inv, __uint_as_float(o[g * 8 + 5]) * inv);
-                        w.w = pack_bf16x2(__uint_as_float(o[g * 8 + 6]) * inv, __uint_as_float(o[g * 8 + 7]) * inv);
-                        *reinterpret_cast<uint4*>(orow + col) = w;
-                    }
-                }
-            }
-        }
-        if (qrow < p.Lq && p.lse) p.lse[((int64_t)b * p.H + h) * p.Lq + qrow] = (m + log2f(l)) * kLn2;
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 4) tmem_dealloc(tmem, p.tmem_cols);
-}
-
-// ---- MMA issue helpers for the single issuing threads -------------------------------------------------------------------------
-// A thread that issues tcgen05.mma runs a chain of dependent uniform-datapath instructions at ~0.15 IPC (ncu: 596 instructions
-// per kv step in the first forward kernel = the whole step time), so its instruction count IS the critical path.  Descriptors are
-// built once and advanced on the low word only (the 14-bit start-address field never carries out for shared-memory addresses),
-// and the k-loops are fully unrolled for the head sizes of the UNets (d 40 / 64 / 80 / 160 -> 3 / 4 / 5 / 10 steps of 16).
-__device__ __forceinline__ uint64_t desc_adv(uint64_t d, uint32_t off16) {
-    return (d & 0xffffffff00000000ull) | (uint64_t)((uint32_t)d + off16);
-}
-// offset (in 16-byte units) of k-step ks inside a K-major operand tile made of 64-column SWIZZLE_128B boxes
-__device__ __forceinline__ constexpr uint32_t kmajor_off(int ks) { return (uint32_t)((ks >> 2) * (TILE_BYTES >> 4) + (ks & 3) * 2); }
-template <int N>
-__device__ __forceinline__ void umma_ss_kmajor(uint32_t tacc, uint64_t a, uint64_t b, uint32_t idesc) {
-#pragma unroll
-    for (int ks = 0; ks < N; ++ks) umma_ss(tacc, desc_adv(a, kmajor_off(ks)), desc_adv(b, kmajor_off(ks)), idesc, ks > 0 ? 1u : 0u);
-}
-__device__ __forceinline__ void umma_ss_kmajor_n(int nks, uint32_t tacc, uint64_t a, uint64_t b, uint32_t idesc) {
-    switch (nks) {
-        case 3: umma_ss_kmajor<3>(tacc, a, b, idesc); break;
-        case 4: umma_ss_kmajor<4>(tacc, a, b, idesc); break;
-        case 5: umma_ss_kmajor<5>(tacc, a, b, idesc); break;
-        case 10: umma_ss_kmajor<10>(tacc, a, b, idesc); break;
-        default:
-#pragma unroll 1
-            for (int ks = 0; ks < nks; ++ks)
-                umma_ss(tacc, desc_adv(a, kmajor_off(ks)), desc_adv(b, kmajor_off(ks)), idesc, ks > 0 ? 1u : 0u);
-    }
-}
-
-// =============================================================================================
-// forward, version 2: two 128-row query tiles per CTA (they share every K/V tile that TMA brings in), 16 softmax warps
-// (per query tile: 4 TMEM lane quarters x 2 column halves) and one control warp that ping-pongs the tensor pipe between the
-// two tiles: while the softmax warps of tile A exponentiate tile j, the pipe runs S_B(j), PV_B(j-1)...  Each softmax thread
-// reads its 64 logits from TMEM ONCE, the row maximum of the two column halves is combined through shared memory.
-// Warp 16 is the TMA producer (Q once, K/V stages), warps 17 and 18 each issue the MMAs of one query tile: three short
-// instruction streams instead of one long one (the single control thread of the first version was busy 90 % of the time and the
-// softmax warps spent a third of theirs waiting for logits it had not issued yet).
-// =============================================================================================
-constexpr int kFwd2Threads = 19 * 32;
-
-struct alignas(64) AttnFwd2Params {
-    CUtensorMap tmQ, tmK, tmV;
-    int B, H, Lq, Lkv, d;
-    int nbox, dn;
-    int nq;              // query tiles per CTA: 2 (d <= 128) or 1
-    int kv_stages;
-    float scale_log2;
-    const float* kv_bias;
-    __nv_bfloat16* O;
-    int64_t ldo;
-    float* lse;
+// NB = 64-column boxes per head row (ceil(d / 64)), KVT = kv rows per tile.  Per thread: KVT / 2 S registers + 32 NB O registers.
+template <int NB, int KVT>
+struct AttnFwdCfg {
+    static constexpr int Q_BYTES = NB * BOX_BYTES;
+    static constexpr int KV_BOX = KVT * 128;
+    static constexpr int KV_BYTES = NB * KV_BOX;          // one K (or V) tile
+    static constexpr int STAGES = 2;
+    static constexpr int SMEM_BYTES = Q_BYTES + 2 * STAGES * KV_BYTES + 256 + 1024;
 };
 
-__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
-    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
-
-__global__ void __launch_bounds__(kFwd2Threads, 1) attn_fwd2_kernel(const __grid_constant__ AttnFwd2Params p) {
+template <int NB, int KVT>
+__global__ void __launch_bounds__(kAttnThreads, 1) attn_fwd_kernel(const __grid_constant__ AttnFwdParams p) {
+    using Cfg = AttnFwdCfg<NB, KVT>;
+    constexpr int STAGES = Cfg::STAGES;
+    constexpr int DN = 64 * NB;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    const int tile_bytes = p.nbox * TILE_BYTES;
-    uint8_t* sQ = smem;                                  // [nq]
-    uint8_t* sK = sQ + p.nq * tile_bytes;                // [kv_stages]
-    uint8_t* sV = sK + p.kv_stages * tile_bytes;         // [kv_stages]
-    float* sx = reinterpret_cast<float*>(sV + p.kv_stages * tile_bytes);   // [2 parity][2 tile][2 half][128] row-max exchange
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sx + 2 * 2 * 2 * 128);
-    uint64_t* q_full = bars + 0;
-    uint64_t* kv_full = bars + 1;     // [3]
-    uint64_t* kv_done = bars + 4;     // [3]
-    uint64_t* s_full = bars + 7;      // [2]
-    uint64_t* p_ready = bars + 9;     // [2]
-    uint64_t* o_full = bars + 11;
-    uint64_t* s_free = bars + 12;     // [2] every softmax thread of the tile holds its logits in registers
-    uint64_t* pv_done = bars + 14;    // [2] PV of the previous kv tile has retired (P / O may be touched again)
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 16);
+    uint8_t* sQ = smem;
+    uint8_t* sK = sQ + Cfg::Q_BYTES;                     // [STAGES]
+    uint8_t* sV = sK + STAGES * Cfg::KV_BYTES;           // [STAGES]
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sV + STAGES * Cfg::KV_BYTES);
+    uint64_t* q_full = bars;
+    uint64_t* kv_full = bars + 1;                        // [STAGES]
+    uint64_t* kv_empty = bars + 1 + STAGES;              // [STAGES]
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int h = blockIdx.y, b = blockIdx.z;
-    const int q0 = blockIdx.x * p.nq * 128;
-    const int nkv = (p.Lkv + 127) / 128;
-    const int S = p.kv_stages;
+    const int warp = warp_id_uniform(), lane = threadIdx.x & 31;
+    const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+    const int nkv = (p.Lkv + KVT - 1) / KVT;
 
     if (threadIdx.x == 0) {
         mbar_init(q_full, 1);
-        for (int i = 0; i < 3; ++i) { mbar_init(&kv_full[i], 1); mbar_init(&kv_done[i], p.nq); }   // one commit per MMA warp
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&s_full[i], 1); mbar_init(&p_ready[i], 256);
-            mbar_init(&s_free[i], 256); mbar_init(&pv_done[i], 1);
-        }
-        mbar_init(o_full, p.nq);
+        for (int s = 0; s < STAGES; ++s) { mbar_init(&kv_full[s], 1); mbar_init(&kv_empty[s], 256); }
         fence_mbar_init();
     }
-    if (warp == 16) {
-        tmem_alloc(tmem_slot, 512);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
     pdl_trigger();
     pdl_wait();
-    // TMEM columns of query tile t: S fp32 [t*256, +128), P bf16 (packed) [t*256+128, +64), O fp32 [t*256+192, +dn).
-    // P has its own columns, so S of the NEXT kv tile can be issued as soon as the softmax warps hold the current logits in
-    // registers: QK^T(j+1) runs on the tensor pipe while the exponentials of tile j are computed.
 
-    if (warp == 16) {
-        // ------------------------------ TMA producer ------------------------------
+    if (warp == 8) {
         if (elect_one()) {
-            mbar_arrive_expect_tx(q_full, p.nq * tile_bytes);
-            for (int t = 0; t < p.nq; ++t)
-                for (int bx = 0; bx < p.nbox; ++bx)
-                    tma_load_4d(sQ + t * tile_bytes + bx * TILE_BYTES, &p.tmQ, q_full, bx * 64, h, q0 + t * 128, b);
-            int st = 0, round = 0;                                       // stage / use count of the stage for kv tile j
+            mbar_arrive_expect_tx(q_full, Cfg::Q_BYTES);
+            for (int bx = 0; bx < NB; ++bx) tma_load_4d(sQ + bx * BOX_BYTES, &p.tmQ, q_full, bx * 64, h, qt * 128, b);
             for (int j = 0; j < nkv; ++j) {
-                if (round > 0) mbar_wait(&kv_done[st], (round - 1) & 1);  // both query tiles have retired P V of the tile that was here
-                mbar_arrive_expect_tx(&kv_full[st], 2 * tile_bytes);
-                for (int bx = 0; bx < p.nbox; ++bx) {
-                    tma_load_4d(sK + st * tile_bytes + bx * TILE_BYTES, &p.tmK, &kv_full[st], bx * 64, h, j * 128, b);
-                    tma_load_4d(sV + st * tile_bytes + bx * TILE_BYTES, &p.tmV, &kv_full[st], bx * 64, h, j * 128, b);
-                }
-                if (++st == S) { st = 0; ++round; }
-            }
-        }
-    } else if (warp >= 17) {
-        // ------------------------------ MMA issue, one warp per query tile ------------------------------
-        const int t = warp - 17;
-        if (t < p.nq && elect_one()) {
-            const int nks = p.dn / 16;
-            const uint32_t idesc_pv = make_idesc_bf16(128, p.dn, 0, 1);
-            const uint32_t idesc_s_full = make_idesc_bf16(128, 128, 0, 0);
-            const int ncols_last = p.Lkv - (nkv - 1) * 128;
-            const uint32_t idesc_s_last = make_idesc_bf16(128, (ncols_last + 15) & ~15, 0, 0);
-            const int nst_last = (ncols_last + 15) >> 4;
-            const uint64_t qd = make_smem_desc(smem_u32(sQ + t * tile_bytes), 16, 1024);
-            const uint64_t kd0 = make_smem_desc(smem_u32(sK), 16, 1024);
-            const uint64_t vd0 = make_smem_desc(smem_u32(sV), TILE_BYTES, 1024);
-            const uint32_t stage16 = (uint32_t)tile_bytes >> 4;
-            const uint32_t ts = tmem + t * 256, tp = ts + 128, to = ts + 192;
-            auto issue_s = [&](int j, int st) {        // S_t = Q_t K_j^T
-                umma_ss_kmajor_n(nks, ts, qd, desc_adv(kd0, st * stage16), j == nkv - 1 ? idesc_s_last : idesc_s_full);
-                umma_commit(&s_full[t]);
-            };
-            auto issue_pv = [&](int j, int st) {       // O_t += P_t V_j  (P from TMEM, V MN-major: 2048 B per k-step)
-                const uint64_t vd = desc_adv(vd0, st * stage16);
-                if (j < nkv - 1 || nst_last == 8) {
-#pragma unroll
-                    for (int ks = 0; ks < 8; ++ks)
-                        umma_ts(to, tp + ks * 8, desc_adv(vd, ks * 128), idesc_pv, (j > 0 || ks > 0) ? 1u : 0u);
-                } else {
-#pragma unroll 1
-                    for (int ks = 0; ks < nst_last; ++ks)
-                        umma_ts(to, tp + ks * 8, desc_adv(vd, ks * 128), idesc_pv, (j > 0 || ks > 0) ? 1u : 0u);
-                }
-                umma_commit(&pv_done[t]);
-                umma_commit(&kv_done[st]);             // K_j / V_j are free once both tiles' commits have arrived
-            };
-            mbar_wait(q_full, 0);
-            mbar_wait(&kv_full[0], 0);
-            // The two query tiles are started half an iteration apart: tile 1 gets its first logits only when tile 0 has pulled
-            // its own into registers and enters the exponential phase.  Each tile's chain (logits -> max -> exp -> P) is strictly
-            // sequential, so the offset persists and the MUFU pipe serves one tile's exponentials while the other tile loads /
-            // reduces / stores (ncu, in-phase start: XU pipe 49 % busy, both tiles contending in the same window).
-            if (t == 1) mbar_wait(&s_free[0], 0);
-            tc_fence_after();
-            issue_s(0, 0);
-            int st = 0, round = 0;
-            for (int j = 0; j < nkv; ++j) {
-                int st1 = st + 1, round1 = round;
-                if (st1 == S) { st1 = 0; ++round1; }
-                if (S > 1 && j + 1 < nkv) {                             // next K tile is resident: issue S(j+1) early
-                    mbar_wait(&kv_full[st1], round1 & 1);
-                    mbar_wait(&s_free[t], j & 1);                       // logits of tile j are in registers
-                    tc_fence_after();
-                    issue_s(j + 1, st1);
-                }
-                mbar_wait(&p_ready[t], j & 1);
-                tc_fence_after();
-                issue_pv(j, st);
-                if (S == 1 && j + 1 < nkv) {                            // single stage (d > 128): the producer reloads, then issue
-                    mbar_wait(&kv_full[0], (j + 1) & 1);
-                    tc_fence_after();
-                    issue_s(j + 1, 0);
-                }
-                st = st1; round = round1;
-            }
-            umma_commit(o_full);
-        }
-    } else if ((warp >> 3) < p.nq) {
-        // ------------------------------ softmax: thread == (query row, 64-column half) ------------------------------
-        const int t = warp >> 3, quarter = warp & 3, half = (warp >> 2) & 1;
-        const int row = quarter * 32 + lane;
-        const int qrow = q0 + t * 128 + row;
-        const uint32_t lb = lane_base(quarter);
-        const uint32_t tS = tmem + t * 256, tP = tS + 128, tO = tS + 192;
-        const float* bias = p.kv_bias ? p.kv_bias + (int64_t)b * p.Lkv : nullptr;
-        float m = -INFINITY, l = 0.f;
-        for (int j = 0; j < nkv; ++j) {
-            const int kv0 = j * 128;
-            const int ncols = min(128, p.Lkv - kv0);
-            const int c0 = half * 64;
-            const bool special = (ncols < 128) || (bias != nullptr);
-            mbar_wait(&s_full[t], j & 1);
-            tc_fence_after();
-            uint32_t v0[32], v1[32];
-            tmem_ld32(tS + lb + c0, v0);
-            tmem_ld32(tS + lb + c0 + 32, v1);
-            tmem_wait_ld();
-            float sc = p.scale_log2;
-            if (bias) {                    // additive key bias: move to the scaled domain in place, then sc = 1
-#pragma unroll
-                for (int e = 0; e < 32; ++e) {
-                    float a = __uint_as_float(v0[e]) * p.scale_log2, c = __uint_as_float(v1[e]) * p.scale_log2;
-                    const int ca = c0 + e, cb = c0 + 32 + e;
-                    if (ca < ncols) a += __ldg(bias + kv0 + ca) * kLog2e;
-                    if (cb < ncols) c += __ldg(bias + kv0 + cb) * kLog2e;
-                    v0[e] = __float_as_uint(ca < ncols ? a : -INFINITY);
-                    v1[e] = __float_as_uint(cb < ncols ? c : -INFINITY);
-                    if ((e & 7) == 7) asm volatile("" ::: "memory");   // keep at most 16 bias loads in flight (register pressure)
-                }
-                sc = 1.f;
-            } else if (special) {          // ragged last tile: columns past Lkv become -inf (the positive scale keeps them there)
-#pragma unroll
-                for (int e = 0; e < 32; ++e) {
-                    if (c0 + e >= ncols) v0[e] = 0xff800000u;
-                    if (c0 + 32 + e >= ncols) v1[e] = 0xff800000u;
-                }
-            }
-            float mx = fmaxf(__uint_as_float(v0[0]), __uint_as_float(v1[0]));
-#pragma unroll
-            for (int e = 1; e < 32; ++e) mx = fmaxf(mx, fmaxf(__uint_as_float(v0[e]), __uint_as_float(v1[e])));
-            mx *= sc;                      // the scale is positive: max commutes with it
-            float* xch = sx + (((j & 1) * 2 + t) * 2) * 128;
-            xch[half * 128 + row] = mx;
-            named_bar_sync(1 + t, 256);
-            mbar_arrive(&s_free[t]);                 // S columns may be overwritten by QK^T of the next kv tile
-            mx = fmaxf(mx, xch[(half ^ 1) * 128 + row]);
-            if (j == 0) {
-                m = (mx == -INFINITY) ? 0.f : mx;
-            } else {
-                const float m_new = fmaxf(m, mx);
-                if (__any_sync(0xffffffffu, m_new - m > 8.f)) {
-                    const float alpha = fast_exp2(m - m_new);
-                    l *= alpha;
-                    if (half == 0) {
-                        mbar_wait(&pv_done[t], (j - 1) & 1);      // O is stable: PV of the previous tile retired
-                        tc_fence_after();
-                        for (int c = 0; c < p.dn / 16; ++c) {
-                            uint32_t o[16];
-                            tmem_ld16(tO + lb + c * 16, o);
-                            tmem_wait_ld();
-#pragma unroll
-                            for (int e = 0; e < 16; ++e) o[e] = __float_as_uint(__uint_as_float(o[e]) * alpha);
-                            tmem_st16(tO + lb + c * 16, o);
-                        }
-                    }
-                    m = m_new;
-                }
-            }
-            const float negm = -m;
-            uint32_t pk[32];
-            float l0 = 0.f, l1 = 0.f;
-#pragma unroll
-            for (int e = 0; e < 32; e += 2) {
-                const float p0 = fast_exp2(fmaf(__uint_as_float(v0[e]), sc, negm));
-                const float p1 = fast_exp2(fmaf(__uint_as_float(v0[e + 1]), sc, negm));
-                const float p2 = fast_exp2(fmaf(__uint_as_float(v1[e]), sc, negm));
-                const float p3 = fast_exp2(fmaf(__uint_as_float(v1[e + 1]), sc, negm));
-                l0 += p0 + p1;
-                l1 += p2 + p3;
-                pk[e >> 1] = pack_bf16x2(p0, p1);
-                pk[16 + (e >> 1)] = pack_bf16x2(p2, p3);
-            }
-            l += l0 + l1;
-            if (j > 0) {
-                mbar_wait(&pv_done[t], (j - 1) & 1);  // the tensor pipe has finished reading the previous P
-                tc_fence_after();
-            }
-            tmem_st32(tP + lb + half * 32, pk);       // P (bf16, packed pairs) into its own TMEM columns
-            tmem_wait_st();
-            tc_fence_before();
-            mbar_arrive(&p_ready[t]);
-        }
-        // combine the two halves' row sums, then each half writes its share of the output columns
-        float* xch = sx + ((0 * 2 + t) * 2) * 128;
-        named_bar_sync(1 + t, 256);
-        xch[half * 128 + row] = l;
-        named_bar_sync(1 + t, 256);
-        l += xch[(half ^ 1) * 128 + row];
-        mbar_wait(o_full, 0);
-        tc_fence_after();
-        const float inv = 1.f / l;
-        __nv_bfloat16* orow = p.O + ((int64_t)b * p.Lq + qrow) * p.ldo + (int64_t)h * p.d;
-        for (int c = half; c < p.dn / 16; c += 2) {
-            uint32_t o[16];
-            tmem_ld16(tO + lb + c * 16, o);
-            tmem_wait_ld();
-            if (qrow < p.Lq) {
-#pragma unroll
-                for (int g = 0; g < 2; ++g) {
-                    const int col = c * 16 + g * 8;
-                    if (col < p.d) {
-                        uint4 w;
-                        w.x = pack_bf16x2(__uint_as_float(o[g * 8 + 0]) * inv, __uint_as_float(o[g * 8 + 1]) * inv);
-                        w.y = pack_bf16x2(__uint_as_float(o[g * 8 + 2]) * inv, __uint_as_float(o[g * 8 + 3]) * inv);
-                        w.z = pack_bf16x2(__uint_as_float(o[g * 8 + 4]) * inv, __uint_as_float(o[g * 8 + 5]) * inv);
-                        w.w = pack_bf16x2(__uint_as_float(o[g * 8 + 6]) * inv, __uint_as_float(o[g * 8 + 7]) * inv);
-                        *reinterpret_cast<uint4*>(orow + col) = w;
-                    }
+                const int st = j % STAGES;
+                mbar_wait(&kv_empty[st], ((j / STAGES) & 1) ^ 1);
+                mbar_arrive_expect_tx(&kv_full[st], 2 * Cfg::KV_BYTES);
+                for (int bx = 0; bx < NB; ++bx) {
+                    tma_load_4d(sK + st * Cfg::KV_BYTES + bx * Cfg::KV_BOX, &p.tmK, &kv_full[st], bx * 64, h, j * KVT, b);
+                    tma_load_4d(sV + st * Cfg::KV_BYTES + bx * Cfg::KV_BOX, &p.tmV, &kv_full[st], bx * 64, h, j * KVT, b);
                 }
             }
         }
-        if (half == 0 && qrow < p.Lq && p.lse) p.lse[((int64_t)b * p.H + h) * p.Lq + qrow] = (m + log2f(l)) * kLn2;
+        return;
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 16) tmem_dealloc(tmem, 512);
+
+    // ------------------------------ MMA warpgroups: rows of a quad's thread are g and g + 8 ------------------------------
+    const int wg = warp >> 2;
+    const int g = lane >> 2, cq = 2 * (lane & 3);
+    const int row0 = wg * 64 + (warp & 3) * 16 + g;      // tile rows row0 and row0 + 8
+    const float* bias = p.kv_bias ? p.kv_bias + (int64_t)b * p.Lkv : nullptr;
+    const float sl2 = p.scale_log2;
+    float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+    float o[DN / 2];
+#pragma unroll
+    for (int i = 0; i < DN / 2; ++i) o[i] = 0.f;
+    const uint64_t qdesc = make_smem_desc(smem_u32(sQ) + wg * 64 * 128, 16, 1024);
+    mbar_wait(q_full, 0);
+    for (int j = 0; j < nkv; ++j) {
+        const int st = j % STAGES;
+        const int kv0 = j * KVT;
+        const int ncols = min(KVT, p.Lkv - kv0);
+        mbar_wait(&kv_full[st], (j / STAGES) & 1);
+        // ---- S = Q K^T
+        float s[KVT / 2];
+        const uint64_t kdesc = make_smem_desc(smem_u32(sK + st * Cfg::KV_BYTES), 16, 1024);
+        wgmma_fence();
+        wgmma_ss<KVT, 0, 0>(s, qdesc, kdesc, 0u);
+        for (int ks = 1; ks < p.nks; ++ks)
+            wgmma_ss<KVT, 0, 0>(s, desc_adv(qdesc, kmajor_off(ks, BOX_BYTES)), desc_adv(kdesc, kmajor_off(ks, Cfg::KV_BOX)), 1u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_acc(s);
+        // ---- online softmax (log2 domain)
+        float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+        for (int c8 = 0; c8 < KVT / 8; ++c8) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int col = c8 * 8 + cq + e;
+                const float bv = (bias && col < ncols) ? bias[kv0 + col] * kLog2e : 0.f;
+#pragma unroll
+                for (int hh = 0; hh < 2; ++hh) {
+                    float v = s[4 * c8 + 2 * hh + e] * sl2 + bv;
+                    v = (col < ncols) ? v : -INFINITY;
+                    s[4 * c8 + 2 * hh + e] = v;
+                    mx[hh] = fmaxf(mx[hh], v);
+                }
+            }
+        }
+        float mu[2];
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+            const float m_new = fmaxf(m[hh], quad_max(mx[hh]));
+            mu[hh] = (m_new == -INFINITY) ? 0.f : m_new;             // a row with no finite score so far: P = 0, nothing to rescale
+            const float alpha = fast_exp2(m[hh] - mu[hh]);           // exp2(-inf) = 0 on the first tile
+            l[hh] *= alpha;
+#pragma unroll
+            for (int c8 = 0; c8 < DN / 8; ++c8) { o[4 * c8 + 2 * hh] *= alpha; o[4 * c8 + 2 * hh + 1] *= alpha; }
+            m[hh] = m_new;
+        }
+        // ---- P = exp2(s - m) as bf16 A fragments; the row sums use the bf16-rounded values the MMA sees
+        uint32_t pa[KVT / 16][4];
+#pragma unroll
+        for (int kk = 0; kk < KVT / 16; ++kk) {
+#pragma unroll
+            for (int r = 0; r < 4; ++r) {
+                const int hh = r & 1;
+                const int i = 8 * kk + 4 * (r >> 1) + 2 * hh;
+                const uint32_t u = pack_bf16x2(fast_exp2(s[i] - mu[hh]), fast_exp2(s[i + 1] - mu[hh]));
+                const float2 f = unpack_bf16x2(u);
+                l[hh] += f.x + f.y;
+                pa[kk][r] = u;
+            }
+        }
+        // ---- O += P V   (V tile: MN-major B operand; LBO = distance between its 64-column boxes)
+        const uint64_t vdesc = make_smem_desc(smem_u32(sV + st * Cfg::KV_BYTES), Cfg::KV_BOX, 1024);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < KVT / 16; ++kk) wgmma_rs<DN, 1>(o, pa[kk], desc_adv(vdesc, kk * 128), 1u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_acc(o);
+        mbar_arrive(&kv_empty[st]);
+    }
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+        const float lt = quad_sum(l[hh]);
+        const int qrow = qt * 128 + row0 + 8 * hh;
+        if (qrow >= p.Lq) continue;
+        const float inv = 1.f / lt;
+        __nv_bfloat16* orow = p.O + ((int64_t)b * p.Lq + qrow) * p.ldo + (int64_t)h * p.d;
+#pragma unroll
+        for (int c8 = 0; c8 < DN / 8; ++c8) {
+            const int col = c8 * 8 + cq;
+            if (col < p.d) *reinterpret_cast<uint32_t*>(orow + col) = pack_bf16x2(o[4 * c8 + 2 * hh] * inv, o[4 * c8 + 2 * hh + 1] * inv);
+        }
+        if (cq == 0 && p.lse) p.lse[((int64_t)b * p.H + h) * p.Lq + qrow] = ((m[hh] == -INFINITY ? 0.f : m[hh]) + log2f(lt)) * kLn2;
+    }
 }
 
 // =============================================================================================
 // backward
 // =============================================================================================
 struct alignas(64) AttnBwdParams {
-    CUtensorMap tmQ, tmK, tmV, tmdO;
+    CUtensorMap tmQ, tmK, tmV, tmdO;   // K / V: boxes of 128 rows; Q / dO: boxes of 64 rows
     int B, H, Lq, Lkv, d;
-    int nbox, dn;
-    int col0, ncols_out;     // output column slice of this launch (col0 multiple of 64)
-    int q_stages;            // 1 or 2
-    int share_pds;           // P and dS share one smem buffer
+    int nks;                 // 16-wide k-steps over d
+    int col0;                // output column slice [col0, col0 + 64) of this launch
     float scale, scale_log2;
     const float* kv_bias;
     const float* lse;        // [B,H,Lq]
     const float* delta;      // [B,H,Lq]  rowsum(dO * O)
-    float* dq_acc;           // [B,H,dq_ld/4,Lq,4] fp32 (nullptr when dq_direct is set)
+    float* dq_acc;           // [B,H,dq_ld/4,Lq,4] fp32
     int dq_ld;
-    __nv_bfloat16* dq_direct; // single kv tile (Lkv <= 128): dQ_i is complete after one pass -> stored as bf16, no accumulator
-    int64_t lddq;
-    int early_sdp;           // 1: dQ un-aliased + double-buffered Q/dO -> S/dP of the next tile are issued early
     int qsplit;              // CTAs per kv tile along the query dimension
     float* dkv_acc;          // [B,H,Lkv,2,dq_ld] fp32 partial dK/dV when qsplit > 1, else nullptr
     __nv_bfloat16 *dK, *dV;
     int64_t lddk, lddv;
-    long long* trace;        // bring-up only (hcp_debug_attn_trace): cycle sums of the lean loop's phases, CTA 0 only
 };
 
-__global__ void __launch_bounds__(kAttnBwdThreads, 1) attn_bwd_kernel(const __grid_constant__ AttnBwdParams p) {
+template <int NB>
+struct AttnBwdCfg {
+    static constexpr int KV_BYTES = NB * BOX_BYTES;       // K or V: 128 rows
+    static constexpr int QBOX = 64 * 128;
+    static constexpr int Q_BYTES = NB * QBOX;             // Q or dO: 64 rows
+    static constexpr int STAGES = 2;
+    static constexpr int DS_BYTES = 64 * 128;             // dS^T of one warpgroup: [64 kv][64 q] bf16 (the two are contiguous)
+    static constexpr int SMEM_BYTES = 2 * KV_BYTES + 2 * STAGES * Q_BYTES + 2 * DS_BYTES + 256 + 1024;
+};
+
+template <int NB>
+__global__ void __launch_bounds__(kAttnThreads, 1) attn_bwd_kernel(const __grid_constant__ AttnBwdParams p) {
+    using Cfg = AttnBwdCfg<NB>;
+    constexpr int STAGES = Cfg::STAGES;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    const int tile_bytes = p.nbox * TILE_BYTES;
     uint8_t* sK = smem;
-    uint8_t* sV = sK + tile_bytes;
-    uint8_t* sQ = sV + tile_bytes;                       // q_stages
-    uint8_t* sdO = sQ + p.q_stages * tile_bytes;         // q_stages
-    uint8_t* sP = sdO + p.q_stages * tile_bytes;         // [128 q rows x 128 kv] bf16 = 2 boxes
-    uint8_t* sdS = p.share_pds ? sP : sP + 2 * TILE_BYTES;
-    uint64_t* bars = reinterpret_cast<uint64_t*>((p.share_pds ? sP : sdS) + 2 * TILE_BYTES);
-    uint64_t* kv_full = bars + 0;
-    uint64_t* q_full = bars + 1;     // [2]
-    uint64_t* sdp_full = bars + 3;   // S and dP ready in TMEM
-    uint64_t* p_ready = bars + 4;    // P in smem           (128 arrivals)
-    uint64_t* ds_ready = bars + 5;   // dS in smem          (128 arrivals)
-    uint64_t* dv_done = bars + 6;    // dV MMA retired (P buffer reusable)
-    uint64_t* dq_full = bars + 7;    // dK, dQ MMAs retired
-    uint64_t* dq_read = bars + 8;    // dQ drained from TMEM (128 arrivals)
-    uint64_t* acc_full = bars + 9;
-    uint64_t* sdp_free = bars + 10;  // every softmax thread holds its S / dP values of the tile in registers
-    uint64_t* q_full2 = bars + 11;   // third Q/dO stage (early_sdp)
-    uint64_t* dp_free = bars + 12;   // ... and its dP values (S and dP are released separately: 32 live registers each)
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 13);
+    uint8_t* sV = sK + Cfg::KV_BYTES;
+    uint8_t* sQ = sV + Cfg::KV_BYTES;                     // [STAGES]
+    uint8_t* sdO = sQ + STAGES * Cfg::Q_BYTES;            // [STAGES]
+    uint8_t* sDS = sdO + STAGES * Cfg::Q_BYTES;           // [2 warpgroups]
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sDS + 2 * Cfg::DS_BYTES);
+    uint64_t* kv_full = bars;
+    uint64_t* q_full = bars + 1;                          // [STAGES]
+    uint64_t* q_empty = bars + 1 + STAGES;                // [STAGES]
 
+    // Register-bound: 288 threads cap every thread at 168 registers, and S, dP, their bf16 fragments and the dV / dK / dQ accumulators
+    // do not fit; ptxas spills (~0.3 KB per thread) and serializes the wgmmas (C7512).  The thread-index form of the warp index below
+    // measured faster than warp_id_uniform() here (the latter spilled more).
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    // blockIdx.x = (kv tile, q split): short-KV problems (cross-attention) have a single kv tile, so the query range is split
-    // over CTAs and the dK/dV partials are reduced with fp32 atomics (dkv_acc) instead of being stored directly.
-    const int jt = blockIdx.x / p.qsplit, qs = blockIdx.x % p.qsplit, h = blockIdx.y, b = blockIdx.z;
-    const int nq_total = (p.Lq + 127) / 128;
-    const int nq_per = (nq_total + p.qsplit - 1) / p.qsplit;
-    const int i0 = qs * nq_per;                                   // first query tile of this CTA
-    const int nq = min(nq_total, i0 + nq_per) - i0;               // >= 1 by construction of qsplit
-    const int kv0 = jt * 128;
-    const int ncols = min(128, p.Lkv - kv0);
+    const int kt = blockIdx.x / p.qsplit, qs = blockIdx.x % p.qsplit;
+    const int h = blockIdx.y, b = blockIdx.z;
+    const int nq = (p.Lq + 63) / 64;
+    const int per = 2 * (((nq + 1) / 2 + p.qsplit - 1) / p.qsplit);     // whole 128-row units per split (plan_qsplit)
+    const int i0 = qs * per, i1 = min(nq, i0 + per);
 
     if (threadIdx.x == 0) {
         mbar_init(kv_full, 1);
-        mbar_init(&q_full[0], 1);
-        mbar_init(&q_full[1], 1);
-        mbar_init(sdp_full, 1);
-        mbar_init(p_ready, kBwdSoftmaxThreads);
-        mbar_init(ds_ready, kBwdSoftmaxThreads);
-        mbar_init(dv_done, 1);
-        mbar_init(dq_full, 1);
-        mbar_init(dq_read, kBwdSoftmaxThreads);
-        mbar_init(acc_full, 1);
-        mbar_init(sdp_free, kBwdSoftmaxThreads);
-        mbar_init(q_full2, 1);
-        mbar_init(dp_free, kBwdSoftmaxThreads);
+        for (int s = 0; s < STAGES; ++s) { mbar_init(&q_full[s], 1); mbar_init(&q_empty[s], 256); }
         fence_mbar_init();
     }
-    if (warp == 4 * kBwdParts) {
-        tmem_alloc(tmem_slot, 512);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
     pdl_trigger();
     pdl_wait();
-    // TMEM columns: S [0,128), dP [128,256), then the accumulators.  dQ aliases S unless `early_sdp` (it then has its own columns).
-    const uint32_t tS = tmem, tdP = tmem + 128;
-    const uint32_t tdV = tmem + 256;
-    const uint32_t tdK = p.early_sdp ? tmem + 256 + p.ncols_out : tmem + 384;
-    const uint32_t tdQ = p.early_sdp ? tmem + 256 + 2 * p.ncols_out : tmem;
 
-    if (warp >= 4 * kBwdParts) {
-        // role 0: TMA prologue + S / dP issue (and the whole schedule when !early_sdp); role 1: dV / dK / dQ issue; role 2: Q/dO
-        // refills.  Three short instruction streams: one thread issuing all ~30 MMAs and the TMA of an iteration was busy 70 %
-        // of the time (ncu) and sat on the critical path (see the forward kernel).
-        const int role = warp - 4 * kBwdParts;
-        if ((role == 0 || p.early_sdp) && elect_one()) {
-            auto qbar = [&](int st) { return st == 2 ? q_full2 : &q_full[st]; };
-            auto load_q = [&](int i) {
-                const int st = i % p.q_stages;
-                mbar_arrive_expect_tx(qbar(st), 2 * tile_bytes);
-                for (int bx = 0; bx < p.nbox; ++bx) {
-                    tma_load_4d(sQ + st * tile_bytes + bx * TILE_BYTES, &p.tmQ, qbar(st), bx * 64, h, (i0 + i) * 128, b);
-                    tma_load_4d(sdO + st * tile_bytes + bx * TILE_BYTES, &p.tmdO, qbar(st), bx * 64, h, (i0 + i) * 128, b);
-                }
-            };
-            if (role == 0) {
-                mbar_arrive_expect_tx(kv_full, 2 * tile_bytes);
-                for (int bx = 0; bx < p.nbox; ++bx) {
-                    tma_load_4d(sK + bx * TILE_BYTES, &p.tmK, kv_full, bx * 64, h, kv0, b);
-                    tma_load_4d(sV + bx * TILE_BYTES, &p.tmV, kv_full, bx * 64, h, kv0, b);
-                }
-                load_q(0);
-                if (p.early_sdp) {
-                    if (nq > 1) load_q(1);
-                    if (nq > 2) load_q(2);
-                }
+    if (warp == 8) {
+        if (elect_one()) {
+            mbar_arrive_expect_tx(kv_full, 2 * Cfg::KV_BYTES);
+            for (int bx = 0; bx < NB; ++bx) {
+                tma_load_4d(sK + bx * BOX_BYTES, &p.tmK, kv_full, bx * 64, h, kt * 128, b);
+                tma_load_4d(sV + bx * BOX_BYTES, &p.tmV, kv_full, bx * 64, h, kt * 128, b);
             }
-            mbar_wait(kv_full, 0);
-            const uint32_t idesc_s = make_idesc_bf16(128, 128, 0, 0);
-            const uint32_t idesc_acc = make_idesc_bf16(128, p.ncols_out, 1, 1);   // dV, dK: A and B MN-major
-            const uint32_t idesc_dq = make_idesc_bf16(128, p.ncols_out, 0, 1);    // dQ: A K-major, B MN-major
-            const uint32_t box0 = (p.col0 / 64) * TILE_BYTES;                     // first box of the output slice
-            const uint32_t kb = smem_u32(sK), vb = smem_u32(sV);
-            const uint32_t pb = smem_u32(sP), dsb = smem_u32(sdS);
-            // The issuing thread is ONE thread: descriptor bases are built once and advanced by constants (see umma_ss_kmajor_n).
-            const int nks = p.dn / 16;                                   // k-steps of the d contraction (<= 12)
-            const uint64_t kdesc_k = make_smem_desc(kb, 16, 1024);           // K as K-major operand (S = Q K^T)
-            const uint64_t vdesc_k = make_smem_desc(vb, 16, 1024);           // V as K-major operand (dP = dO V^T)
-            const uint64_t pdesc_mn = make_smem_desc(pb, TILE_BYTES, 1024);  // P^T  (MN-major A of dV)
-            const uint64_t dsdesc_mn = make_smem_desc(dsb, TILE_BYTES, 1024);// dS^T (MN-major A of dK)
-            const uint64_t dsdesc_k = make_smem_desc(dsb, 16, 1024);         // dS   (K-major A of dQ)
-            const uint64_t kdesc_mn = make_smem_desc(kb + box0, TILE_BYTES, 1024);   // K (MN-major B of dQ)
-            auto issue_s = [&](int st) {            // S = Q K^T  (contraction over d)
-                umma_ss_kmajor_n(nks, tS, make_smem_desc(smem_u32(sQ + st * tile_bytes), 16, 1024), kdesc_k, idesc_s);
-            };
-            auto issue_dp = [&](int st) {           // dP = dO V^T, then signal "S and dP ready"
-                umma_ss_kmajor_n(nks, tdP, make_smem_desc(smem_u32(sdO + st * tile_bytes), 16, 1024), vdesc_k, idesc_s);
-                umma_commit(sdp_full);
-            };
-            auto issue_sdp = [&](int st) { issue_s(st); issue_dp(st); };
-            auto issue_dv = [&](int st, bool acc) {  // dV += P^T dO   (M = kv, K = q rows: both operands MN-major, 2048 B per k-step)
-                const uint64_t dod = make_smem_desc(smem_u32(sdO + st * tile_bytes) + box0, TILE_BYTES, 1024);
-#pragma unroll
-                for (int ks = 0; ks < 8; ++ks)
-                    umma_ss(tdV, desc_adv(pdesc_mn, ks * 128), desc_adv(dod, ks * 128), idesc_acc, (acc || ks > 0) ? 1u : 0u);
-                umma_commit(dv_done);
-            };
-            auto issue_dk = [&](int st, bool acc) {  // dK += dS^T Q
-                const uint64_t qd = make_smem_desc(smem_u32(sQ + st * tile_bytes) + box0, TILE_BYTES, 1024);
-#pragma unroll
-                for (int ks = 0; ks < 8; ++ks)
-                    umma_ss(tdK, desc_adv(dsdesc_mn, ks * 128), desc_adv(qd, ks * 128), idesc_acc, (acc || ks > 0) ? 1u : 0u);
-            };
-            auto issue_dq = [&]() {                  // dQ_i = dS K: dS K-major (two 64-wide boxes), K_j MN-major
-#pragma unroll
-                for (int ks = 0; ks < 8; ++ks)
-                    umma_ss(tdQ, desc_adv(dsdesc_k, kmajor_off(ks)), desc_adv(kdesc_mn, ks * 128), idesc_dq, ks > 0 ? 1u : 0u);
-                umma_commit(dq_full);
-            };
-            if (p.early_sdp) {
-                // dQ has its own TMEM columns and Q/dO have three stages.  The softmax threads pull their S / dP values of tile i
-                // into registers first (sdp_free / dp_free), so S/dP of tile i+1 are issued while the exponentials of tile i are
-                // computed; dV_i, dK_i, dQ_i follow as their operands appear.  The tensor pipe and the softmax warps never wait
-                // for each other except for true data dependencies.
-                if (role == 0) {
-                    mbar_wait(&q_full[0], 0);
-                    tc_fence_after();
-                    issue_sdp(0);
-                    int st1 = 1, ph1 = 0;                        // stage / parity of tile i+1
-                    for (int i = 0; i + 1 < nq; ++i) {
-                        mbar_wait(sdp_free, i & 1);              // S_i is in registers: S_{i+1} may overwrite the columns
-                        mbar_wait(qbar(st1), ph1);
-                        tc_fence_after();
-                        issue_s(st1);
-                        mbar_wait(dp_free, i & 1);               // dP_i is in registers
-                        tc_fence_after();
-                        issue_dp(st1);
-                        if (++st1 == 3) { st1 = 0; ph1 ^= 1; }
-                    }
-                } else if (role == 1) {
-                    int st = 0, ph = 0;
-                    for (int i = 0; i < nq; ++i) {
-                        mbar_wait(qbar(st), ph);                 // (complete long ago: S_i came from this stage) smem visibility
-                        mbar_wait(p_ready, i & 1);
-                        tc_fence_after();
-                        issue_dv(st, i > 0);
-                        mbar_wait(ds_ready, i & 1);
-                        tc_fence_after();
-                        issue_dk(st, i > 0);
-                        if (i > 0) {
-                            mbar_wait(dq_read, (i - 1) & 1);     // dQ_{i-1} drained from TMEM
-                            tc_fence_after();
-                        }
-                        issue_dq();
-                        if (++st == 3) { st = 0; ph ^= 1; }
-                    }
-                    umma_commit(acc_full);
-                } else {
-                    for (int i = 0; i + 3 < nq; ++i) {
-                        mbar_wait(dq_full, i & 1);               // every MMA reading Q_i / dO_i has retired: the stage is free
-                        load_q(i + 3);
-                    }
+            for (int i = i0; i < i1; ++i) {
+                const int st = (i - i0) % STAGES;
+                mbar_wait(&q_empty[st], (((i - i0) / STAGES) & 1) ^ 1);
+                mbar_arrive_expect_tx(&q_full[st], 2 * Cfg::Q_BYTES);
+                for (int bx = 0; bx < NB; ++bx) {
+                    tma_load_4d(sQ + st * Cfg::Q_BYTES + bx * Cfg::QBOX, &p.tmQ, &q_full[st], bx * 64, h, i * 64, b);
+                    tma_load_4d(sdO + st * Cfg::Q_BYTES + bx * Cfg::QBOX, &p.tmdO, &q_full[st], bx * 64, h, i * 64, b);
                 }
-            } else {
-                for (int i = 0; i < nq; ++i) {
-                    const int st = (p.q_stages == 2) ? (i & 1) : 0;
-                    const uint32_t ph = (p.q_stages == 2) ? ((i >> 1) & 1) : (i & 1);
-                    if (p.q_stages == 2 && i + 1 < nq) load_q(i + 1);   // stage (i+1)&1 was released by dq_full of i-1
-                    mbar_wait(&q_full[st], ph);
-                    tc_fence_after();
-                    issue_sdp(st);
-                    mbar_wait(p_ready, i & 1);
-                    tc_fence_after();
-                    issue_dv(st, i > 0);
-                    mbar_wait(ds_ready, i & 1);
-                    tc_fence_after();
-                    issue_dk(st, i > 0);
-                    issue_dq();
-                    if (p.q_stages == 1 && i + 1 < nq) {
-                        mbar_wait(dq_full, i & 1);      // Q/dO tile consumed
-                        load_q(i + 1);
-                    }
-                    mbar_wait(dq_read, i & 1);          // S/dP/dQ columns free again
-                    tc_fence_after();
-                }
-                umma_commit(acc_full);
             }
         }
-    } else {
-        // ------------------------------ thread == query row (S, dP) / kv row (dK, dV) --------------
-        const int quarter = warp & 3, part = warp >> 2;      // lanes [32*quarter, +32), kv columns [128/kBwdParts * part, +...)
-        constexpr int kChunksPerPart = 4 / kBwdParts;        // 32-column TMEM chunks per warp
-        const int row = quarter * 32 + lane;
-        const uint32_t lb = lane_base(quarter);
-        const float* bias = p.kv_bias ? p.kv_bias + (int64_t)b * p.Lkv : nullptr;
-        const bool special = (bias != nullptr) || (ncols < 128);
-        const int64_t stat_base = ((int64_t)b * p.H + h) * p.Lq;
-        auto drain_dq = [&](int qr) {            // TMEM dQ tile -> fp32 accumulator (vector red.global), or straight to bf16 dQ
-            // fp32 accumulator layout [B, H, d/4, Lq, 4]: for a fixed 4-column group the 32 rows of a warp are 32 consecutive
-            // 16-byte slots, so one red.v4 instruction covers 16 full sectors instead of 32 half-used ones
-            float* dqcol = p.dq_direct ? nullptr
-                                       : p.dq_acc + ((((int64_t)b * p.H + h) * (p.dq_ld / 4) + p.col0 / 4) * p.Lq + qr) * 4;
-            __nv_bfloat16* drow = p.dq_direct ? p.dq_direct + ((int64_t)b * p.Lq + qr) * p.lddq + (int64_t)h * p.d + p.col0 : nullptr;
-            for (int c = part; c < p.ncols_out / 16; c += kBwdParts) {
-                uint32_t o[16];
-                tmem_ld16(tdQ + lb + c * 16, o);
-                tmem_wait_ld();
-                if (qr < p.Lq) {
-                    if (drow) {
+        return;
+    }
+
+    const int wg = warp >> 2;
+    const int g = lane >> 2, cq = 2 * (lane & 3);
+    const int r0 = (warp & 3) * 16 + g;                  // rows r0, r0 + 8 of this warpgroup's 64 kv rows
+    const int kvw = kt * 128 + wg * 64;
+    const int64_t bh = (int64_t)b * p.H + h;
+    const float sl2 = p.scale_log2, scale = p.scale;
+    const int cbox = p.col0 / 64;                        // box holding the output column slice
+    float kvb[2];
+    bool kv_ok[2];
 #pragma unroll
-                        for (int g = 0; g < 2; ++g) {
-                            const int col = p.col0 + c * 16 + g * 8;
-                            if (col < p.d) {
-                                uint4 w;
-                                w.x = pack_bf16x2(__uint_as_float(o[g * 8 + 0]), __uint_as_float(o[g * 8 + 1]));
-                                w.y = pack_bf16x2(__uint_as_float(o[g * 8 + 2]), __uint_as_float(o[g * 8 + 3]));
-                                w.z = pack_bf16x2(__uint_as_float(o[g * 8 + 4]), __uint_as_float(o[g * 8 + 5]));
-                                w.w = pack_bf16x2(__uint_as_float(o[g * 8 + 6]), __uint_as_float(o[g * 8 + 7]));
-                                *reinterpret_cast<uint4*>(drow + c * 16 + g * 8) = w;
-                            }
-                        }
-                    } else {
+    for (int hh = 0; hh < 2; ++hh) {
+        const int kv = kvw + r0 + 8 * hh;
+        kv_ok[hh] = kv < p.Lkv;
+        kvb[hh] = (p.kv_bias && kv_ok[hh]) ? p.kv_bias[(int64_t)b * p.Lkv + kv] * kLog2e : 0.f;
+    }
+    float dv[32], dk[32];
 #pragma unroll
-                        for (int g = 0; g < 4; ++g) {
-                            const int col = p.col0 + c * 16 + g * 4;
-                            if (col < p.d)
-                                red_add_v4(dqcol + (int64_t)(c * 4 + g) * p.Lq * 4, __uint_as_float(o[g * 4]), __uint_as_float(o[g * 4 + 1]),
-                                           __uint_as_float(o[g * 4 + 2]), __uint_as_float(o[g * 4 + 3]));
-                        }
-                    }
-                }
+    for (int i = 0; i < 32; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
+    const uint64_t kdesc = make_smem_desc(smem_u32(sK) + wg * 64 * 128, 16, 1024);
+    const uint64_t vdesc = make_smem_desc(smem_u32(sV) + wg * 64 * 128, 16, 1024);
+    // dQ: A = dS^T of all 128 kv rows read transposed, B = the 128 K rows, output columns of the slice (both MN-major)
+    const uint64_t kdesc_mn = make_smem_desc(smem_u32(sK) + cbox * BOX_BYTES, BOX_BYTES, 1024);
+    const uint32_t ds_base = smem_u32(sDS) + wg * Cfg::DS_BYTES;
+    const uint64_t dsdesc = make_smem_desc(smem_u32(sDS), 2 * Cfg::DS_BYTES, 1024);
+    mbar_wait(kv_full, 0);
+    for (int i = i0; i < i1; ++i) {
+        const int st = (i - i0) % STAGES;
+        mbar_wait(&q_full[st], ((i - i0) / STAGES) & 1);
+        const uint32_t qb = smem_u32(sQ + st * Cfg::Q_BYTES), dob = smem_u32(sdO + st * Cfg::Q_BYTES);
+        const uint64_t qdesc = make_smem_desc(qb, 16, 1024), dodesc = make_smem_desc(dob, 16, 1024);
+        // ---- S^T = K Q^T, dP^T = V dO^T  (rows: kv, columns: q)
+        float s[32], dp[32];
+        wgmma_fence();
+        wgmma_ss<64, 0, 0>(s, kdesc, qdesc, 0u);
+        for (int ks = 1; ks < p.nks; ++ks)
+            wgmma_ss<64, 0, 0>(s, desc_adv(kdesc, kmajor_off(ks, BOX_BYTES)), desc_adv(qdesc, kmajor_off(ks, Cfg::QBOX)), 1u);
+        wgmma_ss<64, 0, 0>(dp, vdesc, dodesc, 0u);
+        for (int ks = 1; ks < p.nks; ++ks)
+            wgmma_ss<64, 0, 0>(dp, desc_adv(vdesc, kmajor_off(ks, BOX_BYTES)), desc_adv(dodesc, kmajor_off(ks, Cfg::QBOX)), 1u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_acc(s);
+        wgmma_fence_acc(dp);
+        // ---- P^T, dS^T = scale * P^T (dP^T - delta) as bf16 A fragments (K = q); dS^T also to shared memory for dQ
+        uint32_t pa[4][4], da[4][4];
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {
+            // per-column (query) statistics of the four columns of this k-step this thread holds
+            float lq[4], dq_[4];
+#pragma unroll
+            for (int c = 0; c < 4; ++c) {
+                const int q = i * 64 + 16 * kk + 8 * (c >> 1) + cq + (c & 1);
+                const bool ok = q < p.Lq;
+                lq[c] = ok ? __ldg(p.lse + bh * p.Lq + q) * kLog2e : INFINITY;   // masked query: P = exp2(-inf) = 0
+                dq_[c] = ok ? __ldg(p.delta + bh * p.Lq + q) : 0.f;
             }
-        };
-        float lse_nx = (i0 * 128 + row < p.Lq) ? p.lse[stat_base + i0 * 128 + row] : 0.f;   // software-prefetched one q tile ahead
-        float dlt_nx = (i0 * 128 + row < p.Lq) ? p.delta[stat_base + i0 * 128 + row] : 0.f;
-        // ---- lean loop: full kv tiles without a key bias on the register-resident schedule (every self-attention of the UNet).
-        // The general loop below carries the masking / bias code inside its unrolled bodies and recomputes the swizzled store
-        // addresses and the accumulator pointers per tile: ~700 instructions per thread and q tile for 32 score elements, which
-        // made the 16 softmax warps -- not the tensor pipe or the MUFU -- the limit (2 800 issue cycles per tile against 960 of
-        // tcgen05 work and 1 024 of ex2).  Here everything that does not depend on the tile is hoisted: shared-space store
-        // addresses, TMEM addresses, the fp32 dQ accumulator pointers of this thread's 16-column chunks.
-        const bool lean = p.early_sdp && !special && p.dq_direct == nullptr;
-        if (lean) {
-            const int c = part;
-            const uint32_t sp_a = smem_u32(sP) + (c >> 1) * TILE_BYTES, sds_a = smem_u32(sdS) + (c >> 1) * TILE_BYTES;
-            uint32_t soff[4];
 #pragma unroll
-            for (int g = 0; g < 4; ++g) soff[g] = sw128_offset(row, (c & 1) * 4 + g);
-            const float sl2 = p.scale_log2, sc = p.scale;
-            const uint32_t ts_c = tS + lb + c * 32, tdp_c = tdP + lb + c * 32;
-            const int nch = p.ncols_out / 16;
-            const int64_t lq4 = (int64_t)p.Lq * 4;
-            // fp32 dQ accumulator [B, H, d/4, Lq, 4]: slot of (first 4-column group of the launch, this thread's row of tile 0)
-            float* dq_row = p.dq_acc + ((((int64_t)b * p.H + h) * (p.dq_ld / 4) + p.col0 / 4) * p.Lq + (i0 * 128 + row)) * 4;
-            const int dvalid = p.d - p.col0;                  // valid output columns of this launch
-            auto drain = [&](float* dst, bool ok) {
-                for (int cc = part; cc < nch; cc += kBwdParts) {
-                    uint32_t o[16];
-                    tmem_ld16(tdQ + lb + cc * 16, o);
-                    tmem_wait_ld();
-                    if (ok) {
+            for (int r = 0; r < 4; ++r) {
+                const int hh = r & 1;
+                const int c = 2 * (r >> 1);                     // index into lq / dq_ of the first of the two columns
+                const int idx = 8 * kk + 4 * (r >> 1) + 2 * hh;
+                float pv[2], dsv[2];
 #pragma unroll
-                        for (int g = 0; g < 4; ++g)
-                            if (cc * 16 + g * 4 < dvalid)
-                                red_add_v4(dst + (int64_t)(cc * 4 + g) * lq4, __uint_as_float(o[g * 4]), __uint_as_float(o[g * 4 + 1]),
-                                           __uint_as_float(o[g * 4 + 2]), __uint_as_float(o[g * 4 + 3]));
-                    }
+                for (int e = 0; e < 2; ++e) {
+                    const float pe = kv_ok[hh] ? fast_exp2(s[idx + e] * sl2 + kvb[hh] - lq[c + e]) : 0.f;
+                    pv[e] = pe;
+                    dsv[e] = scale * pe * (dp[idx + e] - dq_[c + e]);
                 }
-            };
-            // phase trace of the loop (tools/probe_attn_trace.py): compiled in only with -DHCP_ATTN_TRACE (HCP_EXTRA_NVCC_FLAGS), the
-            // seven 64-bit accumulators would otherwise sit in every softmax thread's registers
-#ifdef HCP_ATTN_TRACE
-            const bool trc = p.trace && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && threadIdx.x == 0;
-            long long t_wait_sdp = 0, t_exp = 0, t_wait_dq = 0, t_pstore = 0, t_ds = 0, t_dsstore = 0, t_drain = 0, tk = trc ? clock64() : 0;
-            const long long t_begin = tk;
-#define HCP_LAP(acc) do { if (trc) { const long long tn_ = clock64(); acc += tn_ - tk; tk = tn_; } } while (0)
-#else
-#define HCP_LAP(acc) do { } while (0)
-#endif
-            for (int i = 0; i < nq; ++i) {
-                const int qrow = (i0 + i) * 128 + row;
-                const bool qok = qrow < p.Lq;
-                // rows past Lq: Q / dO rows are TMA zero fill, so S = dP = 0 there and a -inf offset makes every P (and dS) exactly 0
-                const float neg_lse2 = qok ? -lse_nx * kLog2e : -INFINITY;
-                const float neg_dlt_s = -dlt_nx * sc;
-                if (i + 1 < nq) {
-                    const int qn = qrow + 128;
-                    lse_nx = (qn < p.Lq) ? p.lse[stat_base + qn] : 0.f;
-                    dlt_nx = (qn < p.Lq) ? p.delta[stat_base + qn] : 0.f;
-                }
-                mbar_wait(sdp_full, i & 1);
-                tc_fence_after();
-                HCP_LAP(t_wait_sdp);
-                uint32_t pk[16];
-                {
-                    uint32_t v0[16], v1[16];
-                    tmem_ld16(ts_c, v0);
-                    tmem_ld16(ts_c + 16, v1);
-                    tmem_wait_ld();
-                    tc_fence_before();
-                    mbar_arrive(sdp_free);                      // S columns free for Q K^T of the next tile
-#pragma unroll
-                    for (int e = 0; e < 16; e += 2) {
-                        pk[e >> 1] = pack_bf16x2(fast_exp2(fmaf(__uint_as_float(v0[e]), sl2, neg_lse2)),
-                                                 fast_exp2(fmaf(__uint_as_float(v0[e + 1]), sl2, neg_lse2)));
-                        pk[8 + (e >> 1)] = pack_bf16x2(fast_exp2(fmaf(__uint_as_float(v1[e]), sl2, neg_lse2)),
-                                                       fast_exp2(fmaf(__uint_as_float(v1[e + 1]), sl2, neg_lse2)));
-                    }
-                }
-                HCP_LAP(t_exp);
-                if (i > 0) {
-                    mbar_wait(dq_full, (i - 1) & 1);            // dK/dQ of the previous tile have finished reading sP / sdS
-                    tc_fence_after();
-                }
-                HCP_LAP(t_wait_dq);
-#pragma unroll
-                for (int g = 0; g < 4; ++g) sts128(sp_a + soff[g], make_uint4(pk[g * 4], pk[g * 4 + 1], pk[g * 4 + 2], pk[g * 4 + 3]));
-                fence_proxy_async_smem();
-                mbar_arrive(p_ready);
-                HCP_LAP(t_pstore);
-                {
-                    uint32_t w0[16], w1[16];
-                    tmem_ld16(tdp_c, w0);
-                    tmem_ld16(tdp_c + 16, w1);
-                    tmem_wait_ld();
-                    tc_fence_before();
-                    mbar_arrive(dp_free);
-                    // dS = P (dP - delta) scale as a packed bf16x2 product with the bf16-rounded P the tensor pipe sees in dV
-#pragma unroll
-                    for (int e = 0; e < 16; e += 2) {
-                        pk[e >> 1] = mul_bf16x2(pk[e >> 1], pack_bf16x2(fmaf(__uint_as_float(w0[e]), sc, neg_dlt_s),
-                                                                        fmaf(__uint_as_float(w0[e + 1]), sc, neg_dlt_s)));
-                        pk[8 + (e >> 1)] = mul_bf16x2(pk[8 + (e >> 1)], pack_bf16x2(fmaf(__uint_as_float(w1[e]), sc, neg_dlt_s),
-                                                                                    fmaf(__uint_as_float(w1[e + 1]), sc, neg_dlt_s)));
-                    }
-                }
-                HCP_LAP(t_ds);
-#pragma unroll
-                for (int g = 0; g < 4; ++g) sts128(sds_a + soff[g], make_uint4(pk[g * 4], pk[g * 4 + 1], pk[g * 4 + 2], pk[g * 4 + 3]));
-                tc_fence_before();
-                fence_proxy_async_smem();
-                mbar_arrive(ds_ready);
-                HCP_LAP(t_dsstore);
-                if (i > 0) {
-                    // dQ of the PREVIOUS tile: its MMAs retired long ago (waited above), so this never blocks, and the tensor pipe is
-                    // meanwhile busy with dV_i, S/dP_{i+1}, dK_i
-                    drain(dq_row + (int64_t)(i - 1) * 512, qrow - 128 < p.Lq);
-                    tc_fence_before();
-                    mbar_arrive(dq_read);
-                }
-                HCP_LAP(t_drain);
-            }
-#undef HCP_LAP
-#ifdef HCP_ATTN_TRACE
-            if (trc) {
-                long long* o = p.trace;
-                o[0] = clock64() - t_begin; o[1] = nq; o[2] = t_wait_sdp; o[3] = t_exp; o[4] = t_wait_dq; o[5] = t_pstore; o[6] = t_ds;
-                o[7] = t_dsstore; o[8] = t_drain;
-            }
-#endif
-            mbar_wait(dq_full, (nq - 1) & 1);
-            tc_fence_after();
-            drain(dq_row + (int64_t)(nq - 1) * 512, (i0 + nq - 1) * 128 + row < p.Lq);
-        } else {
-        for (int i = 0; i < nq; ++i) {
-            const int qrow = (i0 + i) * 128 + row;
-            const bool qok = qrow < p.Lq;
-            const int64_t stat_idx = stat_base + qrow;
-            // rows past Lq: Q / dO rows are TMA zero fill, so S = dP = 0 there and a -inf offset makes every P (and dS) exactly 0
-            const float neg_lse2 = qok ? -lse_nx * kLog2e : -INFINITY;
-            const float neg_dlt_s = -dlt_nx * p.scale;
-            if (i + 1 < nq) {
-                const int qn = qrow + 128;
-                lse_nx = (qn < p.Lq) ? p.lse[stat_base + qn] : 0.f;
-                dlt_nx = (qn < p.Lq) ? p.delta[stat_base + qn] : 0.f;
-            }
-            mbar_wait(sdp_full, i & 1);
-            tc_fence_after();
-            // ---- P = exp2(S*c - lse), dS = P * (dP - delta) * scale -> smem (K-major [q][kv], SWIZZLE_128B,
-            //      two 64-wide boxes each), 16 kv columns at a time.
-            auto emit16 = [&](const uint32_t (&v)[16], const uint32_t (&w)[16], int c, int hf, bool do_p, bool do_ds) {
-                uint32_t pk[8], dk[8];
-                if (!special && qok) {
-#pragma unroll
-                    for (int e = 0; e < 16; e += 2) {
-                        const float p0 = fast_exp2(fmaf(__uint_as_float(v[e]), p.scale_log2, neg_lse2));
-                        const float p1 = fast_exp2(fmaf(__uint_as_float(v[e + 1]), p.scale_log2, neg_lse2));
-                        pk[e >> 1] = pack_bf16x2(p0, p1);
-                        dk[e >> 1] = do_ds ? pack_bf16x2(p0 * fmaf(__uint_as_float(w[e]), p.scale, neg_dlt_s),
-                                                         p1 * fmaf(__uint_as_float(w[e + 1]), p.scale, neg_dlt_s))
-                                           : 0u;
-                    }
-                } else {
-#pragma unroll
-                    for (int e = 0; e < 16; e += 2) {
-                        float pe[2], de[2];
-#pragma unroll
-                        for (int t = 0; t < 2; ++t) {
-                            const int col = c * 32 + hf * 16 + e + t;
-                            float s2 = fmaf(__uint_as_float(v[e + t]), p.scale_log2, neg_lse2);
-                            if (bias && col < ncols) s2 += bias[kv0 + col] * kLog2e;
-                            const float pv = (qok && col < ncols) ? fast_exp2(s2) : 0.f;
-                            pe[t] = pv;
-                            de[t] = do_ds ? pv * fmaf(__uint_as_float(w[e + t]), p.scale, neg_dlt_s) : 0.f;
-                        }
-                        pk[e >> 1] = pack_bf16x2(pe[0], pe[1]);
-                        dk[e >> 1] = pack_bf16x2(de[0], de[1]);
-                    }
-                }
-#pragma unroll
-                for (int g = 0; g < 2; ++g) {
-                    const uint32_t off = (c >> 1) * TILE_BYTES + sw128_offset(row, (c & 1) * 4 + hf * 2 + g);
-                    if (do_p) *reinterpret_cast<uint4*>(sP + off) = make_uint4(pk[g * 4], pk[g * 4 + 1], pk[g * 4 + 2], pk[g * 4 + 3]);
-                    if (do_ds) *reinterpret_cast<uint4*>(sdS + off) = make_uint4(dk[g * 4], dk[g * 4 + 1], dk[g * 4 + 2], dk[g * 4 + 3]);
-                }
-            };
-            if (p.early_sdp) {
-                // The 32 logits of this thread go to registers and the S columns are released to the next tile's Q K^T at once;
-                // P is produced (and dV may start) before the 32 dP values are pulled in and released the same way.
-                static_assert(kChunksPerPart == 1, "the register-resident path assumes one 32-column chunk per warp");
-                const int c = part;
-                uint32_t pk[16];
-                {
-                    uint32_t v0[16], v1[16];
-                    tmem_ld16(tS + lb + c * 32, v0);
-                    tmem_ld16(tS + lb + c * 32 + 16, v1);
-                    tmem_wait_ld();
-                    tc_fence_before();
-                    mbar_arrive(sdp_free);
-#pragma unroll
-                    for (int e = 0; e < 16; e += 2) {
-                        float q0 = fmaf(__uint_as_float(v0[e]), p.scale_log2, neg_lse2), q1 = fmaf(__uint_as_float(v0[e + 1]), p.scale_log2, neg_lse2);
-                        float q2 = fmaf(__uint_as_float(v1[e]), p.scale_log2, neg_lse2), q3 = fmaf(__uint_as_float(v1[e + 1]), p.scale_log2, neg_lse2);
-                        if (special) {
-                            const int col = c * 32 + e;
-                            if (bias) {
-                                if (col < ncols) q0 += bias[kv0 + col] * kLog2e;
-                                if (col + 1 < ncols) q1 += bias[kv0 + col + 1] * kLog2e;
-                                if (col + 16 < ncols) q2 += bias[kv0 + col + 16] * kLog2e;
-                                if (col + 17 < ncols) q3 += bias[kv0 + col + 17] * kLog2e;
-                            }
-                            q0 = (col < ncols) ? q0 : -INFINITY;
-                            q1 = (col + 1 < ncols) ? q1 : -INFINITY;
-                            q2 = (col + 16 < ncols) ? q2 : -INFINITY;
-                            q3 = (col + 17 < ncols) ? q3 : -INFINITY;
-                        }
-                        pk[e >> 1] = pack_bf16x2(fast_exp2(q0), fast_exp2(q1));
-                        pk[8 + (e >> 1)] = pack_bf16x2(fast_exp2(q2), fast_exp2(q3));
-                    }
-                }
-                if (i > 0) {
-                    mbar_wait(dq_full, (i - 1) & 1);        // dK/dQ of the previous tile have finished reading sP / sdS
-                    tc_fence_after();
-                }
-#pragma unroll
-                for (int g = 0; g < 4; ++g)
-                    *reinterpret_cast<uint4*>(sP + (c >> 1) * TILE_BYTES + sw128_offset(row, (c & 1) * 4 + g)) =
-                        make_uint4(pk[g * 4], pk[g * 4 + 1], pk[g * 4 + 2], pk[g * 4 + 3]);
-                fence_proxy_async_smem();
-                mbar_arrive(p_ready);
-                {
-                    uint32_t w0[16], w1[16];
-                    tmem_ld16(tdP + lb + c * 32, w0);
-                    tmem_ld16(tdP + lb + c * 32 + 16, w1);
-                    tmem_wait_ld();
-                    tc_fence_before();
-                    mbar_arrive(dp_free);
-                    // dS = P (dP - delta) scale, with the bf16-rounded P the tensor pipe sees in dV
-#pragma unroll
-                    for (int e = 0; e < 16; e += 2) {
-                        // packed product: (dP - delta) scale is rounded to bf16 like P and multiplied two at a time -- no
-                        // re-expansion of the packed P (2 unpack + 2 FMUL per pair -> 1 HMUL2)
-                        pk[e >> 1] = mul_bf16x2(pk[e >> 1], pack_bf16x2(fmaf(__uint_as_float(w0[e]), p.scale, neg_dlt_s),
-                                                                        fmaf(__uint_as_float(w0[e + 1]), p.scale, neg_dlt_s)));
-                        pk[8 + (e >> 1)] = mul_bf16x2(pk[8 + (e >> 1)], pack_bf16x2(fmaf(__uint_as_float(w1[e]), p.scale, neg_dlt_s),
-                                                                                    fmaf(__uint_as_float(w1[e + 1]), p.scale, neg_dlt_s)));
-                    }
-                }
-#pragma unroll
-                for (int g = 0; g < 4; ++g)
-                    *reinterpret_cast<uint4*>(sdS + (c >> 1) * TILE_BYTES + sw128_offset(row, (c & 1) * 4 + g)) =
-                        make_uint4(pk[g * 4], pk[g * 4 + 1], pk[g * 4 + 2], pk[g * 4 + 3]);
-            } else {
-            for (int pass = 0; pass < (p.share_pds ? 2 : 1); ++pass) {
-                const bool do_p = (pass == 0);
-                const bool do_ds = !p.share_pds || pass == 1;
-                for (int c = part * kChunksPerPart; c < (part + 1) * kChunksPerPart; ++c) {
-#pragma unroll 1
-                  for (int hf = 0; hf < 2; ++hf) {                       // 16 kv columns at a time (register budget)
-                    uint32_t v[16], w[16];
-                    tmem_ld16(tS + lb + c * 32 + hf * 16, v);
-                    if (do_ds) tmem_ld16(tdP + lb + c * 32 + hf * 16, w);
-                    tmem_wait_ld();
-                    emit16(v, w, c, hf, do_p, do_ds);
-                  }
-                }
-                if (do_p) {
-                    fence_proxy_async_smem();
-                    mbar_arrive(p_ready);
-                    if (p.share_pds) mbar_wait(dv_done, i & 1);   // P consumed before dS overwrites the buffer
-                }
-            }
-            }
-            tc_fence_before();
-            fence_proxy_async_smem();
-            mbar_arrive(ds_ready);
-            if (!p.early_sdp) {
-                // ---- drain dQ_i into the fp32 accumulator
-                mbar_wait(dq_full, i & 1);
-                tc_fence_after();
-                drain_dq(qrow);
-                tc_fence_before();
-                mbar_arrive(dq_read);
-            } else if (i > 0) {
-                // dQ of the PREVIOUS tile: its MMAs retired long ago (waited above), so this never blocks, and the tensor pipe is
-                // meanwhile busy with dV_i, S/dP_{i+1}, dK_i
-                drain_dq(qrow - 128);
-                tc_fence_before();
-                mbar_arrive(dq_read);
+                pa[kk][r] = pack_bf16x2(pv[0], pv[1]);
+                da[kk][r] = pack_bf16x2(dsv[0], dsv[1]);
+                // dS^T element (kv row, q col) of the [64 kv][64 q] MN-major SWIZZLE_128B tile
+                const int row = r0 + 8 * hh, col = 16 * kk + 8 * (r >> 1) + cq;
+                asm volatile("st.shared.b32 [%0], %1;" ::"r"(ds_base + sw128_offset(row, col >> 3) + (col & 7) * 2), "r"(da[kk][r]) : "memory");
             }
         }
-        if (p.early_sdp) {
-            mbar_wait(dq_full, (nq - 1) & 1);
-            tc_fence_after();
-            drain_dq((i0 + nq - 1) * 128 + row);
+        fence_proxy_async_smem();
+        asm volatile("bar.sync 1, 256;" ::: "memory");                   // dS^T of both warpgroups in shared memory
+        // ---- dV += P^T dO, dK += dS^T Q (slice columns; MN-major B); one warpgroup: dQ_i = dS K over the CTA's 128 kv rows
+        const bool dq_here = ((i - i0) & 1) == wg;
+        const uint64_t dodesc_mn = make_smem_desc(dob + cbox * Cfg::QBOX, Cfg::QBOX, 1024);
+        const uint64_t qdesc_mn = make_smem_desc(qb + cbox * Cfg::QBOX, Cfg::QBOX, 1024);
+        float dqa[32];
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) wgmma_rs<64, 1>(dv, pa[kk], desc_adv(dodesc_mn, kk * 128), 1u);
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) wgmma_rs<64, 1>(dk, da[kk], desc_adv(qdesc_mn, kk * 128), 1u);
+        wgmma_commit();
+        wgmma_wait<0>();                                 // P^T / dS^T registers free before the dQ accumulator is live
+        wgmma_fence_acc(dv);
+        wgmma_fence_acc(dk);
+        if (dq_here) {
+            wgmma_fence();
+            wgmma_ss<64, 1, 1>(dqa, dsdesc, kdesc_mn, 0u);
+#pragma unroll
+            for (int kk = 1; kk < 8; ++kk) wgmma_ss<64, 1, 1>(dqa, desc_adv(dsdesc, kk * 128), desc_adv(kdesc_mn, kk * 128), 1u);
         }
-        }   // !lean
-        // ---- dK, dV of this kv tile: thread == kv row
-        mbar_wait(acc_full, 0);
-        tc_fence_after();
-        const int kvrow = kv0 + row;
-        for (int which = 0; which < 2; ++which) {
-            const uint32_t t = which ? tdK : tdV;
-            __nv_bfloat16* out = which ? p.dK : p.dV;
-            const int64_t ld = which ? p.lddk : p.lddv;
-            __nv_bfloat16* orow = out + ((int64_t)b * p.Lkv + kvrow) * ld + (int64_t)h * p.d + p.col0;
-            float* arow = p.dkv_acc ? p.dkv_acc + ((((int64_t)b * p.H + h) * p.Lkv + kvrow) * 2 + which) * p.dq_ld + p.col0 : nullptr;
-            for (int c = part; c < p.ncols_out / 16; c += kBwdParts) {
-                uint32_t o[16];
-                tmem_ld16(t + lb + c * 16, o);
-                tmem_wait_ld();
-                if (kvrow < p.Lkv && arow) {
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_acc(dqa);
+        mbar_arrive(&q_empty[st]);
+        asm volatile("bar.sync 1, 256;" ::: "memory");                   // the dS^T tiles may be overwritten by the next query tile
+        if (!dq_here) continue;
+        // ---- dQ of the CTA's kv rows -> fp32 accumulator [B,H,dq_ld/4,Lq,4]
 #pragma unroll
-                    for (int g = 0; g < 4; ++g) {
-                        const int col = p.col0 + c * 16 + g * 4;
-                        if (col < p.d)
-                            red_add_v4(arow + c * 16 + g * 4, __uint_as_float(o[g * 4]), __uint_as_float(o[g * 4 + 1]),
-                                       __uint_as_float(o[g * 4 + 2]), __uint_as_float(o[g * 4 + 3]));
-                    }
-                } else if (kvrow < p.Lkv) {
+        for (int hh = 0; hh < 2; ++hh) {
+            const int q = i * 64 + r0 + 8 * hh;
+            if (q >= p.Lq) continue;
 #pragma unroll
-                    for (int g = 0; g < 2; ++g) {
-                        const int col = p.col0 + c * 16 + g * 8;
-                        if (col < p.d) {
-                            uint4 w;
-                            w.x = pack_bf16x2(__uint_as_float(o[g * 8 + 0]), __uint_as_float(o[g * 8 + 1]));
-                            w.y = pack_bf16x2(__uint_as_float(o[g * 8 + 2]), __uint_as_float(o[g * 8 + 3]));
-                            w.z = pack_bf16x2(__uint_as_float(o[g * 8 + 4]), __uint_as_float(o[g * 8 + 5]));
-                            w.w = pack_bf16x2(__uint_as_float(o[g * 8 + 6]), __uint_as_float(o[g * 8 + 7]));
-                            *reinterpret_cast<uint4*>(orow + c * 16 + g * 8) = w;
-                        }
-                    }
-                }
+            for (int c8 = 0; c8 < 8; ++c8) {
+                const int col = p.col0 + 8 * c8 + cq;
+                if (col < p.d) red_add_v2(p.dq_acc + ((bh * (p.dq_ld / 4) + col / 4) * p.Lq + q) * 4 + (col & 3), dqa[4 * c8 + 2 * hh], dqa[4 * c8 + 2 * hh + 1]);
             }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 4 * kBwdParts) tmem_dealloc(tmem, 512);
+    // ---- dK / dV of this warpgroup's kv rows
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+        if (!kv_ok[hh]) continue;
+        const int kv = kvw + r0 + 8 * hh;
+#pragma unroll
+        for (int c8 = 0; c8 < 8; ++c8) {
+            const int col = p.col0 + 8 * c8 + cq;
+            if (col >= p.d) continue;
+            const float v0 = dv[4 * c8 + 2 * hh], v1 = dv[4 * c8 + 2 * hh + 1];
+            const float k0 = dk[4 * c8 + 2 * hh], k1 = dk[4 * c8 + 2 * hh + 1];
+            if (p.dkv_acc) {
+                float* base = p.dkv_acc + ((bh * p.Lkv + kv) * 2) * p.dq_ld + col;
+                red_add_v2(base, v0, v1);
+                red_add_v2(base + p.dq_ld, k0, k1);
+            } else {
+                *reinterpret_cast<uint32_t*>(p.dV + ((int64_t)b * p.Lkv + kv) * p.lddv + (int64_t)h * p.d + col) = pack_bf16x2(v0, v1);
+                *reinterpret_cast<uint32_t*>(p.dK + ((int64_t)b * p.Lkv + kv) * p.lddk + (int64_t)h * p.d + col) = pack_bf16x2(k0, k1);
+            }
+        }
+    }
 }
 
 // delta[b,h,q] = sum_e dO*O ; also zero-fills the fp32 dQ / dK,dV accumulators (when present).  One thread per (b,q,h): the
@@ -1279,16 +517,46 @@ __global__ void attn_bwd_post_kv_kernel(const float* __restrict__ acc, int dq_ld
     *reinterpret_cast<uint2*>(dst + bk * ld + (int64_t)h * d + e) = o;
 }
 
-static int make_head_map(CUtensorMap* m, const void* base, int64_t ld, int64_t B, int64_t H, int64_t L, int64_t d) {
+static int make_head_map(CUtensorMap* m, const void* base, int64_t ld, int64_t B, int64_t H, int64_t L, int64_t d, uint32_t rows) {
     uint64_t dims[4] = {(uint64_t)d, (uint64_t)H, (uint64_t)L, (uint64_t)B};
     uint64_t strides[3] = {(uint64_t)d * 2, (uint64_t)ld * 2, (uint64_t)L * ld * 2};
-    uint32_t box[4] = {64, 1, 128, 1};
+    uint32_t box[4] = {64, 1, rows, 1};
     return make_tmap_nd(m, base, 4, dims, strides, box);
 }
 
 static int check_common(int64_t B, int64_t H, int64_t Lq, int64_t Lkv, int64_t d) {
     if (B <= 0 || H <= 0 || Lq <= 0 || Lkv <= 0) return set_error(HCP_ERR_INVALID, "attention: empty problem");
     if (d % 8 != 0 || d < 8 || d > 192) return set_error(HCP_ERR_INVALID, "attention: head dim must be a multiple of 8 in [8,192]");
+    return HCP_OK;
+}
+
+template <int NB, int KVT>
+static int launch_attn_fwd(const AttnFwdParams& p, dim3 grid, cudaStream_t stream) {
+    using Cfg = AttnFwdCfg<NB, KVT>;
+    static bool configured = false;
+    if (!configured) {
+        cudaError_t e = cudaFuncSetAttribute(attn_fwd_kernel<NB, KVT>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
+        if (e != cudaSuccess) return set_cuda_error(e, "cudaFuncSetAttribute(attn_fwd)");
+        configured = true;
+    }
+    launch_k(attn_fwd_kernel<NB, KVT>, grid, dim3(kAttnThreads), Cfg::SMEM_BYTES, stream, p);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return set_cuda_error(e, "attn_fwd launch");
+    return HCP_OK;
+}
+
+template <int NB>
+static int launch_attn_bwd(const AttnBwdParams& p, dim3 grid, cudaStream_t stream) {
+    using Cfg = AttnBwdCfg<NB>;
+    static bool configured = false;
+    if (!configured) {
+        cudaError_t e = cudaFuncSetAttribute(attn_bwd_kernel<NB>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
+        if (e != cudaSuccess) return set_cuda_error(e, "cudaFuncSetAttribute(attn_bwd)");
+        configured = true;
+    }
+    launch_k(attn_bwd_kernel<NB>, grid, dim3(kAttnThreads), Cfg::SMEM_BYTES, stream, p);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return set_cuda_error(e, "attn_bwd launch");
     return HCP_OK;
 }
 
@@ -1300,78 +568,40 @@ extern "C" int hcp_attn_fwd_bf16(const hcp_attn_args* a, hcp_stream_t stream_) {
     if (!a || !a->q || !a->k || !a->v || !a->o) return set_error(HCP_ERR_INVALID, "attn_fwd: null pointer");
     int rc = check_common(a->B, a->H, a->Lq, a->Lkv, a->d);
     if (rc) return rc;
-    static const bool use_v1 = getenv("HCP_ATTN_FWD_V1") != nullptr;
-    if (!use_v1) {
-        AttnFwd2Params p;
-        memset(&p, 0, sizeof(p));
-        if ((rc = make_head_map(&p.tmQ, a->q, a->ldq, a->B, a->H, a->Lq, a->d))) return rc;
-        if ((rc = make_head_map(&p.tmK, a->k, a->ldk, a->B, a->H, a->Lkv, a->d))) return rc;
-        if ((rc = make_head_map(&p.tmV, a->v, a->ldv, a->B, a->H, a->Lkv, a->d))) return rc;
-        p.B = (int)a->B; p.H = (int)a->H; p.Lq = (int)a->Lq; p.Lkv = (int)a->Lkv; p.d = (int)a->d;
-        p.nbox = (int)((a->d + 63) / 64);
-        p.dn = (int)((a->d + 15) / 16 * 16);
-        p.nq = (p.dn <= 64 && a->Lq > 128) ? 2 : 1;      // two tiles need 2 x (128 S + 64 P + dn O) <= 512 TMEM columns
-        p.kv_stages = (p.nbox == 1) ? 3 : (p.nbox == 2 ? 2 : 1);
-        p.scale_log2 = a->scale * kLog2e;
-        p.kv_bias = a->kv_bias;
-        p.O = (__nv_bfloat16*)a->o; p.ldo = a->ldo;
-        p.lse = a->lse;
-        const int smem = (p.nq + 2 * p.kv_stages) * p.nbox * TILE_BYTES + 4096 + 256 + 1024;
-        static bool configured2 = false;
-        if (!configured2) {
-            cudaError_t e = cudaFuncSetAttribute(attn_fwd2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-            if (e != cudaSuccess) return set_cuda_error(e, "cudaFuncSetAttribute(attn_fwd2)");
-            configured2 = true;
-        }
-        if (smem > 227 * 1024) return set_error(HCP_ERR_INVALID, "attn_fwd: shared memory budget exceeded");
-        dim3 grid((unsigned)((a->Lq + 128 * p.nq - 1) / (128 * p.nq)), (unsigned)a->H, (unsigned)a->B);
-        launch_k(attn_fwd2_kernel, dim3(grid), dim3(kFwd2Threads), smem, (cudaStream_t)stream_, p);
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) return set_cuda_error(e, "attn_fwd2 launch");
-        return HCP_OK;
-    }
+    const int nb = (int)((a->d + 63) / 64);
+    // kv tile: 128 rows, 64 when the O accumulator of d > 128 leaves no registers for a 128-column S tile
+    const uint32_t kvt = nb == 3 ? 64 : 128;
     AttnFwdParams p;
     memset(&p, 0, sizeof(p));
-    if ((rc = make_head_map(&p.tmQ, a->q, a->ldq, a->B, a->H, a->Lq, a->d))) return rc;
-    if ((rc = make_head_map(&p.tmK, a->k, a->ldk, a->B, a->H, a->Lkv, a->d))) return rc;
-    if ((rc = make_head_map(&p.tmV, a->v, a->ldv, a->B, a->H, a->Lkv, a->d))) return rc;
+    if ((rc = make_head_map(&p.tmQ, a->q, a->ldq, a->B, a->H, a->Lq, a->d, 128))) return rc;
+    if ((rc = make_head_map(&p.tmK, a->k, a->ldk, a->B, a->H, a->Lkv, a->d, kvt))) return rc;
+    if ((rc = make_head_map(&p.tmV, a->v, a->ldv, a->B, a->H, a->Lkv, a->d, kvt))) return rc;
     p.B = (int)a->B; p.H = (int)a->H; p.Lq = (int)a->Lq; p.Lkv = (int)a->Lkv; p.d = (int)a->d;
-    p.nbox = (int)((a->d + 63) / 64);
-    p.dn = (int)((a->d + 15) / 16 * 16);
-    p.tmem_cols = (128 + p.dn <= 256) ? 256 : 512;
+    p.nks = (int)((a->d + 15) / 16);
     p.scale_log2 = a->scale * kLog2e;
     p.kv_bias = a->kv_bias;
     p.O = (__nv_bfloat16*)a->o; p.ldo = a->ldo;
     p.lse = a->lse;
-    p.kv_stages = (p.nbox <= 2) ? 2 : 1;
-    const int smem = (1 + 2 * p.kv_stages) * p.nbox * TILE_BYTES + 256 + 1024;
-    static bool configured = false;
-    if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        if (e != cudaSuccess) return set_cuda_error(e, "cudaFuncSetAttribute(attn_fwd)");
-        configured = true;
-    }
-    dim3 grid((unsigned)((a->Lq + 127) / 128), (unsigned)a->H, (unsigned)a->B);
-    launch_k(attn_fwd_kernel, dim3(grid), dim3(kAttnThreads), smem, (cudaStream_t)stream_, p);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_cuda_error(e, "attn_fwd launch");
-    return HCP_OK;
+    const dim3 grid((unsigned)((a->Lq + 127) / 128), (unsigned)a->H, (unsigned)a->B);
+    cudaStream_t stream = (cudaStream_t)stream_;
+    if (nb == 1) return launch_attn_fwd<1, 128>(p, grid, stream);
+    if (nb == 2) return launch_attn_fwd<2, 128>(p, grid, stream);
+    return launch_attn_fwd<3, 64>(p, grid, stream);
 }
 
+// CTAs per kv tile along the query dimension: when the (kv tile, head, image) CTAs fill less than one wave, the query range is split
+// so that about two CTAs per SM run; the partial dK / dV sums then go through an fp32 buffer
+// (in units of 128 query rows, i.e. two of the kernel's query tiles: two splits -- an order-independent fp32 sum -- cover Lq <= 256)
 static int plan_qsplit(int64_t B, int64_t H, int64_t Lq, int64_t Lkv) {
     const int64_t base = ((Lkv + 127) / 128) * H * B;
     const int64_t nq = (Lq + 127) / 128;
-    if (base >= 120 || nq < 2) return 1;
-    int64_t qs = (296 + base - 1) / base;
+    const int64_t sms = num_sms();
+    if (base >= sms * 4 / 5 || nq < 2) return 1;
+    int64_t qs = (2 * sms + base - 1) / base;
     if (qs > nq) qs = nq;
     const int64_t per = (nq + qs - 1) / qs;
-    return (int)((nq + per - 1) / per);                 // every split owns at least one query tile
+    return (int)((nq + per - 1) / per);                 // every split owns at least one 128-row unit
 }
-
-static long long* g_attn_trace = nullptr;
-// bring-up hook (not in include/hcp_b200.h): the lean loop of CTA (0,0,0) of every later backward launch writes 9 int64 (total cycles,
-// q tiles, then the cycle sums of: wait S/dP, exp, wait dK/dQ of the previous tile, P store, dS arithmetic, dS store, dQ drain)
-extern "C" int hcp_debug_attn_trace(long long* buf) { g_attn_trace = buf; return HCP_OK; }
 
 extern "C" size_t hcp_attn_bwd_workspace_bytes(int64_t B, int64_t H, int64_t Lq, int64_t Lkv, int64_t d) {
     const int64_t dq_ld = (d + 3) / 4 * 4;
@@ -1387,6 +617,7 @@ extern "C" int hcp_attn_bwd_bf16(const hcp_attn_bwd_args* a, hcp_stream_t stream
     if (rc) return rc;
     if (a->workspace_bytes < hcp_attn_bwd_workspace_bytes(a->B, a->H, a->Lq, a->Lkv, a->d))
         return set_error(HCP_ERR_INVALID, "attn_bwd: workspace too small");
+    if ((a->ldo % 8) != 0 || (a->lddo % 8) != 0 || (a->lddq % 8) != 0) return set_error(HCP_ERR_INVALID, "attn_bwd: leading dimensions must be multiples of 8");
     cudaStream_t stream = (cudaStream_t)stream_;
     const int dq_ld = (int)((a->d + 3) / 4 * 4);
     float* delta = a->workspace;
@@ -1394,62 +625,42 @@ extern "C" int hcp_attn_bwd_bf16(const hcp_attn_bwd_args* a, hcp_stream_t stream
     const int qsplit = plan_qsplit(a->B, a->H, a->Lq, a->Lkv);
     const int64_t dkv_n = qsplit > 1 ? a->B * a->H * a->Lkv * 2 * dq_ld : 0;
     float* dkv_acc = qsplit > 1 ? dq_acc + a->B * a->H * a->Lq * dq_ld : nullptr;
-    // a single kv tile sees every key of a query row at once: dQ is final after one pass and is stored directly as bf16
-    const bool dq_direct = a->Lkv <= 128 && getenv("HCP_ATTN_BWD_NO_DIRECT_DQ") == nullptr;
-    if ((a->ldo % 8) != 0 || (a->lddo % 8) != 0 || (a->lddq % 8) != 0) return set_error(HCP_ERR_INVALID, "attn_bwd: leading dimensions must be multiples of 8");
     {
         const int64_t total = a->B * a->Lq * a->H;
         const int threads = 256;
         const int64_t blocks = (total + threads - 1) / threads;
         launch_k(attn_bwd_prep_kernel, dim3((unsigned)blocks), dim3(threads), 0, stream, (const __nv_bfloat16*)a->o, a->ldo,
                  (const __nv_bfloat16*)a->dout, a->lddo, (int)a->B, (int)a->H, (int)a->Lq, (int)a->d, delta,
-                 dq_direct ? (float*)nullptr : dq_acc, (int64_t)(a->B * a->H * a->Lq * dq_ld), dkv_acc, dkv_n);
+                 dq_acc, (int64_t)(a->B * a->H * a->Lq * dq_ld), dkv_acc, dkv_n);
     }
     AttnBwdParams p;
     memset(&p, 0, sizeof(p));
-    if ((rc = make_head_map(&p.tmQ, a->q, a->ldq, a->B, a->H, a->Lq, a->d))) return rc;
-    if ((rc = make_head_map(&p.tmK, a->k, a->ldk, a->B, a->H, a->Lkv, a->d))) return rc;
-    if ((rc = make_head_map(&p.tmV, a->v, a->ldv, a->B, a->H, a->Lkv, a->d))) return rc;
-    if ((rc = make_head_map(&p.tmdO, a->dout, a->lddo, a->B, a->H, a->Lq, a->d))) return rc;
+    if ((rc = make_head_map(&p.tmQ, a->q, a->ldq, a->B, a->H, a->Lq, a->d, 64))) return rc;
+    if ((rc = make_head_map(&p.tmK, a->k, a->ldk, a->B, a->H, a->Lkv, a->d, 128))) return rc;
+    if ((rc = make_head_map(&p.tmV, a->v, a->ldv, a->B, a->H, a->Lkv, a->d, 128))) return rc;
+    if ((rc = make_head_map(&p.tmdO, a->dout, a->lddo, a->B, a->H, a->Lq, a->d, 64))) return rc;
     p.B = (int)a->B; p.H = (int)a->H; p.Lq = (int)a->Lq; p.Lkv = (int)a->Lkv; p.d = (int)a->d;
-    p.nbox = (int)((a->d + 63) / 64);
-    p.dn = (int)((a->d + 15) / 16 * 16);
+    p.nks = (int)((a->d + 15) / 16);
     p.scale = a->scale;
     p.scale_log2 = a->scale * kLog2e;
     p.kv_bias = a->kv_bias;
     p.lse = a->lse;
     p.delta = delta;
-    p.dq_acc = dq_direct ? nullptr : dq_acc;
+    p.dq_acc = dq_acc;
     p.dq_ld = dq_ld;
-    p.dq_direct = dq_direct ? (__nv_bfloat16*)a->dq : nullptr;
-    p.lddq = a->lddq;
     p.qsplit = qsplit;
     p.dkv_acc = dkv_acc;
     p.dK = (__nv_bfloat16*)a->dk; p.lddk = a->lddk;
     p.dV = (__nv_bfloat16*)a->dv; p.lddv = a->lddv;
-    p.trace = g_attn_trace;
-    p.q_stages = (p.nbox == 1) ? 2 : 1;
-    p.share_pds = (p.nbox >= 3) ? 1 : 0;
-    p.early_sdp = (p.q_stages == 2 && 256 + 3 * p.dn <= 512 && getenv("HCP_ATTN_BWD_NO_EARLY") == nullptr) ? 1 : 0;
-    if (p.early_sdp) p.q_stages = 3;
-    const int smem = (2 + 2 * p.q_stages) * p.nbox * TILE_BYTES + (p.share_pds ? 2 : 4) * TILE_BYTES + 256 + 1024;
-    static bool configured = false;
-    if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        if (e != cudaSuccess) return set_cuda_error(e, "cudaFuncSetAttribute(attn_bwd)");
-        configured = true;
-    }
-    if (smem > 227 * 1024) return set_error(HCP_ERR_INVALID, "attn_bwd: shared memory budget exceeded");
-    dim3 grid((unsigned)(((a->Lkv + 127) / 128) * qsplit), (unsigned)a->H, (unsigned)a->B);
-    // output column slices: at most 128 columns per launch, each starting on a 64-column box boundary
-    for (int col0 = 0; col0 < p.dn; col0 += 128) {
+    const int nb = (int)((a->d + 63) / 64);
+    const dim3 grid((unsigned)(((a->Lkv + 127) / 128) * qsplit), (unsigned)a->H, (unsigned)a->B);
+    // output column slices of 64 (one box): dK / dV / dQ accumulators of a slice stay in registers; S and dP are recomputed per slice
+    for (int col0 = 0; col0 < a->d; col0 += 64) {
         p.col0 = col0;
-        p.ncols_out = (p.dn - col0 < 128) ? (p.dn - col0) : 128;
-        launch_k(attn_bwd_kernel, dim3(grid), dim3(kAttnBwdThreads), smem, stream, p);
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) return set_cuda_error(e, "attn_bwd launch");
+        rc = nb == 1 ? launch_attn_bwd<1>(p, grid, stream) : nb == 2 ? launch_attn_bwd<2>(p, grid, stream) : launch_attn_bwd<3>(p, grid, stream);
+        if (rc) return rc;
     }
-    if (!dq_direct) {
+    {
         const int64_t n = a->B * a->Lq * a->H * (a->d / 4);
         launch_k(attn_bwd_post_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, stream, dq_acc, dq_ld, (int)a->B, (int)a->H, (int)a->Lq,
                  (int)a->d, (__nv_bfloat16*)a->dq, a->lddq);

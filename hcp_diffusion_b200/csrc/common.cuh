@@ -1,7 +1,6 @@
 // SPDX-License-Identifier: Apache-2.0
-// Device-side building blocks for the sm_100a kernels of libhcpb200:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (MMA / TMEM alloc / ld / st / commit) wrappers
-// and the UMMA shared-memory / instruction descriptor encoders.
+// Device-side building blocks for the sm_90a kernels of libhcpb200:
+// mbarrier, TMA (cp.async.bulk.tensor), the wgmma shared-memory descriptor encoder (wgmma.cuh: the MMA wrappers).
 //
 // Everything here is inline PTX; no CUTLASS/CuTe dependency in the product.
 #pragma once
@@ -9,6 +8,7 @@
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
 #include <stdint.h>
+#include "wgmma.cuh"
 
 namespace hcp {
 
@@ -19,6 +19,9 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
     return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 __device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31; }
+// warp index broadcast from lane 0: provably warp-uniform, so role branches on it are not divergent paths to ptxas (a wgmma
+// inside a possibly divergent path is serialized: every instruction waits for the previous one to retire)
+__device__ __forceinline__ int warp_id_uniform() { return __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0); }
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred = 0;
     asm volatile(
@@ -34,7 +37,7 @@ __device__ __forceinline__ bool elect_one() {
 // cudaLaunchAttributeProgrammaticStreamSerialization (host_util.h: launch_k), so its CTAs may become resident while the
 // previous kernel of the stream is still draining.  Contract: pdl_wait() before the first global-memory access (it returns
 // once the whole preceding grid has completed and its writes are visible -- covers RAW and WAR hazards on recycled buffers);
-// everything before it (barrier init, TMEM allocation, descriptor prefetch) overlaps the predecessor's tail.
+// everything before it (barrier init, descriptor prefetch) overlaps the predecessor's tail.
 // pdl_trigger() lets the NEXT kernel start launching; it only affects scheduling, never visibility.
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -69,7 +72,7 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 __device__ __forceinline__ void fence_mbar_init() {
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
-// generic-proxy writes to smem -> visible to the async proxy (TMA / tcgen05 operand reads)
+// generic-proxy writes to smem -> visible to the async proxy (TMA / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -138,209 +141,29 @@ __device__ __forceinline__ void tma_load_5d(void* smem, const CUtensorMap* m, ui
         : "memory");
 }
 
-// TMA store (tile mode, shared::cta -> global), tracked by the issuing thread's bulk async-group
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* smem_src_u32_holder, uint32_t smem_addr, int c0, int c1) {
-    (void)smem_src_u32_holder;
-    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-                 ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_addr), "r"(c0), "r"(c1)
-                 : "memory");
-}
-__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-// all bulk groups of this thread have finished READING their shared-memory sources (the buffers may be overwritten)
-__device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-
 // ---------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation
-// ---------------------------------------------------------------------------------------------
-// Whole-warp (.sync.aligned) instructions. `ncols` power of two in [32, 512].
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-                 "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// ---------------------------------------------------------------------------------------------
-// tcgen05: descriptors
-// ---------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor (64 bit):
+// wgmma shared-memory matrix descriptor (64 bit):
 //   [0,14)  start address >> 4          [16,30) leading-dim byte offset >> 4
-//   [32,46) stride-dim byte offset >> 4 [46,48) version (1 on sm_100)
-//   [61,64) layout: 0 none, 2 = 128B swizzle, 4 = 64B, 6 = 32B
+//   [32,46) stride-dim byte offset >> 4 [62,64) layout: 0 interleave, 1 = 128B swizzle, 2 = 64B, 3 = 32B
 //
 // K-major, SWIZZLE_128B, bf16: a tile is rows of 128 B (64 elements of K); 8 consecutive rows form a
-// 1024 B swizzle atom; SBO = 1024 (distance between 8-row groups), LBO unused (1).
+// 1024 B swizzle atom; SBO = 1024 (distance between 8-row groups), LBO unused (1).  A 16-element k-step
+// inside the atom advances the start address by 32 B.
 // MN-major, SWIZZLE_128B, bf16: a row of 128 B holds 64 consecutive MN elements for one k; 8 consecutive k
 // form the 1024 B atom; SBO = distance between 8-k groups, LBO = distance between 64-wide MN chunks.
+// ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     uint64_t d = 0;
     d |= static_cast<uint64_t>((saddr & 0x3FFFF) >> 4);
     d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
     d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= static_cast<uint64_t>(1) << 46;  // version
-    d |= static_cast<uint64_t>(2) << 61;  // SWIZZLE_128B
+    d |= static_cast<uint64_t>(1) << 62;  // SWIZZLE_128B
     return d;
 }
-// Instruction descriptor for kind::f16 with bf16 A/B and fp32 accumulation.
-//   [4,6) C fmt (1 = f32)  [7,10) A fmt (1 = bf16)  [10,13) B fmt (1 = bf16)
-//   [15] A major (0 = K, 1 = MN)  [16] B major  [17,23) N >> 3  [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N, int a_mn_major, int b_mn_major) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(a_mn_major) << 15) |
-           (static_cast<uint32_t>(b_mn_major) << 16) | (static_cast<uint32_t>(N >> 3) << 17) |
-           (static_cast<uint32_t>(M >> 4) << 24);
+// advance a descriptor's start address by `off16` 16-byte units (the 14-bit field never carries out for shared-memory addresses)
+__device__ __forceinline__ uint64_t desc_adv(uint64_t d, uint32_t off16) {
+    return (d & 0xffffffff00000000ull) | (uint64_t)((uint32_t)d + off16);
 }
-
-// D[tmem] (+)= A[smem] * B[smem]; issued by ONE thread on behalf of the CTA.
-__device__ __forceinline__ void umma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                        uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]  (A operand read from tensor memory)
-__device__ __forceinline__ void umma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                        uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// Arrive on an mbarrier when all previously issued MMAs of this thread have completed.
-// (implies tcgen05.fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-
-
-// ---------------------------------------------------------------------------------------------
-// CTA pairs (tcgen05 cta_group::2): two CTAs of one cluster (one TPC) issue ONE MMA of M = 256; each holds 128 rows of A and
-// N/2 rows of B in its own shared memory at the same CTA-relative offsets, and 128 accumulator lanes in its own TMEM.
-// Semantics pinned on the part by tests/native/probe_2cta.cu (profiles/r02_probe_2cta.log):
-//   * tcgen05.alloc / dealloc .cta_group::2 is executed by one warp of EACH CTA and returns the same column base in both;
-//   * a TMA load with .cta_group::2 may signal an mbarrier of the PEER CTA (shared::cluster address): both CTAs' bytes are
-//     credited to the leader's `full` barrier, whose single arrive.expect_tx names the bytes of BOTH;
-//   * the leader's elected thread issues the MMAs; tcgen05.commit .multicast::cluster arrives on the barrier at the same offset
-//     in every CTA of the mask.
-// ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t mapa_u32(uint32_t local_addr, uint32_t rank) {
-    uint32_t remote;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(local_addr), "r"(rank));
-    return remote;
-}
-// arrive (release at cluster scope) on an mbarrier given by its shared::cluster address (own or peer CTA)
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar_cluster_addr) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(bar_cluster_addr) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_pair(void* smem, const CUtensorMap* m, uint32_t bar_cluster_addr, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(smem_u32(smem)), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1)
-        : "memory");
-}
-__device__ __forceinline__ void tma_load_3d_pair(void* smem, const CUtensorMap* m, uint32_t bar_cluster_addr, int c0, int c1, int c2) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-        ::"r"(smem_u32(smem)), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "r"(c2)
-        : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_pair(void* smem, const CUtensorMap* m, uint32_t bar_cluster_addr, int c0, int c1, int c2, int c3) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-        ::"r"(smem_u32(smem)), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-        : "memory");
-}
-__device__ __forceinline__ void tma_load_5d_pair(void* smem, const CUtensorMap* m, uint32_t bar_cluster_addr, int c0, int c1, int c2, int c3,
-                                                 int c4) {
-    asm volatile(
-        "cp.async.bulk.tensor.5d.cta_group::2.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
-        ::"r"(smem_u32(smem)), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_pair() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_ss_pair(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// arrive on the mbarrier at this CTA-relative address in every CTA of `mask` once the pair's MMAs issued so far have retired
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar, uint16_t mask) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(smem_u32(bar)), "h"(mask)
-                 : "memory");
-}
-
-// ---------------------------------------------------------------------------------------------
-// tcgen05: TMEM <-> registers. 32x32b shape: thread i of the warp <-> TMEM lane (base_lane + i),
-// register j <-> column (base_col + j). A warp may only touch the lane quarter (warp_id % 4).
-// ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%32], "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31};"
-        ::"r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-          "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]),
-          "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]),
-          "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31]),
-          "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%16], "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15};"
-        ::"r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-          "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]),
-          "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 // ---------------------------------------------------------------------------------------------
 // small numeric helpers
@@ -364,14 +187,9 @@ __device__ __forceinline__ float warp_max(float v) {
     return v;
 }
 
-// vectorised fp32 reduction to global memory (sm_90+): 4 consecutive floats, 16-byte aligned
-__device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c, float d) {
-    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
-__device__ __forceinline__ uint32_t mul_bf16x2(uint32_t a, uint32_t b) {
-    uint32_t d;
-    asm("mul.rn.bf16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b));
-    return d;
+// vectorised fp32 reduction to global memory (sm_90+): 2 consecutive floats, 8-byte aligned
+__device__ __forceinline__ void red_add_v2(float* addr, float a, float b) {
+    asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
 }
 __device__ __forceinline__ float fast_exp2(float x) {
     float y;
@@ -380,29 +198,12 @@ __device__ __forceinline__ float fast_exp2(float x) {
 }
 
 // Explicit shared-space accesses on 32-bit shared addresses (smem_u32).  Pointers derived from an aligned dynamic-smem base by integer
-// arithmetic lose their address space and compile to generic LD / ST; these keep the LDS / STS forms.
+// arithmetic lose their address space and compile to generic LD; this keeps the LDS form.
 __device__ __forceinline__ uint4 lds128(uint32_t a) {
     uint4 v;
     asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(a) : "memory");
     return v;
 }
-__device__ __forceinline__ void sts128(uint32_t a, uint4 v) {
-    asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
-__device__ __forceinline__ float4 lds_f4(uint32_t a) {
-    float4 v;
-    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a) : "memory");
-    return v;
-}
-__device__ __forceinline__ void sts_f4(uint32_t a, float4 v) {
-    asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(a), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
-}
-__device__ __forceinline__ int64_t lds_b64(uint32_t a) {
-    int64_t v;
-    asm volatile("ld.shared.b64 %0, [%1];" : "=l"(v) : "r"(a) : "memory");
-    return v;
-}
-__device__ __forceinline__ void sts_b64(uint32_t a, int64_t v) { asm volatile("st.shared.b64 [%0], %1;" ::"r"(a), "l"(v) : "memory"); }
 
 // Byte offset of element (row, 16-byte chunk `c16`) inside a K-major SWIZZLE_128B tile whose rows are
 // 128 B and whose base is 1024 B aligned: chunk index is XOR-ed with (row % 8).

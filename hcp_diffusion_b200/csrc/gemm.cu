@@ -1,14 +1,13 @@
 // SPDX-License-Identifier: Apache-2.0
-// tcgen05 + TMA GEMM / implicit-GEMM 3x3 convolution for sm_100a.
+// wgmma + TMA GEMM / implicit-GEMM 3x3 convolution for sm_90a.
 //
 //   out[M,N] = sum_s A_s[M,K_s] . B_s[N,K_s]^T + bias[N] + rowbias[row/rows_per_group, N] + residual[M,N]
 //
-// Persistent kernel, one CTA (or CTA pair, tcgen05 cta_group::2) per SM walking 128 x BN (256 x BN) work items.  Warp roles
-// (320 threads):
-//   warp 0    : TMA producer  (one elected lane; A and B tiles of 64 K-elements per stage, SWIZZLE_128B)
-//   warp 1    : TMEM allocator + MMA issuer (one elected lane issues tcgen05.mma, fp32 accumulators in TMEM)
-//   warps 2-9 : epilogue (tcgen05.ld the accumulator, fused bias / per-image bias / residual, bf16, TMA or coalesced stores);
-//               two TMEM accumulators let the epilogue of item i run under the main loop of item i+1
+// Persistent kernel, one CTA per SM walking 128 x BN work items.  Warp roles (288 threads):
+//   warps 0-7 : two MMA warpgroups; warpgroup g issues wgmma.mma_async for rows [64g, 64g+64) of the tile (fp32 accumulators in
+//               registers) and runs the epilogue of those rows (fused bias / per-image bias / residual, bf16 stores)
+//   warp 8    : TMA producer (one elected lane; A and B tiles of 64 K-elements per stage, SWIZZLE_128B), which runs ahead into the
+//               next work item while the warpgroups drain the current one
 //
 // hcpdiff's LoRA (reference: hcpdiff/models/lora_layers_patch.py:44-57) reaches this kernel in two forms: adapters that apply to all
 // rows are merged into the weight operand once per step (misc.cu: lora_merge_kernel) and their rank products T / U leave as a second
@@ -28,8 +27,8 @@ namespace hcp {
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;
 constexpr int A_STAGE_BYTES = BLOCK_M * BLOCK_K * 2;
-constexpr int kGemmThreads = 320;        // warp 0: TMA, warp 1: MMA, warps 2-9: epilogue (two per TMEM lane quarter)
-constexpr int kGemmEpiThreads = 256;
+constexpr int kGemmMmaThreads = 256;     // two MMA warpgroups
+constexpr int kGemmThreads = kGemmMmaThreads + 32;   // + the TMA producer warp
 constexpr int kMaxTaps = 9;
 
 struct TapEntry {
@@ -43,7 +42,6 @@ struct TapEntry {
 struct alignas(64) GemmKParams {
     CUtensorMap tmA[HCP_GEMM_MAX_SEG];
     CUtensorMap tmB[HCP_GEMM_MAX_SEG];
-    CUtensorMap tmOut, tmOut2;         // [M, n_main] / [M, N - n_main] bf16 outputs, box 16 columns x 128 rows, no swizzle (tma_store)
     int32_t nkb[HCP_GEMM_MAX_SEG];     // 64-wide k-blocks per segment (conv: per tap)
     int32_t klast[HCP_GEMM_MAX_SEG];   // 16-wide k-steps issued in the last k-block of the segment (1..4)
     int32_t nseg;
@@ -72,50 +70,23 @@ struct alignas(64) GemmKParams {
     __nv_bfloat16* out2;
     int64_t ldo2;
     int32_t n_main;
-    int32_t tma_store;                 // 1: the rows of every tile are consecutive rows of `out`: parts leave through TMA stores
     // split-K: CTA (x, y) reduces the k-blocks [y*kb_per_split, (y+1)*kb_per_split) and stores raw fp32 partials
     int32_t splits, kb_per_split;
     float* ws;                         // [splits, M, N] fp32
-    long long* trace;                  // bring-up only (hcp_gemm_set_trace): 16 int64 slots per CTA (clock64 stamps / wait sums), NULL in production
 };
 
-// MSUB = number of 128-row M tiles (per CTA) one work item covers.  MSUB = 2 halves the B (weight) traffic per FLOP -- the long-K
-// convolutions are bound by the L2 -> SM operand stream, not by the tensor pipe -- at the price of using both TMEM accumulators
-// for one item (no epilogue / main-loop overlap, irrelevant when K is thousands).
-// PAIR = the work item is computed by a CTA PAIR (cluster of two CTAs on one TPC, tcgen05 cta_group::2): one MMA of M = 256 whose
-// B operand (BN rows) is split between the two CTAs' shared memories -- each CTA streams 128 rows of A and only BN/2 rows of B per
-// k-block, i.e. 128x320 of output per CTA for 36 KB of operands (71 MAC/B) where the single-CTA 128x160 tile needs the same 36 KB
-// for half the work (35 MAC/B).  The L2 -> SM stream (~44 B/clk/SM whatever the tiling) is what bounds these kernels.
-template <int BN, int MSUB = 1, bool PAIR = false>
+// BN = columns of a work item = N of every wgmma (a multiple of 16, at most 256); each MMA warpgroup holds 64 x BN fp32
+// accumulators (BN / 2 registers per thread).
+template <int BN>
 struct GemmCfg {
-    static constexpr int B_ROWS = PAIR ? BN / 2 : BN;             // rows of B this CTA loads per k-block
-    // one tcgen05.mma covers at most N = 256 columns: wider tiles issue NSPLIT instructions per k-step, each on MMA_N columns.
-    // A CTA of a pair holds MMA_N / 2 rows of B per instruction (rows [h * MMA_N + rank * MMA_N / 2, + MMA_N / 2) of the tile for
-    // instruction h), so the accumulator columns stay in the natural order of the tile.
-    static constexpr int NSPLIT = (BN > 256) ? 2 : 1;
-    static constexpr int MMA_N = BN / NSPLIT;
-    static constexpr int B_BOX_ROWS = B_ROWS / NSPLIT;            // rows per TMA box of B
-    static constexpr int A_BYTES = MSUB * A_STAGE_BYTES;
-    static constexpr int B_STAGE_BYTES = B_ROWS * BLOCK_K * 2;
-    static constexpr int ACC_STRIDE = 256;                         // TMEM columns between the two accumulators
-    static constexpr bool DOUBLE_ACC = (MSUB == 1 && BN <= 256);   // two accumulators alternate between work items
-    // the epilogue walks the accumulator in column parts of EBN (<= 160) columns through one staging buffer
-    static constexpr int EBN = (BN <= 176) ? BN : (BN % 160 == 0 ? 160 : 128);
-    static constexpr int NPART = BN / EBN;
-    static constexpr int EPI_NCH = (EBN / 16 + 1) / 2;             // 16-column TMEM chunks per column half of a part
-    // staging row pitch in bytes, an odd number of 16-byte units: a bf16 row of the part, or the fp32 values of one column half (split-K)
-    static constexpr int STG_PITCH = (EBN * 2 > EPI_NCH * 64 ? EBN * 2 : EPI_NCH * 64) + 16;
-    static constexpr int STG_BYTES = BLOCK_M * STG_PITCH;
-    static constexpr int BIAS_BYTES = ((BN * 4 + 127) / 128) * 128;  // bias slice of the tile's columns, staged once per work item
-    static constexpr int ROW_BYTES = BLOCK_M * 16;                   // per tile row: row of `out` (or -1) and its row-bias group
-    static constexpr int FIXED_BYTES = STG_BYTES + BIAS_BYTES + ROW_BYTES + 256 /*barriers*/ + 1024 /*align*/;
-    static constexpr int STAGE_BYTES = A_BYTES + B_STAGE_BYTES;
+    static constexpr int B_STAGE_BYTES = BN * BLOCK_K * 2;
+    static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
+    static constexpr int FIXED_BYTES = 256 /*barriers*/ + 1024 /*align*/;
     static constexpr int MAX_STAGES = (227 * 1024 - FIXED_BYTES) / STAGE_BYTES;
     // one CTA per SM: the ring must cover the TMA latency alone
-    static constexpr int STAGES = PAIR ? (MAX_STAGES > 6 ? 6 : MAX_STAGES) : (MSUB == 2) ? 3 : (BN > 160) ? 4 : (BN > 64) ? 5 : 8;
+    static constexpr int STAGES = MAX_STAGES > 6 ? 6 : MAX_STAGES;
     static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + FIXED_BYTES;
-    static_assert(BN % EBN == 0 && (MSUB - 1) * ACC_STRIDE + BN <= 512, "accumulators must fit the 512 TMEM columns");
-    static_assert(MMA_N <= 256 && MMA_N % 16 == 0 && (PAIR || NSPLIT == 1) && (B_BOX_ROWS % 8) == 0, "tcgen05.mma shape");
+    static_assert(BN % 16 == 0 && BN <= 256, "wgmma N");
     static_assert(STAGES >= 3, "pipeline too shallow");
 };
 
@@ -123,9 +94,8 @@ struct TileOrigin {
     int m0, img0, h0, w0;
 };
 
-// The output geometry of a launch, copied out of the parameter block BEFORE griddepcontrol.wait: the first touch of every
-// constant-bank line of the 1.6 KB parameter block costs a few hundred cycles, which then overlap the previous kernel's tail
-// instead of delaying this kernel's first TMA / first store.
+// The output geometry of a launch, copied out of the parameter block BEFORE griddepcontrol.wait, so that the first touch of the
+// constant-bank lines of the parameter block overlaps the previous kernel's tail.
 struct TileGeom {
     int conv, bw, bh, bn, tiles_w, tiles_h, oW, oH, sh, sw, oh0, ow0, rows_per_group;
     __device__ __forceinline__ explicit TileGeom(const GemmKParams& p)
@@ -168,10 +138,9 @@ __device__ __forceinline__ int64_t tile_row(const TileGeom& p, const TileOrigin&
 struct KPos {
     int s, t, kb, nkb_s;
 };
-// The reduction of a work item, held in REGISTERS of the single-thread control paths (TMA producer, MMA issuer).  Dynamically indexed
-// loads from the kernel-parameter block (p.nkb[s], p.klast[s], p.taps[t]...) cost about 200 cycles each on those threads: the r01
-// walk-and-skip loop over all k-blocks spent 215 cycles per SKIPPED k-block, i.e. 20 us per launch of the 14-way split 8x8
-// convolutions (profiles/r02_probe_trace_a.txt).  A split seeks its first k-block directly and advances incrementally.
+// The reduction of a work item, held in REGISTERS of the producer and the MMA warpgroups: dynamically indexed loads from the
+// kernel-parameter block (p.nkb[s], p.klast[s], p.taps[t]...) are slow constant-bank accesses.  A split seeks its first k-block
+// directly and advances incrementally.
 struct KPlan {
     int nkb0, nkb1, nkb2, kl0, kl1, kl2, ntap0, seg0, total_kb, conv, btile, kb_per_split;
     __device__ __forceinline__ explicit KPlan(const GemmKParams& p) {
@@ -201,464 +170,176 @@ struct KPlan {
     }
 };
 
-// Persistent kernel: grid = min(#work items, #SMs) CTAs (PAIR: CTA pairs); a work item is (split, m_tile, n_tile) with n fastest so
-// that the CTAs running concurrently share A tiles in L2.  Two TMEM accumulators: the epilogue of item i overlaps the main loop of i+1.
-// Epilogue: the residual tile is prefetched into a padded smem staging buffer with coalesced loads, each thread (== row) adds
-// bias / per-image bias / residual to its TMEM row and writes bf16 back into the staging buffer, then the tile leaves with
-// coalesced 16-byte stores (full 32-byte sectors instead of one 16-byte fragment per row and instruction).
-// PAIR: both CTAs run the TMA producer (own A rows, own half of B; all bytes credited to the LEADER's full barrier), the leader's
-// elected thread issues the M = 256 MMAs and multicasts the commits to both CTAs' empty / tmem_full barriers; each CTA drains its own
-// 128 accumulator rows and tells the leader's tmem_empty barrier (one elected lane per epilogue warp, remote arrive for the peer).
-template <int BN, int MSUB, bool PAIR>
-__global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_constant__ GemmKParams p) {
-    using Cfg = GemmCfg<BN, MSUB, PAIR>;
+// Persistent kernel: grid = min(#work items, #SMs) CTAs; a work item is (split, m_tile, n_tile) with n fastest so that the CTAs
+// running concurrently share A tiles in L2.  The producer runs up to STAGES k-blocks ahead, across work items, so the next item's
+// operands stream in while the warpgroups run the epilogue of the current one.  Split-K items store raw fp32 partials
+// (splitk_finalize_kernel applies bias / residual).
+template <int BN>
+__global__ void __launch_bounds__(kGemmThreads, 1) gemm_wgmma_kernel(const __grid_constant__ GemmKParams p) {
+    using Cfg = GemmCfg<BN>;
     constexpr int STAGES = Cfg::STAGES;
-    constexpr int NCTA = PAIR ? 2 : 1;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* sA = smem;
-    uint8_t* sB = smem + STAGES * Cfg::A_BYTES;
-    uint8_t* sStg = sB + STAGES * Cfg::B_STAGE_BYTES;
-    float* sBias = reinterpret_cast<float*>(sStg + Cfg::STG_BYTES);
-    uint8_t* sRow = sStg + Cfg::STG_BYTES + Cfg::BIAS_BYTES;          // [128] x (int64 row of `out`, int64 row-bias group)
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(sRow + Cfg::ROW_BYTES);
+    uint8_t* sB = smem + STAGES * A_STAGE_BYTES;
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(sB + STAGES * Cfg::B_STAGE_BYTES);
     uint64_t* empty_bar = full_bar + STAGES;
-    uint64_t* tmem_full_bar = empty_bar + STAGES;      // [2]
-    uint64_t* tmem_empty_bar = tmem_full_bar + 2;      // [2]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
 
-    const int warp = threadIdx.x >> 5;
+    const int warp = warp_id_uniform();
     const int lane = threadIdx.x & 31;
-    const uint32_t rank = PAIR ? cluster_ctarank() : 0u;
-    const int worker = PAIR ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;       // index of this CTA (pair) among the persistent workers
-    const int nworkers = PAIR ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-    const int tiles_mn = p.tiles_n * ((p.tiles_m + MSUB * NCTA - 1) / (MSUB * NCTA));      // work items per split
+    const int tiles_mn = p.tiles_n * p.tiles_m;      // work items per split
     const int total_work = tiles_mn * p.splits;
-    // m tile of (work item row mi, sub-tile sub) for this CTA
-    auto m_tile_of = [&](int mi, int sub) { return (mi * MSUB + sub) * NCTA + (int)rank; };
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], 1);
-        }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&tmem_full_bar[i], 1);
-            mbar_init(&tmem_empty_bar[i], PAIR ? 2 * (kGemmEpiThreads / 32) : kGemmEpiThreads);
+            mbar_init(&empty_bar[s], kGemmMmaThreads);
         }
         fence_mbar_init();
         for (int s = 0; s < p.nseg; ++s) {
             tma_prefetch_desc(&p.tmA[s]);
             tma_prefetch_desc(&p.tmB[s]);
         }
-        if (p.tma_store) {
-            tma_prefetch_desc(&p.tmOut);
-            if (p.out2) tma_prefetch_desc(&p.tmOut2);
-        }
     }
-    if constexpr (PAIR) {            // the peer's barriers must be initialised before anything signals them
-        cluster_arrive();
-        cluster_wait();
-    }
-    if (warp == 1) {
-        if constexpr (PAIR) { tmem_alloc_pair(tmem_slot, 512); tmem_relinquish_pair(); }
-        else { tmem_alloc(tmem_slot, 512); tmem_relinquish(); }
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     // parameter block -> registers while the previous kernel of the stream is still draining
     const KPlan kq(p);
     const TileGeom geo(p);
     const int tiles_n = p.tiles_n;
-    const int pN = p.N;
-    const int64_t pM = p.M, pldo = p.ldo, pldr = p.ldr, prowbias_ld = p.rowbias_ld;
-    const bool staged = (p.splits == 1);
-    const float* const pbias = p.bias;
-    const float* const prowbias = p.rowbias;
-    const __nv_bfloat16* const pres = p.residual;
-    __nv_bfloat16* const pout = p.out;
-    __nv_bfloat16* const pout2 = p.out2;
-    const int64_t pldo2 = p.ldo2;
-    const int n_main = p.n_main;
-    const bool tstore = staged && p.tma_store != 0;
-    float* const pws = p.ws;
-    long long* const ptrace = p.trace;
     pdl_trigger();
     pdl_wait();     // the set-up above overlapped the previous kernel's tail; its results are visible from here on
-    long long* trc = ptrace ? ptrace + (int64_t)blockIdx.x * 16 : nullptr;
-    if (trc && threadIdx.x == 0) { trc[0] = clock64(); unsigned long long g; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g)); trc[7] = (long long)g; }
 
-    if (warp == 0) {
+    if (warp == kGemmMmaThreads / 32) {
         // ===================================== TMA producer =====================================
         if (elect_one()) {
             int stage = 0;
             uint32_t phase = 0;
-            long long tr_first = 0, tr_last = 0, tr_wait = 0, tr_n = 0;      // bring-up trace, kept in registers until the role ends
-            for (int w = worker; w < total_work; w += nworkers) {
+            for (int w = blockIdx.x; w < total_work; w += gridDim.x) {
                 const int split = w / tiles_mn, mn = w % tiles_mn;
-                const int n0 = (mn % tiles_n) * BN + (int)rank * Cfg::B_BOX_ROWS;  // PAIR: this CTA's part of every instruction's B rows
-                TileOrigin o[MSUB];
-#pragma unroll
-                for (int sub = 0; sub < MSUB; ++sub) o[sub] = tile_origin(geo, m_tile_of(mn / tiles_n, sub));
+                const int n0 = (mn % tiles_n) * BN;
+                const TileOrigin o = tile_origin(geo, mn / tiles_n);
                 const int kb_lo = split * kq.kb_per_split, kb_hi = min(kb_lo + kq.kb_per_split, kq.total_kb);
                 KPos q = kq.seek(kb_lo);
                 TapEntry te = p.taps[q.t];
                 for (int it = kb_lo; it < kb_hi; ++it) {
                     const int s = q.s, kb = q.kb;
                     const bool tap_seg = kq.conv && s == 0;
-                    const long long tw0 = trc ? clock64() : 0;
                     mbar_wait(&empty_bar[stage], phase ^ 1);
-                    if (trc) { tr_wait += clock64() - tw0; tr_n += 1; }
+                    void* dA = sA + stage * A_STAGE_BYTES;
                     void* dB = sB + stage * Cfg::B_STAGE_BYTES;
                     const int kcol = (tap_seg ? te.wk_off : 0) + kb * BLOCK_K;
-                    const bool btiled = (kq.btile >> s) & 1;
-                    if constexpr (!PAIR) {
-                        mbar_arrive_expect_tx(&full_bar[stage], Cfg::A_BYTES + Cfg::B_STAGE_BYTES);
-#pragma unroll
-                        for (int sub = 0; sub < MSUB; ++sub) {
-                            void* dA = sA + stage * Cfg::A_BYTES + sub * A_STAGE_BYTES;
-                            if (tap_seg) {
-                                if (kq.conv == 4)
-                                    tma_load_4d(dA, &p.tmA[0], &full_bar[stage], te.c0_off + kb * BLOCK_K, o[sub].w0 + te.dw, o[sub].h0 + te.dh, o[sub].img0);
-                                else
-                                    tma_load_5d(dA, &p.tmA[0], &full_bar[stage], te.c0_off + kb * BLOCK_K, o[sub].w0 + te.dw, te.c2, o[sub].h0 + te.dh,
-                                                o[sub].img0);
-                            } else {
-                                tma_load_2d(dA, &p.tmA[s], &full_bar[stage], kb * BLOCK_K, o[sub].m0);
-                            }
-                        }
-                        if (btiled) tma_load_3d(dB, &p.tmB[s], &full_bar[stage], 0, n0, kcol / BLOCK_K);
-                        else tma_load_2d(dB, &p.tmB[s], &full_bar[stage], kcol, n0);
+                    mbar_arrive_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
+                    if (tap_seg) {
+                        if (kq.conv == 4)
+                            tma_load_4d(dA, &p.tmA[0], &full_bar[stage], te.c0_off + kb * BLOCK_K, o.w0 + te.dw, o.h0 + te.dh, o.img0);
+                        else
+                            tma_load_5d(dA, &p.tmA[0], &full_bar[stage], te.c0_off + kb * BLOCK_K, o.w0 + te.dw, te.c2, o.h0 + te.dh, o.img0);
                     } else {
-                        // every byte of the pair lands on the LEADER's barrier: its one arrival names the bytes of both CTAs
-                        const uint32_t lfull = mapa_u32(smem_u32(&full_bar[stage]), 0);
-                        if (rank == 0) mbar_arrive_expect_tx(&full_bar[stage], 2 * (Cfg::A_BYTES + Cfg::B_STAGE_BYTES));
-#pragma unroll
-                        for (int sub = 0; sub < MSUB; ++sub) {
-                            void* dA = sA + stage * Cfg::A_BYTES + sub * A_STAGE_BYTES;
-                            if (tap_seg) {
-                                if (kq.conv == 4)
-                                    tma_load_4d_pair(dA, &p.tmA[0], lfull, te.c0_off + kb * BLOCK_K, o[sub].w0 + te.dw, o[sub].h0 + te.dh, o[sub].img0);
-                                else
-                                    tma_load_5d_pair(dA, &p.tmA[0], lfull, te.c0_off + kb * BLOCK_K, o[sub].w0 + te.dw, te.c2, o[sub].h0 + te.dh,
-                                                     o[sub].img0);
-                            } else {
-                                tma_load_2d_pair(dA, &p.tmA[s], lfull, kb * BLOCK_K, o[sub].m0);
-                            }
-                        }
-#pragma unroll
-                        for (int h = 0; h < Cfg::NSPLIT; ++h) {
-                            void* dBh = (uint8_t*)dB + h * Cfg::B_BOX_ROWS * 128;
-                            if (btiled) tma_load_3d_pair(dBh, &p.tmB[s], lfull, 0, n0 + h * Cfg::MMA_N, kcol / BLOCK_K);
-                            else tma_load_2d_pair(dBh, &p.tmB[s], lfull, kcol, n0 + h * Cfg::MMA_N);
-                        }
+                        tma_load_2d(dA, &p.tmA[s], &full_bar[stage], kb * BLOCK_K, o.m0);
                     }
-                    if (trc) { tr_last = clock64(); if (tr_first == 0) tr_first = tr_last; }
+                    if ((kq.btile >> s) & 1) tma_load_3d(dB, &p.tmB[s], &full_bar[stage], 0, n0, kcol / BLOCK_K);
+                    else tma_load_2d(dB, &p.tmB[s], &full_bar[stage], kcol, n0);
                     if (++stage == STAGES) { stage = 0; phase ^= 1; }
                     if (kq.advance(q)) te = p.taps[q.t];
                 }
             }
-            if (trc) { trc[1] = tr_first; trc[2] = tr_last; trc[9] = tr_wait; trc[11] = tr_n; }
         }
-    } else if (warp == 1) {
-        // ===================================== MMA issuer (PAIR: the leader CTA only) ========================================
-        if (rank == 0 && elect_one()) {
-            constexpr uint32_t idesc = make_idesc_bf16(BLOCK_M * NCTA, Cfg::MMA_N, 0, 0);
-            int stage = 0;
-            uint32_t phase = 0;
-            int item = 0;
-            long long tr_first = 0, tr_wait = 0, tr_acc = 0, tr_commit = 0;
-            for (int w = worker; w < total_work; w += nworkers, ++item) {
-                const int split = w / tiles_mn;
-                const int kb_lo = split * kq.kb_per_split, kb_hi = min(kb_lo + kq.kb_per_split, kq.total_kb);
-                // DOUBLE_ACC: two accumulators alternate between items; otherwise one item owns all the columns in use
-                const int as = Cfg::DOUBLE_ACC ? (item & 1) : 0;
-                const uint32_t eph = Cfg::DOUBLE_ACC ? ((item >> 1) & 1) : (item & 1);
-                const long long te0 = trc ? clock64() : 0;
-                mbar_wait(&tmem_empty_bar[as], eph ^ 1);                     // epilogue(s) drained this accumulator
-                tc_fence_after();
-                if (trc) tr_acc += clock64() - te0;
-                const uint32_t acc = tmem_base + as * Cfg::ACC_STRIDE;
-                uint32_t accum = 0;
-                KPos q = kq.seek(kb_lo);
-                for (int it = kb_lo; it < kb_hi; ++it) {
-                    const long long tw0 = trc ? clock64() : 0;
-                    mbar_wait(&full_bar[stage], phase);
-                    tc_fence_after();
-                    if (trc) { const long long tn = clock64(); tr_wait += tn - tw0; if (tr_first == 0) tr_first = tn; }
-                    const uint64_t adesc = make_smem_desc(smem_u32(sA + stage * Cfg::A_BYTES), 16, 1024);
-                    const uint64_t bdesc = make_smem_desc(smem_u32(sB + stage * Cfg::B_STAGE_BYTES), 16, 1024);
-                    const int ksteps = (q.kb == q.nkb_s - 1) ? kq.klast(q.s) : (BLOCK_K / 16);
-                    for (int k = 0; k < ksteps; ++k) {
-                        // +32 bytes (= 2 in descriptor units) per 16-element k-step inside the swizzle atom
-#pragma unroll
-                        for (int sub = 0; sub < MSUB; ++sub) {   // the M sub-tiles share the B operand of this k-step
-                            if constexpr (PAIR) {
-#pragma unroll
-                                for (int h = 0; h < Cfg::NSPLIT; ++h)
-                                    umma_ss_pair(acc + sub * Cfg::ACC_STRIDE + h * Cfg::MMA_N, adesc + sub * (A_STAGE_BYTES >> 4) + 2 * k,
-                                                 bdesc + h * ((Cfg::B_BOX_ROWS * 128) >> 4) + 2 * k, idesc, accum);
-                            } else {
-                                umma_ss(acc + sub * Cfg::ACC_STRIDE, adesc + sub * (A_STAGE_BYTES >> 4) + 2 * k, bdesc + 2 * k, idesc, accum);
-                            }
-                        }
-                        accum = 1;
-                    }
-                    // frees the smem slot (in both CTAs of a pair) when these MMAs retire
-                    if constexpr (PAIR) umma_commit_pair(&empty_bar[stage], 0b11);
-                    else umma_commit(&empty_bar[stage]);
-                    if (++stage == STAGES) { stage = 0; phase ^= 1; }
-                    kq.advance(q);
-                }
-                if constexpr (PAIR) umma_commit_pair(&tmem_full_bar[as], 0b11);
-                else umma_commit(&tmem_full_bar[as]);
-                if (trc) tr_commit = clock64();
-            }
-            if (trc) { trc[3] = tr_first; trc[4] = tr_commit; trc[8] = tr_wait; trc[10] = tr_acc; }
-        }
-    } else {
-        // ===================================== epilogue ==========================================
-        // Every shared-memory access below is an explicit ld.shared / st.shared on a 32-bit shared address: the staging pointers
-        // are derived from the aligned dynamic-smem base through integer arithmetic, which makes nvcc fall back to GENERIC loads
-        // and stores, and the r01 code had one branch per 8-column group -- together 2 600 cycles to convert one 128x160 part and
-        // 2 000 (GEMM) / 5 100 (convolution: four integer divisions per 16-byte unit) to store it (profiles/r02_probe_trace_c.txt):
-        // the K = 320 GEMMs of the 64x64 level were bound by this epilogue, not by their main loop.
-        constexpr int EBN = Cfg::EBN;
-        const int quarter = warp & 3;                 // TMEM lane quarter this warp may access
-        const int half = (warp - 2) >> 2;             // which half of the part's columns this warp converts
-        const int r = quarter * 32 + lane;            // row inside the tile
-        const int et = threadIdx.x - 64;              // 0..255 among the epilogue threads
-        constexpr int UNITS = EBN / 8;                // 16-byte units per staged row
-        constexpr int CH16 = EBN / 16;                // 16-column TMEM chunks per part
-        constexpr int NCH = Cfg::EPI_NCH;             // chunks per column half
-        const uint32_t stg = smem_u32(sStg), sbias = smem_u32(sBias), srow = smem_u32(sRow);
-        const uint32_t my_stg = stg + r * Cfg::STG_PITCH;
-        const int N = pN;
-        const int64_t Mrows = pM;
-        const bool has_bias = staged && pbias != nullptr, has_res = staged && pres != nullptr;
-        const float* const rowbias = staged ? prowbias : nullptr;
-        const int64_t rowbias_ld = prowbias_ld;
-        // TMA-store layout of the staging buffer: one dense [128 rows x 32 B] box per 16-column chunk (the padded row layout is
-        // kept for the manual store loop).  `pending`: a TMA store of the previous part may still be reading the buffer.
-        auto unit_addr = [&](int rr, int cu) -> uint32_t {
-            return tstore ? stg + (cu >> 1) * 4096 + rr * 32 + (cu & 1) * 16 : stg + rr * Cfg::STG_PITCH + cu * 16;
-        };
-        bool pending = false;
-        auto staging_acquire = [&]() {
-            if (pending) {
-                if (lane == 0) bulk_wait_read0();
-                asm volatile("bar.sync 1, 256;" ::: "memory");
-                pending = false;
-            }
-        };
-        int item = 0;
-        for (int w = worker; w < total_work; w += nworkers, ++item) {
-            const int split = w / tiles_mn, mn = w % tiles_mn;
-            const int n0 = (mn % tiles_n) * BN;
-            const int as = Cfg::DOUBLE_ACC ? (item & 1) : 0;
-            const uint32_t fph = Cfg::DOUBLE_ACC ? ((item >> 1) & 1) : (item & 1);
-            if (has_bias) {
-                // the bias slice of this item's columns goes to shared memory once; the previous item's trailing bar.sync guarantees
-                // nobody still reads the old slice.  Columns >= N read as zero.
-                for (int c = et; c < BN / 4; c += kGemmEpiThreads)
-                    sts_f4(sbias + c * 16, (n0 + c * 4 < n_main) ? *reinterpret_cast<const float4*>(pbias + n0 + c * 4) : make_float4(0.f, 0.f, 0.f, 0.f));
-            }
-#pragma unroll 1
-            for (int part = 0; part < MSUB * Cfg::NPART; ++part) {
-                const int sub = part / Cfg::NPART;
-                const int nc0 = (part % Cfg::NPART) * EBN;          // first column of this part inside the item's BN columns
-                const bool last_part = (part == MSUB * Cfg::NPART - 1);
-                const bool dbg = trc && et == 0 && item == 0 && part == 0;
-                int group = 0;
-                int64_t grow = -1;
-                if (nc0 == 0) {
-                    // row of `out` behind every tile row, once per M sub-tile (the store loops below read it back instead of redoing the
-                    // integer divisions of the pixel <-> row mapping for every 16-byte unit); -1 = row beyond M
-                    const TileOrigin o = tile_origin(geo, m_tile_of(mn / tiles_n, sub));
-                    grow = tile_row(geo, o, r, group);
-                    if (grow >= Mrows) grow = -1;
-                    if (half == 0) { sts_b64(srow + r * 16, grow); sts_b64(srow + r * 16 + 8, (int64_t)group); }
-                }
-                if (has_res) {
-                    // coalesced prefetch of the residual tile into the staging buffer (overlaps the main loop).  All loads of a thread
-                    // are issued before the first store: one L2 round trip per tile instead of one per 16-byte unit.
-                    if (nc0 == 0) asm volatile("bar.sync 1, 256;" ::: "memory");          // row table visible
-                    constexpr int NRES = (BLOCK_M * UNITS + kGemmEpiThreads - 1) / kGemmEpiThreads;
-                    uint4 rbuf[NRES];
-#pragma unroll
-                    for (int it = 0; it < NRES; ++it) {
-                        const int u = et + it * kGemmEpiThreads;
-                        const int rr = u / UNITS, cu = u % UNITS;
-                        rbuf[it] = make_uint4(0u, 0u, 0u, 0u);
-                        if (u < BLOCK_M * UNITS) {
-                            const int64_t g = lds_b64(srow + rr * 16);
-                            const int col = n0 + nc0 + cu * 8;
-                            if (g >= 0 && col < n_main) rbuf[it] = *reinterpret_cast<const uint4*>(pres + g * pldr + col);
-                        }
-                    }
-                    staging_acquire();
-#pragma unroll
-                    for (int it = 0; it < NRES; ++it) {
-                        const int u = et + it * kGemmEpiThreads;
-                        if (u < BLOCK_M * UNITS) sts128(unit_addr(u / UNITS, u % UNITS), rbuf[it]);
-                    }
-                }
-                if (has_res || has_bias || nc0 == 0) asm volatile("bar.sync 1, 256;" ::: "memory");      // residual / bias / row table staged
-                if (nc0 != 0) {             // later column parts of the same rows: this thread's row comes back from the table
-                    grow = lds_b64(srow + r * 16);
-                    group = (int)lds_b64(srow + r * 16 + 8);
-                }
-                const bool row_ok = grow >= 0;
-                if (part == 0) mbar_wait(&tmem_full_bar[as], fph);
-                tc_fence_after();
-                if (trc && et == 0 && trc[5] == 0) trc[5] = clock64();
-                const int acc_idx = Cfg::DOUBLE_ACC ? as : sub;
-                const uint32_t trow = tmem_base + acc_idx * Cfg::ACC_STRIDE + nc0 + (static_cast<uint32_t>(quarter * 32) << 16);
-                // all TMEM chunks of this thread are pulled into registers with ONE wait and the accumulator goes back to the MMA warp
-                // before any arithmetic (PAIR: one elected lane per warp tells the LEADER's barrier -- a remote arrive for the peer CTA)
-                uint32_t vv[NCH][16];
-#pragma unroll
-                for (int cl = 0; cl < NCH; ++cl)
-                    if (half * NCH + cl < CH16) tmem_ld16(trow + (half * NCH + cl) * 16, vv[cl]);
-                tmem_wait_ld();
-                if (dbg) trc[12] = clock64();
-                if (last_part) {
-                    tc_fence_before();
-                    if constexpr (PAIR) {
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive_cluster(mapa_u32(smem_u32(&tmem_empty_bar[as]), 0));
-                    } else {
-                        mbar_arrive(&tmem_empty_bar[as]);
-                    }
-                }
-                if (staged) {
-                    staging_acquire();
-                    // bias + per-image row bias + residual -> bf16 -> this thread's row of the staging buffer; no branches: columns >= N
-                    // carry zeros (TMA zero fill, zeroed bias / residual slots) and are masked by the store loop
-                    const float* rb = (rowbias && row_ok) ? rowbias + (int64_t)group * rowbias_ld + n0 + nc0 : nullptr;
-#pragma unroll
-                    for (int cl = 0; cl < NCH; ++cl) {
-                        const int c = half * NCH + cl;
-                        if (c < CH16) {
-#pragma unroll
-                            for (int g = 0; g < 2; ++g) {
-                                const int cc = c * 16 + g * 8;                 // first column of the group inside the part
-                                float f[8];
-#pragma unroll
-                                for (int j = 0; j < 8; ++j) f[j] = __uint_as_float(vv[cl][g * 8 + j]);
-                                if (has_bias) {
-                                    const float4 b0 = lds_f4(sbias + (nc0 + cc) * 4), b1 = lds_f4(sbias + (nc0 + cc) * 4 + 16);
-                                    f[0] += b0.x; f[1] += b0.y; f[2] += b0.z; f[3] += b0.w;
-                                    f[4] += b1.x; f[5] += b1.y; f[6] += b1.z; f[7] += b1.w;
-                                }
-                                if (rb && n0 + nc0 + cc < n_main) {
-                                    const float4 b0 = __ldg(reinterpret_cast<const float4*>(rb + cc)), b1 = __ldg(reinterpret_cast<const float4*>(rb + cc + 4));
-                                    f[0] += b0.x; f[1] += b0.y; f[2] += b0.z; f[3] += b0.w;
-                                    f[4] += b1.x; f[5] += b1.y; f[6] += b1.z; f[7] += b1.w;
-                                }
-                                const uint32_t slot = unit_addr(r, c * 2 + g);
-                                if (has_res) {
-                                    const uint4 rv = lds128(slot);
-                                    float2 t;
-                                    t = unpack_bf16x2(rv.x); f[0] += t.x; f[1] += t.y;
-                                    t = unpack_bf16x2(rv.y); f[2] += t.x; f[3] += t.y;
-                                    t = unpack_bf16x2(rv.z); f[4] += t.x; f[5] += t.y;
-                                    t = unpack_bf16x2(rv.w); f[6] += t.x; f[7] += t.y;
-                                }
-                                sts128(slot, make_uint4(pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]), pack_bf16x2(f[4], f[5]), pack_bf16x2(f[6], f[7])));
-                            }
-                        }
-                    }
-                    if (dbg) trc[13] = clock64();
-                    if (tstore) {
-                        // the part leaves through the TMA unit: one box store per 16-column chunk (rows / columns beyond the tensor are
-                        // clipped by the map), issued by one thread; the buffer is re-acquired lazily (staging_acquire)
-                        fence_proxy_async_smem();
-                        asm volatile("bar.sync 1, 256;" ::: "memory");
-                        if (dbg) trc[14] = clock64();
-                        if (lane == 0) {                                            // one issuing lane per epilogue warp: 8 short streams
-                            const int row0 = (int)lds_b64(srow);                    // row of `out` behind tile row 0
-#pragma unroll 1
-                            for (int c = warp - 2; c < CH16; c += kGemmEpiThreads / 32) {
-                                const int col = n0 + nc0 + c * 16;
-                                if (col >= N) break;
-                                if (col < n_main) tma_store_2d(&p.tmOut, nullptr, stg + c * 4096, col, row0);
-                                else tma_store_2d(&p.tmOut2, nullptr, stg + c * 4096, col - n_main, row0);
-                            }
-                            bulk_commit_group();
-                        }
-                        pending = true;
-                        if (dbg) trc[15] = clock64();
-                        continue;
-                    }
-                    asm volatile("bar.sync 1, 256;" ::: "memory");
-                    if (dbg) trc[14] = clock64();
-                    if (n0 + nc0 + EBN <= n_main) {                                   // (uniform) the usual case: one output
-                        for (int u = et; u < BLOCK_M * UNITS; u += kGemmEpiThreads) {     // coalesced 16-byte stores
-                            const int rr = u / UNITS, cu = u % UNITS;
-                            const int64_t g = lds_b64(srow + rr * 16);
-                            if (g >= 0) *reinterpret_cast<uint4*>(pout + g * pldo + (n0 + nc0 + cu * 8)) = lds128(stg + rr * Cfg::STG_PITCH + cu * 16);
-                        }
-                    } else {                                                          // N tail and / or the second output
-                        for (int u = et; u < BLOCK_M * UNITS; u += kGemmEpiThreads) {
-                            const int rr = u / UNITS, cu = u % UNITS;
-                            const int64_t g = lds_b64(srow + rr * 16);
-                            const int col = n0 + nc0 + cu * 8;
-                            if (g >= 0 && col < N) {
-                                __nv_bfloat16* dst = (col < n_main) ? pout + g * pldo + col : pout2 + g * pldo2 + (col - n_main);
-                                *reinterpret_cast<uint4*>(dst) = lds128(stg + rr * Cfg::STG_PITCH + cu * 16);
-                            }
-                        }
-                    }
-                    asm volatile("bar.sync 1, 256;" ::: "memory");     // staging buffer / row table reusable
-                    if (dbg) trc[15] = clock64();
-                } else {
-                    // split-K partials (raw fp32; bias / residual are applied by splitk_finalize_kernel).  The fp32 values of one column
-                    // HALF of the part fill the staging buffer exactly (NCH * 64 + 16 bytes per row = the bf16 pitch), so the two halves
-                    // take turns: park, then all 256 threads write whole 16-byte units of consecutive columns.
-                    static_assert(NCH * 64 + 16 <= Cfg::STG_PITCH, "fp32 half part must fit the staging row");
-                    constexpr int FU = NCH * 4;                       // float4 units per staged row
-#pragma unroll 1
-                    for (int hp = 0; hp < 2; ++hp) {
-                        if (half == hp) {
-#pragma unroll
-                            for (int cl = 0; cl < NCH; ++cl)
-                                if (hp * NCH + cl < CH16) {
-#pragma unroll
-                                    for (int j = 0; j < 4; ++j)
-                                        sts128(my_stg + cl * 64 + j * 16, make_uint4(vv[cl][4 * j], vv[cl][4 * j + 1], vv[cl][4 * j + 2], vv[cl][4 * j + 3]));
-                                }
-                        }
-                        asm volatile("bar.sync 1, 256;" ::: "memory");
-                        const int ncols_h = min(CH16 - hp * NCH, NCH) * 16;           // columns this half holds
-                        for (int u = et; u < BLOCK_M * FU; u += kGemmEpiThreads) {
-                            const int rr = u / FU, cu = u % FU;
-                            const int64_t g = lds_b64(srow + rr * 16);
-                            const int col = n0 + nc0 + hp * NCH * 16 + cu * 4;
-                            if (cu * 4 < ncols_h && g >= 0 && col < N)
-                                *reinterpret_cast<uint4*>(pws + ((int64_t)split * Mrows + g) * N + col) = lds128(stg + rr * Cfg::STG_PITCH + cu * 16);
-                        }
-                        asm volatile("bar.sync 1, 256;" ::: "memory");
-                    }
-                }
-            }   // part
-        }
-        if (pending && lane == 0) bulk_wait_read0();    // the last stores have left shared memory before the CTA may exit
+        return;
     }
 
-    if (trc && threadIdx.x == 64) trc[6] = clock64();
-    tc_fence_before();
-    if constexpr (PAIR) {            // neither CTA frees TMEM / exits while the peer may still touch the pair's state
-        cluster_arrive();
-        cluster_wait();
-    } else {
-        __syncthreads();
-    }
-    if (warp == 1) {
-        if constexpr (PAIR) tmem_dealloc_pair(tmem_base, 512);
-        else tmem_dealloc(tmem_base, 512);
+    // ===================================== MMA warpgroups + epilogue =====================================
+    const int wg = warp >> 2;                     // rows [64 wg, 64 wg + 64) of the tile
+    const int r_lo = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // accumulator rows of this thread: r_lo and r_lo + 8
+    const int cq = 2 * (lane & 3);                       // first of the two adjacent columns per 8-column group
+    const int N = p.N, n_main = p.n_main;
+    const int64_t Mrows = p.M, ldo = p.ldo, ldr = p.ldr, ldo2 = p.ldo2, rowbias_ld = p.rowbias_ld;
+    const float* const bias = p.bias;
+    const float* const rowbias = p.rowbias;
+    const __nv_bfloat16* const res = p.residual;
+    __nv_bfloat16* const out = p.out;
+    __nv_bfloat16* const out2 = p.out2;
+    float* const ws = p.ws;
+    const bool split_k = p.splits > 1;
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int w = blockIdx.x; w < total_work; w += gridDim.x) {
+        const int split = w / tiles_mn, mn = w % tiles_mn;
+        const int n0 = (mn % tiles_n) * BN;
+        const int kb_lo = split * kq.kb_per_split, kb_hi = min(kb_lo + kq.kb_per_split, kq.total_kb);
+        float acc[BN / 2];
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+        KPos q = kq.seek(kb_lo);
+        int held = -1;                                   // stage whose operands the wgmma group in flight still reads
+        for (int it = kb_lo; it < kb_hi; ++it) {
+            mbar_wait(&full_bar[stage], phase);
+            const uint64_t adesc = make_smem_desc(smem_u32(sA + stage * A_STAGE_BYTES + wg * 64 * 128), 16, 1024);
+            const uint64_t bdesc = make_smem_desc(smem_u32(sB + stage * Cfg::B_STAGE_BYTES), 16, 1024);
+            const int ksteps = (q.kb == q.nkb_s - 1) ? kq.klast(q.s) : (BLOCK_K / 16);
+            wgmma_fence();
+            // +32 bytes (= 2 in descriptor units) per 16-element k-step inside the swizzle atom
+            wgmma_ss<BN, 0, 0>(acc, adesc, bdesc, 1u);
+            for (int k = 1; k < ksteps; ++k) wgmma_ss<BN, 0, 0>(acc, desc_adv(adesc, 2 * k), desc_adv(bdesc, 2 * k), 1u);
+            wgmma_commit();
+            wgmma_wait<1>();                             // the previous k-block's group has retired: its stage goes back to the producer
+            if (held >= 0) mbar_arrive(&empty_bar[held]);
+            held = stage;
+            if (++stage == STAGES) { stage = 0; phase ^= 1; }
+            kq.advance(q);
+        }
+        wgmma_wait<0>();
+        wgmma_fence_acc(acc);
+        if (held >= 0) mbar_arrive(&empty_bar[held]);
+
+        // rows of `out` behind this thread's two accumulator rows (-1: beyond M)
+        const TileOrigin o = tile_origin(geo, mn / tiles_n);
+        int64_t grow[2];
+        int group[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            grow[h] = tile_row(geo, o, r_lo + 8 * h, group[h]);
+            if (grow[h] >= Mrows) grow[h] = -1;
+        }
+        if (split_k) {
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) {
+                const int col = n0 + 8 * j + cq;
+                if (col >= N) continue;
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+                    if (grow[h] >= 0)
+                        *reinterpret_cast<float2*>(ws + ((int64_t)split * Mrows + grow[h]) * N + col) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+            }
+            continue;
+        }
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+            const int col = n0 + 8 * j + cq;
+            if (col >= N) continue;
+            if (col < n_main) {
+                float b0 = 0.f, b1 = 0.f;
+                if (bias) { b0 = __ldg(bias + col); b1 = __ldg(bias + col + 1); }
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    if (grow[h] < 0) continue;
+                    float f0 = acc[4 * j + 2 * h] + b0, f1 = acc[4 * j + 2 * h + 1] + b1;
+                    if (rowbias) {
+                        const float* rb = rowbias + (int64_t)group[h] * rowbias_ld + col;
+                        f0 += __ldg(rb); f1 += __ldg(rb + 1);
+                    }
+                    if (res) {
+                        const float2 t = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(res + grow[h] * ldr + col));
+                        f0 += t.x; f1 += t.y;
+                    }
+                    *reinterpret_cast<uint32_t*>(out + grow[h] * ldo + col) = pack_bf16x2(f0, f1);
+                }
+            } else {
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+                    if (grow[h] >= 0)
+                        *reinterpret_cast<uint32_t*>(out2 + grow[h] * ldo2 + (col - n_main)) = pack_bf16x2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+            }
+        }
     }
 }
 
@@ -716,12 +397,13 @@ __global__ void splitk_finalize_kernel(const float* __restrict__ ws, int splits,
 static int plan_splits(int64_t ctas, int64_t total_kb, int64_t N) {
     // splitting costs a second (finalize) launch and an fp32 round trip: never for the skinny LoRA projections or short reductions
     if (total_kb < 8 || N <= 64) return 1;
-    if (ctas >= 48) {
-        // 48..74 output tiles leave half of the 148 SMs idle for the whole reduction: two K halves fill them, worth it when each
-        // half is still a long main loop (>= 20 k-blocks): the 16x16 / 8x8 level convolutions and the K >= 2560 linears at M = 1024
-        return (ctas <= 74 && total_kb >= 40) ? 2 : 1;
+    const int64_t sms = num_sms();
+    if (ctas >= sms / 3) {
+        // a third to a half of the SMs busy for the whole reduction: two K halves fill them, worth it when each half is still a long
+        // main loop (>= 20 k-blocks): the 16x16 / 8x8 level convolutions and the K >= 2560 linears at M = 1024
+        return (ctas <= sms / 2 && total_kb >= 40) ? 2 : 1;
     }
-    int64_t s = 148 / ctas;                 // persistent grid: keep the work items within one wave of 148 SMs
+    int64_t s = sms / ctas;                 // persistent grid: keep the work items within one wave of SMs
     if (s > total_kb / 4) s = total_kb / 4;
     if (s > 16) s = 16;
     return s < 2 ? 1 : (int)s;
@@ -731,11 +413,11 @@ static int plan_splits(int64_t ctas, int64_t total_kb, int64_t N) {
 // LoRA gradients on the tensor pipe:  D[n, j] = sum_m X[m, n] * S[m, j]   (reduction over the M token rows)
 //   dW_down[j, k] = sum_m U[m, c0+j] x[m, k]          S = U = dY . (alpha B),  X = x
 //   dW_up[o, j]   = alpha * sum_m dY[m, o0+o] T[m, c0+j]   S = T = x . A^T,        X = dY
-// Both operands are read straight from their row-major [M, *] tensors as MN-major UMMA operands (TMA boxes of 64 columns x
-// 128 rows), so no transpose ever exists.  One CTA owns 128 columns of X and a slice of the rows (split-K); the 128 x 64
-// fp32 accumulator is reduced into the flat gradient buffer with red.global.
+// Both operands are read straight from their row-major [M, *] tensors as MN-major wgmma operands (TMA boxes of 64 columns x
+// 128 rows), so no transpose ever exists.  One CTA owns 128 columns of X and a slice of the rows (split-K); MMA warpgroup g
+// accumulates the 64 x 64 fp32 block of X columns [64g, 64g+64) and reduces it into the flat gradient buffer with atomics.
 // =============================================================================================
-constexpr int kLgThreads = 192;   // warp 0: TMA, warp 1: MMA, warps 2-5: reduction epilogue
+constexpr int kLgThreads = 288;   // warps 0-7: two MMA warpgroups, warp 8: TMA
 constexpr int LG_STAGES = 3;
 constexpr int LG_STAGE_BYTES = 3 * 128 * 128;      // two X boxes + one S box
 constexpr int LG_SMEM_BYTES = LG_STAGES * LG_STAGE_BYTES + 256 + 1024;
@@ -769,15 +451,12 @@ __global__ void __launch_bounds__(kLgThreads, 1) lora_grad_tc_kernel(const __gri
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + LG_STAGES * LG_STAGE_BYTES);
     uint64_t* empty_bar = full_bar + LG_STAGES;
-    uint64_t* tmem_full_bar = empty_bar + LG_STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = warp_id_uniform(), lane = threadIdx.x & 31;
     // flat grid over (problem, column chunk, row split)
     int bid = blockIdx.x, z = 0;
     if (p.nprob == 2 && bid >= p.prob[0].col_chunks * p.prob[0].splits) { bid -= p.prob[0].col_chunks * p.prob[0].splits; z = 1; }
-    // The reduction epilogue walks `p.prob[z].blk[b]` with run-time z and b -- chains of dynamically indexed constant-bank loads
-    // (~200 cycles each, 119 of them in the r01 SASS).  The epilogue warps copy the descriptor to shared memory while the main
-    // loop runs (below); the producer / MMA threads only need the three scalars read here.
+    // The reduction epilogue walks `p.prob[z].blk[b]` with run-time z and b (dynamically indexed constant-bank loads): the MMA
+    // threads copy the descriptor to shared memory first; the producer only needs the scalars read here.
     __shared__ LGProblem sq;
     const LGProblem& q = z ? p.prob[1] : p.prob[0];
     const CUtensorMap* tmX = z ? &p.tmX[1] : &p.tmX[0];
@@ -788,19 +467,14 @@ __global__ void __launch_bounds__(kLgThreads, 1) lora_grad_tc_kernel(const __gri
     const int t1 = min(total_tiles, t0 + q.tiles_per_cta);
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < LG_STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        mbar_init(tmem_full_bar, 1);
+        for (int s = 0; s < LG_STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 256); }
         fence_mbar_init();
     }
-    if (warp == 1) { tmem_alloc(tmem_slot, 64); tmem_relinquish(); }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     pdl_trigger();
     pdl_wait();
 
-    if (warp == 0) {
+    if (warp == 8) {
         if (elect_one()) {
             int stage = 0; uint32_t phase = 0;
             for (int t = t0; t < t1; ++t) {
@@ -831,88 +505,73 @@ __global__ void __launch_bounds__(kLgThreads, 1) lora_grad_tc_kernel(const __gri
                 if (++stage == LG_STAGES) { stage = 0; phase ^= 1; }
             }
         }
-    } else if (warp == 1) {
-        if (elect_one()) {
-            constexpr uint32_t idesc = make_idesc_bf16(128, 64, 1, 1);     // A (X^T) and B (S^T) both MN-major
-            int stage = 0; uint32_t phase = 0; uint32_t accum = 0;
-            for (int t = t0; t < t1; ++t) {
-                mbar_wait(&full_bar[stage], phase);
-                tc_fence_after();
-                const uint32_t xb = smem_u32(smem + stage * LG_STAGE_BYTES);
-                const uint32_t sb = xb + 2 * 128 * 128;
-                for (int ks = 0; ks < 8; ++ks) {                         // 16 token rows per k-step = 2048 B
-                    umma_ss(tmem_base, make_smem_desc(xb + ks * 2048, 128 * 128, 1024), make_smem_desc(sb + ks * 2048, 128 * 128, 1024),
-                            idesc, accum);
-                    accum = 1;
-                }
-                umma_commit(&empty_bar[stage]);
-                if (++stage == LG_STAGES) { stage = 0; phase ^= 1; }
-            }
-            umma_commit(tmem_full_bar);
-        }
-    } else {
-        {   // descriptor -> shared memory by the 128 epilogue threads, hidden behind the main loop
-            const uint32_t* src = reinterpret_cast<const uint32_t*>(&q);
-            uint32_t* dst = reinterpret_cast<uint32_t*>(&sq);
-            for (int i = threadIdx.x - 64; i < (int)(sizeof(LGProblem) / 4); i += 128) dst[i] = src[i];
-            asm volatile("bar.sync 1, 128;" ::: "memory");
-        }
-        const LGProblem& q = sq;                                         // (shadows the constant-bank reference)
-        const int quarter = warp & 3;
-        const int n = ncol0 + quarter * 32 + lane;                       // this thread's column of X
-        mbar_wait(tmem_full_bar, 0);
-        tc_fence_after();
-        const uint32_t trow = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16);
-#pragma unroll 1
-        for (int c = 0; c < 4; ++c) {
-            uint32_t v[16];
-            tmem_ld16(trow + c * 16, v);
-            tmem_wait_ld();
-            if (t1 > t0 && n < q.n_end) {
-                for (int b = 0; b < q.nblocks; ++b) {
-                    const LGBlock& k = q.blk[b];
-                    if (n < k.n_lo || n >= k.n_hi) continue;
+        return;
+    }
+    {   // descriptor -> shared memory
+        const uint32_t* src = reinterpret_cast<const uint32_t*>(&q);
+        uint32_t* dst = reinterpret_cast<uint32_t*>(&sq);
+        for (int i = threadIdx.x; i < (int)(sizeof(LGProblem) / 4); i += 256) dst[i] = src[i];
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+    }
+    const int wg = warp >> 2;
+    float acc[32];
 #pragma unroll
-                    for (int e = 0; e < 16; ++e) {
-                        const int j = c * 16 + e - k.c0;
-                        if (j >= 0 && j < k.rank) {
-                            const float val = __uint_as_float(v[e]) * k.scale;
-                            float* dst = k.transpose_out ? k.dst + (int64_t)(n - k.n_lo) * k.dst_ld + j
-                                                         : k.dst + (int64_t)j * k.dst_ld + (int64_t)(n - k.n_lo) * k.n_stride;
-                            atomicAdd(dst, val);
-                        }
-                    }
+    for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+    int stage = 0; uint32_t phase = 0;
+    for (int t = t0; t < t1; ++t) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t xb = smem_u32(smem + stage * LG_STAGE_BYTES) + wg * 128 * 128;   // this warpgroup's 64 X columns
+        const uint32_t sb = smem_u32(smem + stage * LG_STAGE_BYTES) + 2 * 128 * 128;
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < 8; ++ks)                                   // 16 token rows per k-step = 2048 B
+            wgmma_ss<64, 1, 1>(acc, make_smem_desc(xb + ks * 2048, 128 * 128, 1024), make_smem_desc(sb + ks * 2048, 128 * 128, 1024), 1u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        mbar_arrive(&empty_bar[stage]);
+        if (++stage == LG_STAGES) { stage = 0; phase ^= 1; }
+    }
+    wgmma_fence_acc(acc);
+    if (t1 <= t0) return;
+    const LGProblem& qs = sq;
+    const int n_lo_row = ncol0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int n = n_lo_row + 8 * h;                                  // column of X
+        if (n >= qs.n_end) continue;
+        for (int b = 0; b < qs.nblocks; ++b) {
+            const LGBlock& k = qs.blk[b];
+            if (n < k.n_lo || n >= k.n_hi) continue;
+#pragma unroll
+            for (int i = 0; i < 16; ++i) {
+                const int jj = 8 * (i >> 1) + 2 * (lane & 3) + (i & 1);   // column of S
+                const int j = jj - k.c0;
+                if (j >= 0 && j < k.rank) {
+                    const float val = acc[4 * (i >> 1) + 2 * h + (i & 1)] * k.scale;
+                    float* dst = k.transpose_out ? k.dst + (int64_t)(n - k.n_lo) * k.dst_ld + j
+                                                 : k.dst + (int64_t)j * k.dst_ld + (int64_t)(n - k.n_lo) * k.n_stride;
+                    atomicAdd(dst, val);
                 }
             }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, 64);
 }
 
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
-template <int BN, int MSUB, bool PAIR>
+template <int BN>
 static int launch_gemm(const GemmKParams& kp, cudaStream_t stream) {
-    using Cfg = GemmCfg<BN, MSUB, PAIR>;
+    using Cfg = GemmCfg<BN>;
     static bool configured = false;
-    static int num_sms = 148;
     if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(gemm_tc_kernel<BN, MSUB, PAIR>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             Cfg::SMEM_BYTES);
+        cudaError_t e = cudaFuncSetAttribute(gemm_wgmma_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
         if (e != cudaSuccess) return set_cuda_error(e, "cudaFuncSetAttribute(gemm)");
-        int dev = 0;
-        if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
         configured = true;
     }
-    constexpr int NCTA = PAIR ? 2 : 1;
-    const int total = kp.tiles_n * ((kp.tiles_m + MSUB * NCTA - 1) / (MSUB * NCTA)) * kp.splits;
-    const int workers = num_sms / NCTA;
-    dim3 grid((total < workers ? total : workers) * NCTA);
-    if (PAIR) launch_k_cluster(gemm_tc_kernel<BN, MSUB, PAIR>, dim3(grid), dim3(kGemmThreads), Cfg::SMEM_BYTES, stream, 2u, kp);
-    else launch_k(gemm_tc_kernel<BN, MSUB, PAIR>, dim3(grid), dim3(kGemmThreads), Cfg::SMEM_BYTES, stream, kp);
+    const int total = kp.tiles_n * kp.tiles_m * kp.splits;
+    const int workers = num_sms();
+    launch_k(gemm_wgmma_kernel<BN>, dim3(total < workers ? total : workers), dim3(kGemmThreads), Cfg::SMEM_BYTES, stream, kp);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return set_cuda_error(e, "gemm launch");
     return HCP_OK;
@@ -934,88 +593,21 @@ static int pick_bn(int64_t N) {
     return best;
 }
 
-// CTA-pair tiling (256 x BN per pair, BN in {256, 320}) and its K-split.  bn == 0: keep the single-CTA kernel.
-//   * plenty of 256-row work items for the 74 pairs (whole waves: a part-filled last wave costs a full main loop): no split;
-//   * FEW items but a long reduction (the 16x16 / 8x8 levels: M = 1024 / 256 rows against 1280..2560-channel weights -- pure weight
-//     streaming): the reduction is cut so that items x splits fill one wave of pairs.  A pair streams every weight byte ONCE for its
-//     256 rows where two single CTAs each stream all of it, which halves the L2 -> SM traffic these launches are bound by.
-// BN = 256 (two accumulators: epilogue of item i under the main loop of i + 1) when it divides N, else 320 (one accumulator).
-struct PairPlan {
-    int bn, splits;
-};
-static PairPlan plan_pair(int64_t N, int64_t m_tiles, int64_t total_kb, bool allow_split) {
-    static const int mode = [] { const char* e = getenv("HCP_GEMM_PAIR"); return e ? atoi(e) : 1; }();
-    static const int min_kb = [] { const char* e = getenv("HCP_PAIR_MIN_KB"); return e ? atoi(e) : 10; }();
-    static const int split_min_kb = [] { const char* e = getenv("HCP_PAIR_SPLIT_MIN_KB"); return e ? atoi(e) : 40; }();
-    PairPlan none{0, 1};
-    if (mode == 0 || total_kb < min_kb || N < 256) return none;
-    const int bn = (N % 256 == 0 && getenv("HCP_PAIR_NO256") == nullptr) ? 256 : (N % 320 == 0) ? 320 : 0;
-    if (!bn) return none;
-    const int64_t items = ((m_tiles + 1) / 2) * (N / bn);
-    if (mode == 2) return PairPlan{bn, 1};                      // forced (bring-up / A-B runs)
-    const int64_t waves = (items + 73) / 74;
-    const double fill = (double)items / (double)(waves * 74);
-    if (items >= 56 && fill >= 0.75) return PairPlan{bn, 1};
-    if (allow_split && mode != 3 && items <= 37 && total_kb >= split_min_kb) {
-        int64_t s = 74 / items;
-        if (s > total_kb / 8) s = total_kb / 8;                 // at least 8 k-blocks per item
-        if (s > 16) s = 16;
-        if (s >= 2) return PairPlan{bn, (int)s};
-    }
-    return none;
-}
-
-static long long* g_gemm_trace = nullptr;
-
-static int dispatch_gemm(int bn, bool cta_pair, GemmKParams& kp, int m_tiles, cudaStream_t stream) {
+static int dispatch_gemm(int bn, GemmKParams& kp, int m_tiles, cudaStream_t stream) {
     kp.tiles_m = m_tiles;
-    kp.trace = g_gemm_trace;
-    if (cta_pair) {
-        if (bn == 320) return launch_gemm<320, 1, true>(kp, stream);
-        if (bn == 256) return launch_gemm<256, 1, true>(kp, stream);
-        return set_error(HCP_ERR_INVALID, "unsupported CTA-pair BLOCK_N");
-    }
-    // two M tiles per work item when the reduction is long (operand-stream bound) and there are plenty of tiles
-    int64_t total_kb = 0;
-    for (int s = 0; s < kp.nseg; ++s) total_kb += (int64_t)kp.nkb[s] * ((kp.conv && s == 0) ? kp.ntaps : 1);
-    static const int msub2_min_kb = [] { const char* e = getenv("HCP_MSUB2_MIN_KB"); return e ? atoi(e) : 40; }();
-    const bool msub2 = bn == 160 && kp.splits == 1 && total_kb >= msub2_min_kb && (int64_t)kp.tiles_n * m_tiles >= 200 &&
-                       getenv("HCP_GEMM_NO_MSUB2") == nullptr;
-    if (msub2) return launch_gemm<160, 2, false>(kp, stream);
     switch (bn) {
-        case 32: return launch_gemm<32, 1, false>(kp, stream);
-        case 64: return launch_gemm<64, 1, false>(kp, stream);
-        case 128: return launch_gemm<128, 1, false>(kp, stream);
-        case 160: return launch_gemm<160, 1, false>(kp, stream);
-        case 176: return launch_gemm<176, 1, false>(kp, stream);
+        case 32: return launch_gemm<32>(kp, stream);
+        case 64: return launch_gemm<64>(kp, stream);
+        case 128: return launch_gemm<128>(kp, stream);
+        case 160: return launch_gemm<160>(kp, stream);
+        case 176: return launch_gemm<176>(kp, stream);
         default: return set_error(HCP_ERR_INVALID, "unsupported BLOCK_N");
     }
 }
 
-// Output tensor maps of the TMA-store epilogue: [rows, cols] bf16 with row pitch ld, box 16 columns x 128 rows, no swizzle.
-static int make_out_maps(GemmKParams& kp) {
-    static const bool off = [] { const char* e = getenv("HCP_GEMM_TMA_STORE"); return e && atoi(e) == 0; }();
-    kp.tma_store = 0;
-    if (off || (kp.n_main % 16) != 0 || (kp.ldo % 8) != 0 || (kp.out2 && (kp.ldo2 % 8) != 0)) return HCP_OK;
-    uint64_t dims[2] = {(uint64_t)kp.n_main, (uint64_t)kp.M};
-    uint64_t strides[1] = {(uint64_t)kp.ldo * 2};
-    uint32_t box[2] = {16, BLOCK_M};
-    int rc = make_tmap_nd(&kp.tmOut, kp.out, 2, dims, strides, box, false);
-    if (rc) return rc;
-    if (kp.out2) {
-        uint64_t dims2[2] = {(uint64_t)(kp.N - kp.n_main), (uint64_t)kp.M};
-        uint64_t strides2[1] = {(uint64_t)kp.ldo2 * 2};
-        rc = make_tmap_nd(&kp.tmOut2, kp.out2, 2, dims2, strides2, box, false);
-        if (rc) return rc;
-    }
-    kp.tma_store = 1;
-    return HCP_OK;
-}
-
 // plain or split-K launch (+ finalize).  `ws` may be NULL / too small: then the launch is not split.
-static int run_gemm(int bn, bool cta_pair, int pair_splits, GemmKParams& kp, int m_tiles, int64_t total_kb, float* ws, size_t ws_bytes,
-                    bool allow_split, cudaStream_t stream) {
-    int splits = !allow_split ? 1 : cta_pair ? pair_splits : plan_splits((int64_t)m_tiles * kp.tiles_n, total_kb, kp.N);
+static int run_gemm(int bn, GemmKParams& kp, int m_tiles, int64_t total_kb, float* ws, size_t ws_bytes, bool allow_split, cudaStream_t stream) {
+    int splits = !allow_split ? 1 : plan_splits((int64_t)m_tiles * kp.tiles_n, total_kb, kp.N);
     if (splits > 1 && (!ws || ws_bytes < (size_t)splits * kp.M * kp.N * sizeof(float))) splits = 1;
     if (splits > 1) {
         kp.kb_per_split = (int)((total_kb + splits - 1) / splits);
@@ -1025,11 +617,11 @@ static int run_gemm(int bn, bool cta_pair, int pair_splits, GemmKParams& kp, int
         kp.splits = 1;
         kp.kb_per_split = 1 << 30;
         kp.ws = nullptr;
-        return dispatch_gemm(bn, cta_pair, kp, m_tiles, stream);
+        return dispatch_gemm(bn, kp, m_tiles, stream);
     }
     kp.splits = splits;
     kp.ws = ws;
-    int rc = dispatch_gemm(bn, cta_pair, kp, m_tiles, stream);
+    int rc = dispatch_gemm(bn, kp, m_tiles, stream);
     if (rc) return rc;
     const int64_t n = (int64_t)kp.M * (kp.N / 8);
     launch_k(splitk_finalize_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, stream, ws, splits, kp.M, kp.N, kp.bias, kp.rowbias,
@@ -1044,20 +636,13 @@ static int run_gemm(int bn, bool cta_pair, int pair_splits, GemmKParams& kp, int
 
 using namespace hcp;
 
-// bring-up hook (not in include/hcp_b200.h): every GEMM / conv launched after this call records 16 int64 slots per CTA (stamps and wait-cycle sums, see gemm_tc_kernel) into
-// `buf` (device memory, zeroed by the caller, 16 x 8 bytes per CTA of the largest grid); NULL switches tracing off
-extern "C" int hcp_debug_gemm_trace(long long* buf) { g_gemm_trace = buf; return HCP_OK; }
-
 extern "C" size_t hcp_splitk_workspace_bytes(int64_t M, int64_t N, int64_t total_k) {
     const int bn = pick_bn(N);
     const int64_t m_tiles = (M + BLOCK_M - 1) / BLOCK_M;
-    const PairPlan pp = plan_pair(N, m_tiles, (total_k + BLOCK_K - 1) / BLOCK_K, true);
-    if (pp.bn) return pp.splits > 1 ? (size_t)pp.splits * M * N * sizeof(float) : 0;
     const int64_t ctas = m_tiles * ((N + bn - 1) / bn);
     const int splits = plan_splits(ctas, (total_k + BLOCK_K - 1) / BLOCK_K, N);
     return splits > 1 ? (size_t)splits * M * N * sizeof(float) : 0;
 }
-
 extern "C" int hcp_gemm_bf16(const hcp_gemm_args* a, hcp_stream_t stream_) {
     if (!a || a->nseg < 1 || a->nseg > HCP_GEMM_MAX_SEG) return set_error(HCP_ERR_INVALID, "gemm: nseg");
     if (a->M <= 0 || a->N <= 0 || (a->N % 8) != 0) return set_error(HCP_ERR_INVALID, "gemm: M/N (N must be a multiple of 8)");
@@ -1065,13 +650,8 @@ extern "C" int hcp_gemm_bf16(const hcp_gemm_args* a, hcp_stream_t stream_) {
     if (a->residual && (a->ldr % 8) != 0) return set_error(HCP_ERR_INVALID, "gemm: ldr");
     GemmKParams kp;
     memset(&kp, 0, sizeof(kp));
-    int rc0 = HCP_OK;
-    int64_t kb_all = 0;
-    for (int s = 0; s < a->nseg; ++s) kb_all += (a->k[s] + BLOCK_K - 1) / BLOCK_K;
-    const PairPlan pp = plan_pair(a->N, (a->M + BLOCK_M - 1) / BLOCK_M, kb_all, a->workspace != nullptr);
-    const int pair_bn = pp.bn;
-    const int bn = pair_bn ? pair_bn : pick_bn(a->N);
-    const int b_box_rows = pair_bn ? (pair_bn > 256 ? pair_bn / 4 : pair_bn / 2) : bn;       // rows of one TMA box of B (see GemmCfg::B_BOX_ROWS)
+    const int bn = pick_bn(a->N);
+    const int b_box_rows = bn;       // rows of one TMA box of B
     for (int s = 0; s < a->nseg; ++s) {
         if (a->k[s] <= 0) return set_error(HCP_ERR_INVALID, "gemm: k must be positive");
         if ((a->lda[s] % 8) != 0 || (((a->flags >> s) & 1) == 0 && (a->ldb[s] % 8) != 0)) return set_error(HCP_ERR_INVALID, "gemm: lda/ldb");
@@ -1114,11 +694,10 @@ extern "C" int hcp_gemm_bf16(const hcp_gemm_args* a, hcp_stream_t stream_) {
         kp.ldo2 = a->ldo2;
         kp.n_main = (int)a->n_main;
     }
-    if ((rc0 = make_out_maps(kp))) return rc0;
     const int m_tiles = (int)((a->M + BLOCK_M - 1) / BLOCK_M);
     int64_t total_kb = 0;
     for (int s = 0; s < a->nseg; ++s) total_kb += kp.nkb[s];
-    return run_gemm(bn, pair_bn != 0, pp.splits, kp, m_tiles, total_kb, a->workspace, a->workspace_bytes, a->out2 == nullptr, (cudaStream_t)stream_);
+    return run_gemm(bn, kp, m_tiles, total_kb, a->workspace, a->workspace_bytes, a->out2 == nullptr, (cudaStream_t)stream_);
 }
 
 // Conv2d LoRA: out += T . Bl^T as K-segment 1 (plain 2D operands; the rows of an M tile of the convolution are contiguous pixels)
@@ -1143,7 +722,7 @@ extern "C" int hcp_conv3x3_bf16(const hcp_conv3x3_args* a, hcp_stream_t stream_)
     if (a->mode != 0 && !(a->mode == 1)) return set_error(HCP_ERR_INVALID, "conv3x3: mode");
     GemmKParams kp;
     memset(&kp, 0, sizeof(kp));
-    int bn = pick_bn(a->Cout);
+    const int bn = pick_bn(a->Cout);
     const int64_t Cin = a->Cin;
 
     // geometry of the "tile grid" (the grid the 128-pixel M tiles walk over) and of the output map
@@ -1187,20 +766,8 @@ extern "C" int hcp_conv3x3_bf16(const hcp_conv3x3_args* a, hcp_stream_t stream_)
     kp.ldo = a->Cout;
     kp.n_main = (int)a->Cout;
     const int m_tiles = (bnimg == 1) ? (int)(a->B * kp.tiles_w * kp.tiles_h) : (int)((a->B + bnimg - 1) / bnimg);
-    // CTA pairs for the forward-mode launches (mode 1 = four short phase launches of the stride-2 dgrad: single CTAs)
-    const PairPlan pp = (a->mode == 0) ? plan_pair(a->Cout, m_tiles, 9 * (Cin / BLOCK_K) + (a->lora_t ? (a->lora_ld + BLOCK_K - 1) / BLOCK_K : 0),
-                                                   a->workspace != nullptr)
-                                       : PairPlan{0, 1};
-    const int pair_bn = pp.bn;
-    if (pair_bn) {
-        bn = pair_bn;
-        kp.tiles_n = (int)((a->Cout + bn - 1) / bn);
-    }
-    const int b_box_rows = pair_bn ? (pair_bn > 256 ? pair_bn / 4 : pair_bn / 2) : bn;
+    const int b_box_rows = bn;
     int rc;
-    // the 128 pixels of a forward-mode tile are consecutive rows of `out` (full-width rows of one or several images, or 128 pixels of
-    // one row): its parts can leave through TMA stores; the strided phase launches of the stride-2 dgrad (mode 1) store by hand
-    if (a->mode == 0 && (rc = make_out_maps(kp))) return rc;
     if (a->w_tiled) {          // k-block-major weights [9*Cin/64][Cout][64]
         uint64_t dims[3] = {BLOCK_K, (uint64_t)a->Cout, (uint64_t)(9 * Cin / BLOCK_K)};
         uint64_t strides[2] = {BLOCK_K * 2, (uint64_t)a->Cout * BLOCK_K * 2};
@@ -1229,7 +796,7 @@ extern "C" int hcp_conv3x3_bf16(const hcp_conv3x3_args* a, hcp_stream_t stream_)
             }
         kp.sh = kp.sw = 1; kp.oh0 = kp.ow0 = 0;
         if ((rc = conv_lora_segment(a, kp, b_box_rows))) return rc;
-        return run_gemm(bn, pair_bn != 0, pp.splits, kp, m_tiles, (int64_t)9 * kp.nkb[0] + (kp.nseg > 1 ? kp.nkb[1] : 0), a->workspace, a->workspace_bytes, true, stream);
+        return run_gemm(bn, kp, m_tiles, (int64_t)9 * kp.nkb[0] + (kp.nseg > 1 ? kp.nkb[1] : 0), a->workspace, a->workspace_bytes, true, stream);
     }
     if (a->mode == 0 && a->stride == 2) {
         // view x as [B][Hin/2][2][Win/2][2*Cin]: input row ih = 2*oh + kh - 1 -> (phase, index)
@@ -1253,7 +820,7 @@ extern "C" int hcp_conv3x3_bf16(const hcp_conv3x3_args* a, hcp_stream_t stream_)
             }
         kp.sh = kp.sw = 1; kp.oh0 = kp.ow0 = 0;
         if ((rc = conv_lora_segment(a, kp, b_box_rows))) return rc;
-        return run_gemm(bn, pair_bn != 0, pp.splits, kp, m_tiles, (int64_t)9 * kp.nkb[0] + (kp.nseg > 1 ? kp.nkb[1] : 0), a->workspace, a->workspace_bytes, true, stream);
+        return run_gemm(bn, kp, m_tiles, (int64_t)9 * kp.nkb[0] + (kp.nseg > 1 ? kp.nkb[1] : 0), a->workspace, a->workspace_bytes, true, stream);
     }
     if (a->lora_t) return set_error(HCP_ERR_INVALID, "conv3x3: the LoRA segment is only available in mode 0");
     // mode 1: dgrad of the stride-2 conv.  x = dY [B, Hin, Win, Cin] (Cin = Cout of the fwd conv),
@@ -1285,7 +852,7 @@ extern "C" int hcp_conv3x3_bf16(const hcp_conv3x3_args* a, hcp_stream_t stream_)
             }
             kp.ntaps = nt;
             kp.oh0 = ph; kp.ow0 = pw;
-            rc = run_gemm(bn, false, 1, kp, m_tiles, 0, nullptr, 0, false, stream);
+            rc = run_gemm(bn, kp, m_tiles, 0, nullptr, 0, false, stream);
             if (rc) return rc;
         }
     return HCP_OK;
@@ -1339,7 +906,7 @@ extern "C" int hcp_lora_grad(const void* S, int64_t lds, const void* X, int64_t 
     LoraGradParams p;
     memset(&p, 0, sizeof(p));
     p.M = (int)M; p.nprob = 1;
-    int rc = lg_fill(p, 0, S, lds, X, ldx, M, n_begin, n_end, blocks, nblocks, 148);
+    int rc = lg_fill(p, 0, S, lds, X, ldx, M, n_begin, n_end, blocks, nblocks, num_sms());
     if (rc) return rc;
     return lg_launch(p, (cudaStream_t)stream_);
 }
@@ -1387,7 +954,7 @@ extern "C" int hcp_lora_grad_conv3x3(const void* S, int64_t lds, const void* x, 
     q.n_begin = 0; q.n_end = (int)Cin; q.nblocks = nblocks;
     q.col_chunks = (int)((Cin + 127) / 128);
     const int total_tiles = (int)((M + 127) / 128);
-    int splits = 148 / q.col_chunks;
+    int splits = num_sms() / q.col_chunks;
     if (splits < 1) splits = 1;
     if (splits > total_tiles) splits = total_tiles;
     q.tiles_per_cta = (total_tiles + splits - 1) / splits;
@@ -1422,14 +989,15 @@ extern "C" int hcp_lora_grad_pair(const void* U, const void* x, int64_t ldx, int
     LoraGradParams p;
     memset(&p, 0, sizeof(p));
     p.M = (int)M; p.nprob = 2;
-    // split the 148 SMs between the two problems in proportion to their column counts (one CTA per SM: 147 KB of smem each)
+    // split the SMs between the two problems in proportion to their column counts (one CTA per SM: 147 KB of smem each)
     const int64_t ck = (K + 127) / 128, cn = (N + 127) / 128;
-    int t0 = (int)((148 * ck + (ck + cn) / 2) / (ck + cn));
+    const int sms = num_sms();
+    int t0 = (int)((sms * ck + (ck + cn) / 2) / (ck + cn));
     if (t0 < 1) t0 = 1;
-    if (t0 > 147) t0 = 147;
+    if (t0 > sms - 1) t0 = sms - 1;
     int rc = lg_fill(p, 0, U, lds, x, ldx, M, 0, K, down, nblocks, t0);
     if (rc) return rc;
-    rc = lg_fill(p, 1, T, lds, dy, lddy, M, 0, N, up, nblocks, 148 - t0);
+    rc = lg_fill(p, 1, T, lds, dy, lddy, M, 0, N, up, nblocks, sms - t0);
     if (rc) return rc;
     return lg_launch(p, (cudaStream_t)stream_);
 }

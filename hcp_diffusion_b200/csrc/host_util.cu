@@ -19,13 +19,23 @@ int set_cuda_error(cudaError_t e, const char* where) {
     return HCP_ERR_CUDA;
 }
 
+int num_sms() {
+    static const int n = [] {
+        int dev = 0, v = 0;
+        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0)
+            return 132;                     // H100 SXM
+        return v;
+    }();
+    return n;
+}
+
 static std::atomic<unsigned long long> g_launches{0};
 void note_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 
 bool pdl_enabled() {
     static const bool on = [] {
-        // measured on B200 inside the captured step graph: 22.67 ms with the programmatic edges vs 23.02 ms without
-        // (profiles/r01_bench_v11*.json; ~0.8 us per kernel boundary in tools/bench_ops.py).  HCP_PDL=0 turns them off.
+        // programmatic edges let a kernel's prologue overlap its predecessor's tail inside the captured step graph.
+        // HCP_PDL=0 turns them off.
         const char* e = getenv("HCP_PDL");
         return !(e && e[0] == '0');
     }();
@@ -101,9 +111,11 @@ extern "C" int hcp_device_check(void) {
     int dev = 0;
     cudaError_t e = cudaGetDevice(&dev);
     if (e != cudaSuccess) return hcp::set_cuda_error(e, "cudaGetDevice");
-    int major = 0;
+    int major = 0, minor = 0;
     e = cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
+    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
     if (e != cudaSuccess) return hcp::set_cuda_error(e, "cudaDeviceGetAttribute");
-    if (major != 10) return hcp::set_error(HCP_ERR_NO_DEVICE, "libhcpb200 needs a compute-capability 10.x (B200) device");
+    // the kernels are built for sm_90a only (wgmma): their cubin loads on compute capability 9.0 and nothing else
+    if (major != 9 || minor != 0) return hcp::set_error(HCP_ERR_NO_DEVICE, "libhcpb200 needs a compute-capability 9.0 (H100) device");
     return HCP_OK;
 }

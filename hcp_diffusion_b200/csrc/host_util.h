@@ -11,6 +11,8 @@ namespace hcp {
 
 int set_error(int code, const char* msg);
 int set_cuda_error(cudaError_t e, const char* where);
+// streaming multiprocessors of the current device (queried once); launch planning sizes its waves by it
+int num_sms();
 
 // bf16, SWIZZLE_128B, zero fill for out-of-bounds elements.  `dims`/`box` innermost first;
 // `strides_bytes` has rank-1 entries (the innermost stride is the element size).
@@ -44,29 +46,6 @@ inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, siz
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = pdl_enabled() ? 1 : 0;
-    note_launch();
-    return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
-}
-
-// Thread-block clusters of `cluster_x` CTAs along x AND programmatic stream serialization (the CTA-pair GEMM).
-template <typename... KArgs, typename... Args>
-inline cudaError_t launch_k_cluster(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, unsigned cluster_x,
-                                    Args&&... args) {
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = grid;
-    cfg.blockDim = block;
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = cluster_x;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = pdl_enabled() ? 2 : 1;
     note_launch();
     return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }

@@ -1,5 +1,5 @@
 // SPDX-License-Identifier: Apache-2.0
-// Small kernels at the edges of the UNet hot path (sm_100a): the 4-channel convolutions conv_in / conv_out
+// Small kernels at the edges of the UNet hot path (sm_90a): the 4-channel convolutions conv_in / conv_out
 // (NCHW fp32 at the module boundary <-> bf16 NHWC inside), the timestep-embedding MLP and all ResnetBlock2D
 // time_emb_proj layers as one skinny linear, LoRA parameter packing and LoRA gradient reduction, and the loss /
 // optimizer kernels either side of the UNet call.
@@ -284,7 +284,7 @@ __global__ void __launch_bounds__(256) lora_merge_kernel(const hcp_lora_merge_jo
     pdl_trigger();
     pdl_wait();
     // job of this tile: one load from the caller's tile -> job table, or (no table) the last job with tile0 <= blockIdx.x by a
-    // binary search -- seven DEPENDENT global loads per CTA, which was most of the r02 first version's 320 us
+    // binary search -- seven DEPENDENT global loads per CTA
     int lo = 0;
     if (tile_job) {
         lo = tile_job[blockIdx.x];
@@ -647,7 +647,7 @@ extern "C" int hcp_adamw_flat_dev(float* p, const float* g, float* m, float* v, 
     launch_k(incr_step_kernel, dim3(1), dim3(1), 0, (cudaStream_t)st, step_device);
     if (((uintptr_t)p | (uintptr_t)g | (uintptr_t)m | (uintptr_t)v) & 15) return set_error(HCP_ERR_INVALID, "adamw_dev: buffers must be 16-byte aligned");
     int64_t blocks = ((n >> 2) + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > num_sms() * 16) blocks = num_sms() * 16;
     if (blocks < 1) blocks = 1;
     launch_k(adamw_flat_dev_kernel, dim3((unsigned)blocks), dim3(256), 0, (cudaStream_t)st, p, g, m, v, n, hyper_device, grad_scale,
              sumsq_device, max_norm, step_device);

@@ -1,5 +1,5 @@
 // SPDX-License-Identifier: Apache-2.0
-// HBM-bound kernels of the UNet hot path (sm_100a): GroupNorm(+SiLU) and LayerNorm forward/backward with
+// HBM-bound kernels of the UNet hot path (sm_90a): GroupNorm(+SiLU) and LayerNorm forward/backward with
 // warp-shuffle reductions, GEGLU, nearest-2x upsample.  All activations are bf16 NHWC / token-major, statistics
 // and accumulation fp32, 16-byte vector accesses.
 //
@@ -765,8 +765,7 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const __nv_bfloat16* __r
         }
     }
     // Software pipeline over the rows of this warp: the raw 16-byte vectors of row r+1 (x, and dY / the residual gradient in the
-    // backward) are requested BEFORE row r is reduced, normalised and stored.  The first version walked its rows strictly one after
-    // the other -- 7 rows x one full memory round trip each = the 9.4 us it took for 10 MB at M = 16384, C = 320.
+    // backward) are requested BEFORE row r is reduced, normalised and stored, so a warp never waits one full memory round trip per row.
     const int64_t row_begin = warp_g * rows_per_warp;
     if (row_begin >= M) return;
     const int64_t row_end = (row_begin + rows_per_warp < M) ? row_begin + rows_per_warp : M;
@@ -863,8 +862,9 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const __nv_bfloat16* __r
 template <bool BWD>
 static void launch_layernorm(const __nv_bfloat16* x, const __nv_bfloat16* dy, const __nv_bfloat16* add, const float* gamma,
                              const float* beta, float eps, int64_t M, int C, float* stats, __nv_bfloat16* out, cudaStream_t st) {
-    // one wave of CTAs: 148 SMs x 2 resident CTAs (the register-resident rows + affine parameters cost 75-190 registers) x 8 warps
-    int rpw = (int)((M + 2367) / 2368);
+    // one wave of CTAs: SMs x 2 resident CTAs (the register-resident rows + affine parameters cost 75-190 registers) x 8 warps
+    const int64_t wave = (int64_t)num_sms() * 2 * 8;
+    int rpw = (int)((M + wave - 1) / wave);
     if (rpw < 1) rpw = 1;
     if (rpw > 32) rpw = 32;
     const int64_t warps = (M + rpw - 1) / rpw;

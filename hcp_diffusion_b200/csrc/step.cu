@@ -1,5 +1,5 @@
 // SPDX-License-Identifier: Apache-2.0
-// Training-step kernels either side of the UNet call that the plain MSE / AdamW pair of misc.cu does not cover (sm_100a):
+// Training-step kernels either side of the UNet call that the plain MSE / AdamW pair of misc.cu does not cover (sm_90a):
 //   * SNR-weighted eps loss (reference hcpdiff/loss/min_snr_loss.py:5-52: MinSNR / SoftMinSNR / KDiffMinSNR / EDM weights)
 //   * exponential moving average of the flat trainable buffer (reference hcpdiff/utils/ema.py:18-32)
 //   * nn.Dropout on a patched layer's output (reference hcpdiff/models/lora_base_patch.py:74), counter-based RNG so that the

@@ -1,8 +1,8 @@
 // SPDX-License-Identifier: Apache-2.0
 // Weight gradients of the base model (full fine-tune, reference `unet:` config items: hcpdiff/utils/cfg_net_tools.py:96-106,
-// cfgs/train/examples/DreamBooth.yaml:6-10) for sm_100a:
-//   * wgrad_tc_kernel<SN>: dW = dY^T . X on the tensor pipe (tcgen05 TN GEMM, both operands read MN-major straight from the row-major
-//     activations through TMA; the X operand of a 3x3 convolution is the shifted NHWC box of the forward kernel), fp32 `red` into
+// cfgs/train/examples/DreamBooth.yaml:6-10) for sm_90a:
+//   * wgrad_tc_kernel<SN>: dW = dY^T . X on the tensor cores (wgmma TN GEMM, both operands read MN-major straight from the row-major
+//     activations through TMA; the X operand of a 3x3 convolution is the shifted NHWC box of the forward kernel), fp32 atomics into
 //     the flat gradient buffer;
 //   * column sums (bias gradients, per-image time-embedding gradients), GroupNorm / LayerNorm affine gradients;
 //   * the 4-channel boundary convolutions' weight gradients, the small fp32 linears of the time-embedding path (M = batch rows);
@@ -24,10 +24,10 @@ namespace hcp {
 // D[j, n] += scale * sum_m S[m, j0 + j] * X[m, n0 + n]        (reduction over the M token / pixel rows)
 //   linear:  dW[o, k] : S = dY [M, N], X = x [M, K]
 //   conv3x3: dW[co, ci, kh, kw] : S = dY, X = x shifted by the tap (4-D / 5-D NHWC box, zero padding by TMA)
-// One CTA owns 128 columns of X and SN columns of S over a slice of the rows; MMA M = 128 (X columns), N = SN (S columns),
-// K = 16 rows per instruction; the 128 x SN fp32 accumulator is reduced into dst[j * ld_j + n * ld_n] with red.global.
+// One CTA owns 128 columns of X and SN columns of S over a slice of the rows; MMA warpgroup g computes X columns [64g, 64g+64)
+// (wgmma M = 64, N = SN, K = 16 rows per instruction) and reduces its 64 x SN fp32 block into dst[j * ld_j + n * ld_n] with atomics.
 // =============================================================================================
-constexpr int kWgThreads = 192;   // warp 0: TMA, warp 1: MMA, warps 2-5: reduction epilogue
+constexpr int kWgThreads = 288;   // warps 0-7: two MMA warpgroups, warp 8: TMA
 
 struct WgConv {
     int32_t rank;            // 0: plain [M, ldx] matrix; 4 / 5: rank of the NHWC tensor map
@@ -50,7 +50,7 @@ struct WgCfg {
     static constexpr int X_BYTES = 2 * 128 * 128;             // two 64-column boxes of 128 rows
     static constexpr int S_BYTES = (SN / 64) * 128 * 128;
     static constexpr int STAGE_BYTES = X_BYTES + S_BYTES;
-    static constexpr int STAGES = (SN == 256) ? 2 : 3;
+    static constexpr int STAGES = 3;
     static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 256 + 1024;
 };
 
@@ -62,9 +62,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
     uint64_t* empty_bar = full_bar + STAGES;
-    uint64_t* tmem_full_bar = empty_bar + STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = warp_id_uniform(), lane = threadIdx.x & 31;
     // flat grid over (row split, j tile, n tile): n fastest so that concurrent CTAs share the S tile in L2
     const int bid = blockIdx.x;
     const int nt = bid % p.n_tiles, jt = (bid / p.n_tiles) % p.j_tiles, sp = bid / (p.n_tiles * p.j_tiles);
@@ -74,21 +72,16 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
     const int t1 = min(total_tiles, t0 + p.tiles_per_cta);
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        mbar_init(tmem_full_bar, 1);
+        for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 256); }
         fence_mbar_init();
         tma_prefetch_desc(&p.tmX);
         tma_prefetch_desc(&p.tmS);
     }
-    if (warp == 1) { tmem_alloc(tmem_slot, SN < 32 ? 32 : SN); tmem_relinquish(); }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     pdl_trigger();
     pdl_wait();
 
-    if (warp == 0) {
+    if (warp == 8) {
         if (elect_one()) {
             int stage = 0; uint32_t phase = 0;
             for (int t = t0; t < t1; ++t) {
@@ -121,51 +114,41 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
                 if (++stage == STAGES) { stage = 0; phase ^= 1; }
             }
         }
-    } else if (warp == 1) {
-        if (elect_one()) {
-            constexpr uint32_t idesc = make_idesc_bf16(128, SN, 1, 1);     // A (X^T) and B (S^T) both MN-major
-            int stage = 0; uint32_t phase = 0; uint32_t accum = 0;
-            for (int t = t0; t < t1; ++t) {
-                mbar_wait(&full_bar[stage], phase);
-                tc_fence_after();
-                const uint32_t xb = smem_u32(smem + stage * Cfg::STAGE_BYTES);
-                const uint32_t sb = xb + Cfg::X_BYTES;
-                for (int ks = 0; ks < 8; ++ks) {                         // 16 rows per k-step = 2048 B inside each 64-column box
-                    // MN-major SWIZZLE_128B: LBO = distance between 64-wide MN chunks (one box = 16 KB), SBO = 8 k rows = 1024 B
-                    umma_ss(tmem_base, make_smem_desc(xb + ks * 2048, 128 * 128, 1024), make_smem_desc(sb + ks * 2048, 128 * 128, 1024),
-                            idesc, accum);
-                    accum = 1;
-                }
-                umma_commit(&empty_bar[stage]);
-                if (++stage == STAGES) { stage = 0; phase ^= 1; }
-            }
-            umma_commit(tmem_full_bar);
-        }
-    } else {
-        const int quarter = warp & 3;
-        const int n = ncol0 + quarter * 32 + lane;                       // this thread's column of X
-        mbar_wait(tmem_full_bar, 0);
-        tc_fence_after();
-        const uint32_t trow = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16);
-        const bool n_ok = (t1 > t0) && n < p.n_cols;
-        float* dcol = p.dst + (int64_t)n * p.ld_n;
-#pragma unroll 1
-        for (int c = 0; c < SN / 16; ++c) {
-            uint32_t v[16];
-            tmem_ld16(trow + c * 16, v);
-            tmem_wait_ld();
-            if (n_ok) {
+        return;
+    }
+    const int wg = warp >> 2;
+    float acc[SN / 2];
 #pragma unroll
-                for (int e = 0; e < 16; ++e) {
-                    const int j = jcol0 + c * 16 + e;
-                    if (j < p.j_cols) atomicAdd(dcol + (int64_t)j * p.ld_j, __uint_as_float(v[e]) * p.scale);
-                }
-            }
+    for (int i = 0; i < SN / 2; ++i) acc[i] = 0.f;
+    int stage = 0; uint32_t phase = 0;
+    for (int t = t0; t < t1; ++t) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t xb = smem_u32(smem + stage * Cfg::STAGE_BYTES) + wg * 128 * 128;   // this warpgroup's 64 X columns
+        const uint32_t sb = smem_u32(smem + stage * Cfg::STAGE_BYTES) + Cfg::X_BYTES;
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < 8; ++ks)       // 16 rows per k-step = 2048 B inside each 64-column box
+            // MN-major SWIZZLE_128B: LBO = distance between 64-wide MN chunks (one box = 16 KB), SBO = 8 k rows = 1024 B
+            wgmma_ss<SN, 1, 1>(acc, make_smem_desc(xb + ks * 2048, 128 * 128, 1024), make_smem_desc(sb + ks * 2048, 128 * 128, 1024), 1u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        mbar_arrive(&empty_bar[stage]);
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+    }
+    wgmma_fence_acc(acc);
+    if (t1 <= t0) return;
+    const float scale = p.scale;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int n = ncol0 + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;     // column of X
+        if (n >= p.n_cols) continue;
+        float* dcol = p.dst + (int64_t)n * p.ld_n;
+#pragma unroll
+        for (int i = 0; i < SN / 4; ++i) {
+            const int j = jcol0 + 8 * (i >> 1) + 2 * (lane & 3) + (i & 1);          // column of S
+            if (j < p.j_cols) atomicAdd(dcol + (int64_t)j * p.ld_j, acc[4 * (i >> 1) + 2 * h + (i & 1)] * scale);
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, SN < 32 ? 32 : SN);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -569,19 +552,18 @@ static int launch_wgrad(const WgradParams& p, int ctas, cudaStream_t stream) {
 }
 
 static int run_wgrad(WgradParams& p, int64_t j_cols, int64_t n_cols, cudaStream_t stream) {
-    const int sn = (j_cols > 128) ? 256 : (j_cols > 64) ? 128 : 64;
+    const int sn = (j_cols > 64) ? 128 : 64;
     p.n_tiles = (int)((n_cols + 127) / 128);
     p.j_tiles = (int)((j_cols + sn - 1) / sn);
     p.n_cols = (int)n_cols; p.j_cols = (int)j_cols;
     const int total_tiles = (p.M + 127) / 128;
     const int out_tiles = p.n_tiles * p.j_tiles;
-    int splits = (2 * 148 + out_tiles - 1) / out_tiles;          // about two waves of CTAs
+    int splits = (2 * num_sms() + out_tiles - 1) / out_tiles;    // about two waves of CTAs
     if (splits < 1) splits = 1;
     if (splits > total_tiles) splits = total_tiles;
     p.tiles_per_cta = (total_tiles + splits - 1) / splits;
     p.splits = (total_tiles + p.tiles_per_cta - 1) / p.tiles_per_cta;
     const int ctas = out_tiles * p.splits;
-    if (sn == 256) return launch_wgrad<256>(p, ctas, stream);
     if (sn == 128) return launch_wgrad<128>(p, ctas, stream);
     return launch_wgrad<64>(p, ctas, stream);
 }

@@ -1,4 +1,4 @@
-"""The training step around the UNet call, B200-native.
+"""The training step around the UNet call, H100-native.
 
 What the reference does per step (hcpdiff/train_ac.py:467-504): H2D copies, `make_noise` (:437-447), the CFG context
 (`DreamArtistPTContext.pre/post`, hcpdiff/models/cfg_context.py:12-38), UNet forward through accelerate's autocast + DDP, the
@@ -227,6 +227,7 @@ class LoraTrainStep:
             self.ema = self.flat.data.clone()
         self.acp = ddpm_alphas_cumprod(num_train_timesteps).to(dev)
         self.loss = torch.zeros(1, dtype=torch.float32, device=dev)
+        self.noise_pred: Optional[torch.Tensor] = None     # the UNet output of the last micro-step (kept alive across graph replays)
         self.gsq = torch.zeros(1, dtype=torch.float32, device=dev)
         self.use_graph = use_cuda_graph
         self.pg = process_group
@@ -297,6 +298,7 @@ class LoraTrainStep:
         if self.cfg_ctx is not None:
             pred = _CfgMixFn.apply(pred, t, *self.cfg_ctx)
         leaf = pred.detach()
+        self.noise_pred = leaf
         dpred = torch.empty_like(leaf)
         gscale = 1.0 / self.accum                          # accelerator.backward: loss / gradient_accumulation_steps
         if self.loss_cfg is None:

@@ -1,4 +1,4 @@
-"""Layer-wise LoRA adapters with hcpdiff's plugin surface, executed by the fused sm_100a kernels.
+"""Layer-wise LoRA adapters with hcpdiff's plugin surface, executed by the fused sm_90a kernels.
 
 Same classes, constructor signatures, parameter names and checkpoint keys as the reference's active implementation
 (hcpdiff/models/lora_base_patch.py: LoraPatchContainer :20-35, LoraBlock :37-156, LoraGroup :175-194;
@@ -60,7 +60,7 @@ class LoraBlock(PatchPluginBlock):
         else:
             raise NotImplementedError(f"No lora for {type(host)}")
         if bias:
-            raise NotImplementedError("LoRA bias is not supported on the B200 hot path")
+            raise NotImplementedError("LoRA bias is not supported on the H100 hot path")
         self.dropout = nn.Dropout(dropout)
         self.rank = self.layer.rank
         self.register_buffer("alpha", torch.tensor(alpha / self.rank if alpha_auto_scale else alpha))
@@ -146,7 +146,7 @@ class LoraLayer(LoraBlock):
         def __init__(self, host: nn.Conv2d, rank, bias, block):
             super().__init__(host, rank, bias, block)
             if host.groups != 1 or host.dilation != (1, 1):
-                raise NotImplementedError("Conv2d LoRA on grouped / dilated convolutions is not supported on the B200 hot path")
+                raise NotImplementedError("Conv2d LoRA on grouped / dilated convolutions is not supported on the H100 hot path")
             dev = host.weight.device
             self.W_down = nn.Parameter(torch.empty(self.rank, host.in_channels, *host.kernel_size, device=dev))
             self.W_up = nn.Parameter(torch.empty(host.out_channels, self.rank, 1, 1, device=dev))

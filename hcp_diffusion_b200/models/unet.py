@@ -398,11 +398,11 @@ class UNet2DConditionModel(nn.Module):
 
     def enable_gradient_checkpointing(self):
         """Accepted for config compatibility (reference cfgs/train/train_base.yaml:69).  Activation recomputation is not used:
-        a B200 holds the SD1.5 activations of the benchmark batch sizes many times over."""
+        an H100 holds the SD1.5 activations of the benchmark batch sizes many times over."""
         self.gradient_checkpointing = True
 
     def enable_xformers_memory_efficient_attention(self, *args, **kwargs):
-        """No-op: attention always runs the fused tcgen05 kernel (reference hcpdiff/train_ac.py:258-263 toggles xFormers here)."""
+        """No-op: attention always runs the fused wgmma kernel (reference hcpdiff/train_ac.py:258-263 toggles xFormers here)."""
 
     def resnets_in_order(self) -> List[ResnetBlock2D]:
         out = []
@@ -455,11 +455,11 @@ class UNet2DConditionModel(nn.Module):
             from .lora import DAPPPatchContainer, LoraPatchContainer
             for p in (te.linear_1, te.linear_2):
                 if not isinstance(p, nn.Linear):
-                    raise NotImplementedError("plugins on time_embedding.linear_1 / linear_2 are not supported on the B200 hot path")
+                    raise NotImplementedError("plugins on time_embedding.linear_1 / linear_2 are not supported on the H100 hot path")
             for r in resnets:
                 m = r.time_emb_proj
                 if isinstance(m, DAPPPatchContainer) or not isinstance(m, (nn.Linear, LoraPatchContainer)):
-                    raise NotImplementedError(f"{type(m).__name__} on time_emb_proj is not supported on the B200 hot path")
+                    raise NotImplementedError(f"{type(m).__name__} on time_emb_proj is not supported on the H100 hot path")
             rt = SimpleNamespace(sig=sig)
             # LoRA on time_emb_proj: per patched resnet the stacked blocks; their rank-r products are two small fp32 linears each
             rt.temb_lora = [[m[name] for name in m.plugin_names] if isinstance(m, LoraPatchContainer) else []
@@ -483,7 +483,7 @@ class UNet2DConditionModel(nn.Module):
                 ae = self.add_embedding
                 for p in (ae.linear_1, ae.linear_2):
                     if not isinstance(p, nn.Linear) or p.weight.requires_grad:
-                        raise NotImplementedError("plugins / training on the additional-embedding layers are not supported on the B200 hot path")
+                        raise NotImplementedError("plugins / training on the additional-embedding layers are not supported on the H100 hot path")
                 if rt.train_time:
                     raise NotImplementedError("training the time embedding of a UNet with an additional (text_time) embedding is not supported")
                 rt.add = SimpleNamespace(
@@ -529,7 +529,7 @@ class UNet2DConditionModel(nn.Module):
     def forward(self, sample: torch.Tensor, timestep, encoder_hidden_states: torch.Tensor,
                 encoder_attention_mask: Optional[torch.Tensor] = None, return_dict: bool = True, **kwargs):
         if not sample.is_cuda:
-            raise _lib.HcpError("hcp_diffusion_b200.UNet2DConditionModel runs on a CUDA (sm_100) device only; there is no CPU fallback")
+            raise _lib.HcpError("hcp_diffusion_b200.UNet2DConditionModel runs on a CUDA (sm_90) device only; there is no CPU fallback")
         for key in ("class_labels", "down_block_additional_residuals", "mid_block_additional_residual"):
             if kwargs.get(key) is not None:
                 raise NotImplementedError(f"`{key}` is not supported by the hot path")

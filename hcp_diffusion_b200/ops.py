@@ -1,6 +1,6 @@
 """Autograd wrappers around the C-ABI kernels (libhcpb200).
 
-Every function here enqueues hand-written sm_100a kernels on the current CUDA stream through `_lib.call`; torch only
+Every function here enqueues hand-written sm_90a kernels on the current CUDA stream through `_lib.call`; torch only
 allocates the buffers and records the autograd graph.  Activations are bf16, "NHWC": a feature map [B,H,W,C] and the
 token matrix [B*H*W, C] are the same memory.
 
@@ -661,7 +661,7 @@ class FusedLinearFn(torch.autograd.Function):
         N, R = pack.N, pack.R
         U = None
         if pack.train:
-            # full fine-tune: dW[o, k] += sum_m dY[m, o] x[m, k] per trained host (tcgen05 TN GEMM), db[o] += colsum(dY)
+            # full fine-tune: dW[o, k] += sum_m dY[m, o] x[m, k] per trained host (wgmma TN GEMM), db[o] += colsum(dY)
             xs_t = ctx.saved_tensors[:len(ks)]
             for w, b, o0, n in pack.train:
                 gw = _acc_grad(w)

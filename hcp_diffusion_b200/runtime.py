@@ -79,7 +79,7 @@ class LinearGroup:
         hosts = [host_and_blocks(ch) for ch in self.children]
         for host, _ in hosts:
             if not host.weight.is_cuda:
-                raise _lib.HcpError("hcp_diffusion_b200 runs on CUDA only: move the model to a B200 device (there is no CPU path)")
+                raise _lib.HcpError("hcp_diffusion_b200 runs on CUDA only: move the model to an H100 device (there is no CPU path)")
         w = torch.cat([_weight_2d(h) for h, _ in hosts], dim=0)
         biases = [h.bias for h, _ in hosts]
         bias = None
@@ -135,7 +135,7 @@ class LinearGroup:
         take NCHW like the reference layer (the NHWC view is the boundary conversion, the product path inside the UNet never
         leaves NHWC)."""
         if not x.is_cuda:
-            raise _lib.HcpError("hcp_diffusion_b200 has no CPU path: LoRA layers run on a B200 only")
+            raise _lib.HcpError("hcp_diffusion_b200 has no CPU path: LoRA layers run on an H100 only")
         pack = self.prepare()
         if pack.lora:
             pack_lora([self])
@@ -275,7 +275,7 @@ class ConvGroup:
     def run_standalone(self, x: torch.Tensor) -> torch.Tensor:
         """LoraPatchContainer.forward on a 3x3 host: NCHW in / out like the reference layer."""
         if not x.is_cuda:
-            raise _lib.HcpError("hcp_diffusion_b200 has no CPU path: LoRA layers run on a B200 only")
+            raise _lib.HcpError("hcp_diffusion_b200 has no CPU path: LoRA layers run on an H100 only")
         pack = self.prepare()
         if pack.lora:
             pack_lora([self])

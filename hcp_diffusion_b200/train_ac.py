@@ -3,7 +3,7 @@
 The reference entrypoint (hcpdiff/train_ac.py:559-566: `load_config_with_cli` -> `Trainer(conf)` -> `trainer.train()`), reduced to
 the hot path: build the UNet (cfg `model.unet`, the reference's injection seam train_ac.py:220), apply the `unet:` (full-layer
 training) and `lora_unet:` lists through `make_hcpdiff` (train_ac.py:324-359), then run `train.train_steps` optimizer steps with
-the B200 engine and save `ckpts/unet-<step>.safetensors` every `train.save_step` in the reference checkpoint format
+the H100 engine and save `ckpts/unet-<step>.safetensors` every `train.save_step` in the reference checkpoint format
 (train_ac.py:523-544).  Honoured `train.*` keys: `gradient_accumulation_steps`, `max_grad_norm`, `scale_lr`, `optimizer.{lr,
 weight_decay, betas, eps}`, `scheduler.{name, num_warmup_steps, num_training_steps, scheduler_kwargs}` (one_cycle / constant /
 constant_with_warmup), `loss.criterion` (`torch.nn.MSELoss` or `hcpdiff.loss.MinSNRLoss`-family `_target_` + `gamma`), `cfg_scale`
@@ -48,7 +48,7 @@ def loss_from_cfg(loss_cfg):
         return None
     if target in _SNR_LOSSES:
         return {"type": target, "gamma": float(crit.get("gamma", 1.0))}
-    raise NotImplementedError(f"train.loss.criterion {target!r} is not supported on the B200 hot path")
+    raise NotImplementedError(f"train.loss.criterion {target!r} is not supported on the H100 hot path")
 
 
 def make_scheduler(cfg, step_fn: LoraTrainStep):
@@ -208,7 +208,7 @@ class Trainer:
 
 
 def main(argv=None):
-    ap = argparse.ArgumentParser(description="HCP-Diffusion LoRA training on the B200 hot path")
+    ap = argparse.ArgumentParser(description="HCP-Diffusion LoRA training on the H100 hot path")
     ap.add_argument("--cfg", type=str, required=True)
     args, overrides = ap.parse_known_args(argv)
     conf = load_config_with_cli(args.cfg, args_list=overrides)

@@ -1,6 +1,6 @@
 /* SPDX-License-Identifier: Apache-2.0
  *
- * libhcpb200 -- C ABI of the B200 (sm_100a) kernels behind the HCP-Diffusion UNet denoising hot path.
+ * libhcpb200 -- C ABI of the H100 (sm_90a) kernels behind the HCP-Diffusion UNet denoising hot path.
  *
  * The reference (IrisRainbowNeko/HCP-Diffusion @ 404f0e85) has NO native code and NO FFI: every op
  * below replaces a PyTorch call made from the pure-Python hot path.  Each entry point cites the
@@ -31,7 +31,7 @@ enum hcp_status {
     HCP_OK = 0,
     HCP_ERR_INVALID = -1,   /* bad argument / unsupported shape */
     HCP_ERR_CUDA = -2,      /* CUDA runtime or driver error (see hcp_last_error_string) */
-    HCP_ERR_NO_DEVICE = -3, /* no sm_100 device / driver entry point missing */
+    HCP_ERR_NO_DEVICE = -3, /* no sm_90 device / driver entry point missing */
 };
 
 int hcp_version(void);                     /* ABI version, bumps on any signature change */
@@ -42,7 +42,7 @@ int hcp_device_check(void);                /* HCP_OK iff the current device is c
 unsigned long long hcp_launch_count(void);
 
 /* ------------------------------------------------------------------------------------------------
- * GEMM family (tcgen05 + TMA).  out[M,N] = sum_s A_s[M,K_s] . B_s[N,K_s]^T  (+ epilogue)
+ * GEMM family (wgmma + TMA).  out[M,N] = sum_s A_s[M,K_s] . B_s[N,K_s]^T  (+ epilogue)
  *
  * Replaces: LinearLayer.forward -> torch.mm(x2d, (W_host + dW).T)   hcpdiff/models/lora_layers_patch.py:50-57
  *           LinearLayer.get_weight -> alpha*mm(W_up, W_down)         hcpdiff/models/lora_layers_patch.py:44-45
@@ -85,11 +85,11 @@ typedef struct hcp_gemm_args {
 
 int hcp_gemm_bf16(const hcp_gemm_args* args, hcp_stream_t stream);
 /* Bytes of fp32 scratch that let a GEMM / conv with this output and total reduction extent (sum of K over segments;
- * 9*Cin for a 3x3 conv) split its reduction over several CTAs when the output alone cannot fill 148 SMs; 0 = no split. */
+ * 9*Cin for a 3x3 conv) split its reduction over several CTAs when the output alone cannot fill the SMs; 0 = no split. */
 size_t hcp_splitk_workspace_bytes(int64_t M, int64_t N, int64_t total_k);
 
 /* ------------------------------------------------------------------------------------------------
- * 3x3 convolution as implicit GEMM (tcgen05; the im2col gather is done by 4D/5D TMA boxes with
+ * 3x3 convolution as implicit GEMM (wgmma; the im2col gather is done by 4D/5D TMA boxes with
  * out-of-bounds zero fill standing in for the padding).
  *
  * Replaces: F.conv2d inside diffusers ResnetBlock2D.conv1/conv2, Downsample2D.conv (stride 2),
@@ -124,7 +124,7 @@ typedef struct hcp_conv3x3_args {
 int hcp_conv3x3_bf16(const hcp_conv3x3_args* args, hcp_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
- * Fused attention (tcgen05 flash-style forward, and backward).
+ * Fused attention (wgmma flash-style forward, and backward).
  *
  * Replaces: diffusers Attention -> F.scaled_dot_product_attention / xformers.memory_efficient_attention
  *           (selected at reference hcpdiff/train_ac.py:258-263) for BasicTransformerBlock.attn1 / attn2
@@ -366,7 +366,7 @@ int hcp_cfg_mix_f32(const float* eps2, const float* dout, const int64_t* t, int6
  * (fp32, atomics / read-modify-write) into caller-owned buffers -- the flat gradient buffer of the engine -- so that
  * gradient accumulation over micro-batches needs nothing extra.
  * ---------------------------------------------------------------------------------------------- */
-/* dst[j * ld_j + n * ld_n] += scale * sum_m S[m, j] X[m, n],  j < j_cols, n < n_cols   (tcgen05 TN GEMM; S, X bf16 row-major [M, *])
+/* dst[j * ld_j + n * ld_n] += scale * sum_m S[m, j] X[m, n],  j < j_cols, n < n_cols   (wgmma TN GEMM; S, X bf16 row-major [M, *])
  * nn.Linear weight gradient dW[out, in] = dY^T x:  S = dY (lds = N), X = x (ldx = K), ld_j = K, ld_n = 1. */
 int hcp_wgrad_bf16(const void* S, int64_t lds, int64_t j_cols, const void* X, int64_t ldx, int64_t n_cols, int64_t M, float scale,
                    float* dst, int64_t ld_j, int64_t ld_n, hcp_stream_t stream);

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA (B200) device; run with `pytest -m gpu` on the GPU box")
+    config.addinivalue_line("markers", "gpu: needs a CUDA (H100) device; run with `pytest -m gpu`")
 
 
 @pytest.fixture(scope="session")

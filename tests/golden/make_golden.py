@@ -14,6 +14,7 @@ Outputs (small, committed):
                           pre/post (hcpdiff/models/cfg_context.py), get_cfg_range (hcpdiff/utils/utils.py), and DAPPLayer on a 3x3
                           Conv2d host (batch = [negative | positive])
   lora_webui_keys.json    hcpdiff <-> webui key maps of the REAL reference LoraConverter for the 160 SD1.5 attention/ff LoRA layers
+  ref_lora_wrap_linear.pt LoraLayer.wrap_layer on a biased nn.Linear(40, 24), rank 8, alpha 2.0: weights, input and the wrapped output
 """
 import importlib
 import json
@@ -167,6 +168,23 @@ class _DappConvNet(nn.Module):
         self.conv = nn.Conv2d(8, 16, 3, padding=1)
         self.conv_s2 = nn.Conv2d(8, 16, 3, stride=2, padding=1)
         self.proj = nn.Conv2d(8, 16, 1)
+
+
+def make_wrap_linear():
+    """One reference LoraLayer wrapped around a biased Linear through wrap_layer (alpha auto-scaled by the rank)."""
+    plugin, base, layers = import_reference_lora()
+    torch.manual_seed(3)
+    holder = nn.Module()
+    holder.lin = nn.Linear(40, 24, bias=True)
+    blk = layers.LoraLayer.wrap_layer(0, holder.lin, rank=8, alpha=2.0, parent_block=holder, host_name="lin")
+    with torch.no_grad():
+        blk.layer.W_up.normal_(0, 0.1)
+    x = torch.randn(5, 40)
+    out = holder.lin(x)
+    fx = {"x": x, "weight": holder.lin._host.weight.detach().clone(), "bias": holder.lin._host.bias.detach().clone(),
+          "W_down": blk.layer.W_down.detach().clone(), "W_up": blk.layer.W_up.detach().clone(), "alpha": float(blk.alpha),
+          "out": out.detach().clone()}
+    torch.save(fx, os.path.join(HERE, "ref_lora_wrap_linear.pt"))
 
 
 def make_dapp_conv():
@@ -359,6 +377,7 @@ if __name__ == "__main__":
         sys.exit(0)
     make_struct()
     make_lora()
+    make_wrap_linear()
     make_dapp_conv()
     make_step()
     make_webui_keys()

@@ -1,5 +1,5 @@
 // SPDX-License-Identifier: Apache-2.0
-// Attention fwd/bwd bring-up tests (test infrastructure): tcgen05 kernels vs naive fp32 CUDA-core references.
+// Attention fwd/bwd bring-up tests (test infrastructure): wgmma kernels vs naive fp32 CUDA-core references.
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
 #include <stdio.h>

@@ -1,9 +1,9 @@
 // SPDX-License-Identifier: Apache-2.0
-// Stand-alone bring-up harness for libhcpb200 (no Python, no torch): checks the tcgen05 GEMM / conv kernels
+// Stand-alone bring-up harness for libhcpb200 (no Python, no torch): checks the wgmma GEMM / conv kernels
 // against naive CUDA-core reference kernels on the same GPU and prints achieved TFLOP/s.  Test infrastructure
 // only -- the parity tests proper live in tests/test_*.py and go through the same C ABI.
 //
-//   build: see Makefile in this directory;   run on the GPU box:  timeout 600 tests/native/test_kernels [filter]
+//   build: see Makefile in this directory;   run on an H100:  timeout 600 tests/native/test_kernels [filter]
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
 #include <stdio.h>
@@ -239,7 +239,6 @@ static void run_conv_case(const ConvCase& c) {
     cudaFree(out); cudaFree(ref);
 }
 
-void run_probe_tests(const char* filter, int* pass, int* fail);   // probe_mma.cu
 void run_attn_tests(const char* filter, int* pass, int* fail);    // test_attn.cu (optional, weak)
 __attribute__((weak)) void run_attn_tests(const char*, int*, int*) {}
 
@@ -290,7 +289,6 @@ int main(int argc, char** argv) {
     };
     for (const auto& c : conv_cases) run_conv_case(c);
 
-    run_probe_tests(g_filter, &g_pass, &g_fail);
     run_attn_tests(g_filter, &g_pass, &g_fail);
 
     printf("SUMMARY pass=%d fail=%d\n", g_pass, g_fail);

@@ -1,4 +1,4 @@
-"""The C-ABI library builds for sm_100a without a GPU, loads, and exports every symbol include/hcp_b200.h declares."""
+"""The C-ABI library builds for sm_90a without a GPU, loads, and exports every symbol include/hcp_b200.h declares."""
 import ctypes
 import os
 import re

@@ -256,7 +256,7 @@ def test_train_ac_entrypoint_writes_loadable_checkpoint_and_resumes(tmp_path):
 # ----------------------------------------------------------------------------------------------------------------------
 # data parallel: N ranks over NCCL == 1 rank on the concatenated batch
 # ----------------------------------------------------------------------------------------------------------------------
-@pytest.mark.skipif(not torch.cuda.is_available() or torch.cuda.device_count() < 2, reason="needs 2 GPUs (gpurun --gpus 2)")
+@pytest.mark.skipif(not torch.cuda.is_available() or torch.cuda.device_count() < 2, reason="needs 2 GPUs")
 def test_two_rank_nccl_step_equals_single_rank_on_concatenated_batch(tmp_path):
     out = os.path.join(tmp_path, "dp")
     os.makedirs(out)

@@ -1,4 +1,4 @@
-"""GPU parity tests (run with `pytest -m gpu` on a B200): the CUDA path, called through the C ABI, against
+"""GPU parity tests (run with `pytest -m gpu` on an H100): the CUDA path, called through the C ABI, against
   * plain fp32 PyTorch references of each op (same inputs, bf16-rounded where the kernel rounds),
   * the golden vectors generated from the real reference LoRA classes (tests/golden/ref_lora_linear.pt),
   * the CPU oracle (oracle/unet_ref.py) on the TINY topology and on full-size SD1.5.

@@ -1,4 +1,4 @@
-"""GPU parity tests of the training step either side of the UNet call (`pytest -m gpu` on a B200).
+"""GPU parity tests of the training step either side of the UNet call (`pytest -m gpu` on an H100).
 
 Every kernel of `engine.LoraTrainStep` -- add_noise, the (SNR-weighted) loss and its gradient, the CFG mix, the global-norm
 clip, AdamW, EMA -- against the fp32 oracle (oracle/step_ref.py, itself pinned to vectors of the real reference code in

@@ -1,7 +1,7 @@
 """In-graph micro-benchmarks of the library's kernels at the shapes of the SD1.5 bs=4 step.
 
 ncu launch lists (profiles/*launches*.csv) time every kernel cold and serialised; inside the captured step graph the operands of a
-kernel were just written by its producer and sit in the 126 MB L2.  This script reproduces that regime: every op is captured
+kernel were just written by its producer and sit in the 50 MB L2.  This script reproduces that regime: every op is captured
 REPS times back to back into one CUDA graph, cycling over a small ring of buffers, and the graph replay is timed with CUDA events.
 
   python tools/bench_ops.py [filter-substring]      -> one line per op: us per launch, TF/s or GB/s (algorithmic bytes)

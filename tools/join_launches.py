@@ -19,21 +19,23 @@ kern = [(re.sub(r"\(.*", "", r["Kernel Name"]), float(r["Metric Value"].replace(
 
 # fn -> list of (kernel-name substring, min count, max count), consumed in order
 SEQ = {
-    "hcp_gemm_bf16": [("gemm_tc_kernel", 1, 1), ("splitk_finalize", 0, 1)],
+    "hcp_gemm_bf16": [("gemm_wgmma_kernel", 1, 1), ("splitk_finalize", 0, 1)],
     "hcp_attn_fwd_bf16": [("attn_fwd", 1, 1)],
-    "hcp_attn_bwd_bf16": [("attn_bwd_prep", 1, 1), ("attn_bwd_kernel", 1, 2), ("attn_bwd_post_kernel", 0, 1), ("attn_bwd_post_kv", 0, 1)],
+    # one attn_bwd_kernel launch per 64-column output slice of the head (d <= 192: at most three)
+    "hcp_attn_bwd_bf16": [("attn_bwd_prep", 1, 1), ("attn_bwd_kernel", 1, 3), ("attn_bwd_post_kernel", 1, 1), ("attn_bwd_post_kv", 0, 1)],
     "hcp_groupnorm_fwd_bf16": [("gn", 1, 3)],
     "hcp_groupnorm_bwd_bf16": [("gn", 1, 3)],
     "hcp_lora_grad_pair": [("lora_grad", 1, 1)],
     "hcp_lora_grad": [("lora_grad", 1, 1)],
     "hcp_adamw_flat": [("incr_step", 0, 1), ("adamw", 1, 1)],
+    "hcp_adamw_flat_dev": [("incr_step", 1, 1), ("adamw_flat_dev", 1, 1)],
 }
 
 
 def seq_of(c):
     f = c["fn"]
     if f == "hcp_conv3x3_bf16":
-        return [("gemm_tc_kernel", 4, 4)] if c.get("mode") == 1 else SEQ["hcp_gemm_bf16"]
+        return [("gemm_wgmma_kernel", 4, 4)] if c.get("mode") == 1 else SEQ["hcp_gemm_bf16"]
     return SEQ.get(f, [("", 1, 1)])
 
 

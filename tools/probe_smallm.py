@@ -1,6 +1,6 @@
 """Small-M (weight-streaming) layers, cold vs L2-warm weights, row-major vs k-block-major weight operands.
 
-Every case is captured REPS times into one CUDA graph; `cold` cycles over NW distinct weight packs (NW x weights >> 126 MB L2, the
+Every case is captured REPS times into one CUDA graph; `cold` cycles over NW distinct weight packs (NW x weights >> 50 MB L2, the
 regime of the real step where each layer's weights are read once per pass), `warm` reuses one pack.
 
   python tools/probe_smallm.py            -> table
