@@ -508,7 +508,11 @@ def test_tiny_unet_dapp_and_conv1x1_lora_forward_backward():
     assert math.sqrt(num / den) < 5e-2
 
 
-@pytest.mark.parametrize("B,H,Cin,Cout,stride,ranks", [(2, 16, 64, 128, 1, (4,)), (2, 16, 128, 64, 2, (4, 8)), (1, 32, 64, 64, 1, (8,))])
+# last rows: rank 20 (one slab, 2 of 4 k-steps), rank 80 (R = 128: two slabs, the second one part-filled), 128-wide output maps
+# (one-row 128-pixel boxes) at stride 1 and 2
+@pytest.mark.parametrize("B,H,Cin,Cout,stride,ranks", [(2, 16, 64, 128, 1, (4,)), (2, 16, 128, 64, 2, (4, 8)), (1, 32, 64, 64, 1, (8,)),
+                                                       (1, 16, 64, 128, 1, (20,)), (2, 16, 64, 64, 2, (80,)), (1, 128, 64, 64, 1, (80,)),
+                                                       (1, 256, 64, 64, 2, (20,))])
 def test_conv3x3_lora_fwd_bwd(B, H, Cin, Cout, stride, ranks):
     """Conv2d LoRA (LoCon) on a 3x3 convolution: y = conv(x, W + sum_b alpha_b W_up_b x W_down_b) (reference
     lora_layers_patch.py:91-98) through the factored kernels vs the materialised fp32 formula; x, W_down and W_up gradients."""
