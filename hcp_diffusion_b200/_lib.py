@@ -17,7 +17,7 @@ import torch
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("HCP_LIB", os.path.join(_HERE, "lib", "libhcpb200.so"))     # HCP_LIB: an alternative build (A/B experiments)
 CSRC = os.path.join(_HERE, "csrc")
-SOURCES = ["gemm.cu", "host_util.cu", "attention.cu", "norms.cu", "misc.cu", "step.cu", "wgrad.cu"]
+SOURCES = ["gemm.cu", "host_util.cu", "attention.cu", "norms.cu", "misc.cu", "step.cu", "wgrad.cu", "optim.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "--shared", "-Xcompiler", "-fPIC"]
 
 MAX_SEG = 3
@@ -151,7 +151,7 @@ EXPORTS = [
     "hcp_lora_pack", "hcp_lora_merge", "hcp_lora_pack_conv", "hcp_lora_grad", "hcp_lora_grad_pair", "hcp_lora_grad_conv3x3", "hcp_add_noise", "hcp_mse_loss", "hcp_sumsq", "hcp_adamw_flat",
     "hcp_adamw_flat_dev", "hcp_snr_mse_loss", "hcp_ema_flat", "hcp_dropout_bf16", "hcp_counter_add_u64", "hcp_cfg_mix_f32",
     "hcp_wgrad_bf16", "hcp_wgrad_conv3x3_bf16", "hcp_colsum_bf16", "hcp_norm_affine_grad_bf16", "hcp_small_linear_bwd_f32", "hcp_silu_f32",
-    "hcp_conv_in_wgrad_f32", "hcp_conv_out_wgrad_f32", "hcp_repack_weights",
+    "hcp_conv_in_wgrad_f32", "hcp_conv_out_wgrad_f32", "hcp_repack_weights", "hcp_adafactor_flat",
 ]
 
 
@@ -207,6 +207,7 @@ def lib() -> C.CDLL:
             l.hcp_sumsq.argtypes = [vp, i64, vp, vp]
             l.hcp_adamw_flat.argtypes = [vp, vp, vp, vp, i64, vp, f32, f32, f32, f32, f32, vp, f32, vp, vp]
             l.hcp_adamw_flat_dev.argtypes = [vp, vp, vp, vp, i64, vp, f32, vp, f32, vp, vp]
+            l.hcp_adafactor_flat.argtypes = [vp, vp, vp, vp, vp, vp, vp, i64, vp, i64, vp, vp, C.c_int32, f32, vp, f32, vp]
             l.hcp_snr_mse_loss.argtypes = [vp, vp, vp, vp, f32, C.c_int32, i64, i64, f32, vp, vp, vp]
             l.hcp_ema_flat.argtypes = [vp, vp, i64, vp, f32, f32, f32, vp]
             l.hcp_dropout_bf16.argtypes = [vp, i64, vp, i64, vp, i64, i64, i64, i64, f32, vp, C.c_uint32, vp, i64, vp]

@@ -19,11 +19,12 @@ from __future__ import annotations
 
 from typing import Dict, Iterable, List, Optional, Sequence, Union
 
+import numpy as np
 import torch
 import torch.distributed as dist
 from torch import nn
 
-from . import _lib, ops
+from . import _lib, adafactor, ops
 from ._lib import call, stream_ptr
 
 SNR_LOSS_MODES = {"min_snr": 0, "soft_min_snr": 1, "kdiff_min_snr": 2, "edm": 3,
@@ -168,13 +169,31 @@ class LoraTrainStep:
     (`train.gradient_accumulation_steps`).  `loss`: None / 'mse' or {'type': 'min_snr' | 'soft_min_snr' | 'kdiff_min_snr' | 'edm',
     'gamma': g}.  `ema`: None or {'decay_max', 'inv_gamma', 'power'} (ModelEMA defaults).  `cfg_scale`: None or the reference's
     `train.cfg_scale` string / (lo, hi, fn) for DreamArtist training: the UNet then runs on the doubled batch
-    [latents | latents] against a text embedding of 2B rows [negative | positive]."""
+    [latents | latents] against a text embedding of 2B rows [negative | positive].
+
+    `optimizer`: 'adamw' (torch.optim.AdamW with `lr`, `betas`, `eps`, `weight_decay`) or 'adafactor'
+    (transformers.optimization.Adafactor; `optimizer_kwargs` takes its constructor keys with its defaults -- `lr`, `eps`,
+    `clip_threshold`, `decay_rate`, `beta1`, `weight_decay`, `scale_parameter`, `relative_step`, `warmup_init` -- and a group's own
+    'lr' / 'weight_decay' win over them).  Adafactor keeps factored second moments per tensor of the module's shape (state sized by
+    adafactor.state_numel), plus one flat first-moment buffer only when `beta1` is set."""
 
     def __init__(self, unet: nn.Module, params: Union[Iterable[nn.Parameter], Sequence[dict]], lr: float = 1e-4, betas=(0.9, 0.999),
                  eps: float = 1e-8, weight_decay: float = 1e-2, max_grad_norm: float = 1.0, use_cuda_graph: bool = True,
                  process_group: Optional[dist.ProcessGroup] = None, side_stream: bool = True, grad_accum_steps: int = 1,
-                 loss: Union[None, str, dict] = None, ema: Optional[dict] = None, cfg_scale=None, num_train_timesteps: int = 1000):
+                 loss: Union[None, str, dict] = None, ema: Optional[dict] = None, cfg_scale=None, num_train_timesteps: int = 1000,
+                 optimizer: str = "adamw", optimizer_kwargs: Optional[dict] = None):
         self.unet = unet
+        if optimizer not in ("adamw", "adafactor"):
+            raise ValueError(f"optimizer {optimizer!r}: one of 'adamw', 'adafactor'")
+        self.optimizer = optimizer
+        af_opts = None
+        if optimizer == "adafactor":
+            af_opts = adafactor.check_options(optimizer_kwargs)
+            weight_decay = af_opts["weight_decay"]
+            if af_opts["lr"] is not None:
+                lr = af_opts["lr"]
+        elif optimizer_kwargs:
+            raise ValueError("optimizer_kwargs are the Adafactor options; AdamW takes lr / betas / eps / weight_decay")
         params = list(params)
         if params and isinstance(params[0], dict):
             groups = [{"params": list(g["params"]), "lr": float(g.get("lr", lr)), "weight_decay": float(g.get("weight_decay", weight_decay))}
@@ -188,8 +207,12 @@ class LoraTrainStep:
             flat_list += g["params"]
         self.flat = FlatParams(flat_list)
         dev = self.flat.data.device
-        self.m = torch.zeros_like(self.flat.data)
-        self.v = torch.zeros_like(self.flat.data)
+        self.m = self.v = None
+        if af_opts is not None:
+            self._init_adafactor(groups, af_opts)
+        else:
+            self.m = torch.zeros_like(self.flat.data)
+            self.v = torch.zeros_like(self.flat.data)
         # parameter groups = contiguous segments of the flat buffer, each with a device-side lr and step counter
         self.segments, i0 = [], 0
         for g in groups:
@@ -197,9 +220,13 @@ class LoraTrainStep:
             if n == 0:
                 continue
             lo, hi = self.flat.offsets[i0], self.flat.end_of(i0 + n - 1)
-            hyper = torch.tensor([g["lr"], betas[0], betas[1], eps, g["weight_decay"]], dtype=torch.float32, device=dev)
-            self.segments.append({"lo": lo, "hi": hi, "hyper": hyper, "lr": hyper[0:1], "base_lr": g["lr"],
-                                  "step": torch.zeros(1, dtype=torch.int32, device=dev)})
+            if af_opts is not None:                        # rows of the [groups, 8] table the Adafactor kernels read
+                gi = len(self.segments)
+                hyper, step = self.af_hyper[gi], self.af_steps[gi:gi + 1]
+            else:
+                hyper = torch.tensor([g["lr"], betas[0], betas[1], eps, g["weight_decay"]], dtype=torch.float32, device=dev)
+                step = torch.zeros(1, dtype=torch.int32, device=dev)
+            self.segments.append({"lo": lo, "hi": hi, "hyper": hyper, "lr": hyper[0:1], "base_lr": g["lr"], "step": step})
             i0 += n
         self.lr = self.segments[0]["lr"]
         self.step_count = self.segments[0]["step"]
@@ -244,6 +271,34 @@ class LoraTrainStep:
         # _forward_backward and is joined there, before anything reads the gradients (HCP_SIDE_STREAM=0 keeps a single stream)
         self.side_stream = side_stream
 
+    def _init_adafactor(self, groups, opts):
+        dev = self.flat.data.device
+        groups = [g for g in groups if g["params"]]          # the segments: a group emptied by de-duplication has none
+        group_of = [gi for gi, g in enumerate(groups) for _ in g["params"]]
+        self.af_layout = adafactor.Layout([tuple(p.shape) for p in self.flat.params], self.flat.offsets, group_of)
+        lay = self.af_layout
+        rows = [adafactor.hyper_row(opts, g["lr"], g["weight_decay"]) for g in groups]
+        self.af_hyper = torch.tensor(rows, dtype=torch.float32, device=dev)
+        self.af_steps = torch.zeros(len(groups), dtype=torch.int32, device=dev)
+        self.af_state = torch.zeros(lay.state_numel, dtype=torch.float32, device=dev)
+        self.af_exp_avg = torch.zeros_like(self.flat.data) if opts["beta1"] is not None else None
+        self.af_work = torch.zeros(lay.work_numel, dtype=torch.float32, device=dev)
+        to_dev = lambda a: torch.from_numpy(a.view(np.uint8).copy()).to(dev)      # noqa: E731  (packed C structs)
+        self.af_tensors, self.af_items = to_dev(lay.tensors), to_dev(lay.items)
+        self.af_factor_items = to_dev(lay.factor_items) if lay.factor_items.size else None
+
+    @property
+    def optimizer_state_bytes(self) -> int:
+        """Bytes of optimizer state (moments; not the parameters, gradients or scratch)."""
+        if self.optimizer == "adafactor":
+            return 4 * (self.af_state.numel() + (0 if self.af_exp_avg is None else self.af_exp_avg.numel()))
+        return 4 * (self.m.numel() + self.v.numel())
+
+    def _opt_buffers(self) -> List[torch.Tensor]:
+        if self.optimizer == "adafactor":
+            return [self.af_state, self.af_steps] + ([] if self.af_exp_avg is None else [self.af_exp_avg])
+        return [self.m, self.v] + [s["step"] for s in self.segments]
+
     def set_lr(self, lr: float, group: Optional[int] = None):
         """Set the lr of one group, or scale every group's configured lr by lr / base lr of group 0 (what an LR scheduler does)."""
         if group is not None:
@@ -259,6 +314,8 @@ class LoraTrainStep:
         if lr is not None:
             h[0:1].fill_(lr)
         if beta1 is not None:
+            if self.optimizer != "adamw":
+                raise ValueError("beta1 is scheduled for AdamW only")
             h[1:2].fill_(beta1)
 
     def sync_params(self, src: int = 0):
@@ -313,7 +370,13 @@ class LoraTrainStep:
         self.gsq.zero_()
         n = self.flat.numel
         call("hcp_sumsq", self.flat.grad.data_ptr(), n, self.gsq.data_ptr(), stream_ptr())
-        for s in self.segments:
+        if self.optimizer == "adafactor":
+            lay = self.af_layout
+            call("hcp_adafactor_flat", self.flat.data.data_ptr(), self.flat.grad.data_ptr(), self.af_state.data_ptr(),
+                 _lib.ptr(self.af_exp_avg), self.af_work.data_ptr(), self.af_tensors.data_ptr(), self.af_items.data_ptr(), lay.items.size,
+                 _lib.ptr(self.af_factor_items), lay.factor_items.size, self.af_hyper.data_ptr(), self.af_steps.data_ptr(),
+                 len(self.segments), 1.0 / self.world, self.gsq.data_ptr(), float(self.max_norm or 0.0), stream_ptr())
+        for s in (self.segments if self.optimizer == "adamw" else ()):
             lo, cnt = s["lo"], s["hi"] - s["lo"]
             call("hcp_adamw_flat_dev", self.flat.data.data_ptr() + 4 * lo, self.flat.grad.data_ptr() + 4 * lo, self.m.data_ptr() + 4 * lo,
                  self.v.data_ptr() + 4 * lo, cnt, s["hyper"].data_ptr(), 1.0 / self.world, self.gsq.data_ptr(), float(self.max_norm or 0.0),
@@ -379,16 +442,16 @@ class LoraTrainStep:
         return {p: self.ema[o:o + p.numel()].view_as(p) for p, o in zip(self.flat.params, self.flat.offsets)}
 
     def _snapshot(self):
-        return (self.flat.data.clone(), self.m.clone(), self.v.clone(), [s["step"].clone() for s in self.segments],
+        return (self.flat.data.clone(), [b.clone() for b in self._opt_buffers()],
                 None if self.ema is None else self.ema.clone(), ops.dropout_state_snapshot())
 
     def _restore(self, saved):
-        self.flat.data.copy_(saved[0]); self.m.copy_(saved[1]); self.v.copy_(saved[2])
-        for s, c in zip(self.segments, saved[3]):
-            s["step"].copy_(c)
+        self.flat.data.copy_(saved[0])
+        for b, c in zip(self._opt_buffers(), saved[1]):
+            b.copy_(c)
         if self.ema is not None:
-            self.ema.copy_(saved[4])
-        ops.dropout_state_restore(saved[5])
+            self.ema.copy_(saved[2])
+        ops.dropout_state_restore(saved[3])
         self.flat.grad.zero_()
 
     def _capture(self, latents, noise, t, ehs, added=None):

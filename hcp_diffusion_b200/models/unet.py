@@ -450,7 +450,9 @@ class UNet2DConditionModel(nn.Module):
                tuple((self._temb_host(r).weight._version, self._temb_host(r).weight.data_ptr(), self._temb_host(r).weight.requires_grad,
                       id(r.time_emb_proj), tuple(getattr(r.time_emb_proj, "plugin_names", ()))) for r in resnets),
                te.linear_1.weight.requires_grad, te.linear_2.weight.requires_grad, self.conv_in.weight.requires_grad,
-               self.conv_out.weight.requires_grad, self.conv_in.weight.data_ptr(), self.conv_out.weight.data_ptr())
+               self.conv_out.weight.requires_grad, self.conv_in.weight.data_ptr(), self.conv_out.weight.data_ptr(),
+               tuple((lin.weight.requires_grad, lin.bias.requires_grad, lin.weight.data_ptr()) for lin in
+                     ((self.add_embedding.linear_1, self.add_embedding.linear_2) if hasattr(self, "add_embedding") else ())))
         if rt is None or rt.sig != sig:
             from .lora import DAPPPatchContainer, LoraPatchContainer
             for p in (te.linear_1, te.linear_2):
@@ -477,15 +479,25 @@ class UNet2DConditionModel(nn.Module):
             rt.w2 = te.linear_2.weight.detach().to(torch.bfloat16).contiguous()
             rt.b2 = te.linear_2.bias.detach().float().contiguous()
             rt.add = None
+            rt.add_unfused = False
             if hasattr(self, "add_embedding"):
-                # emb = time_embedding(t) + add_embedding(cat[text_embeds, sinusoid(time_ids)]): the two second linears are one
-                # skinny GEMM over the concatenated hidden vectors [e1 | a1] with W = [W2 | Wa2], b = b2 + ba2
                 ae = self.add_embedding
                 for p in (ae.linear_1, ae.linear_2):
-                    if not isinstance(p, nn.Linear) or p.weight.requires_grad:
-                        raise NotImplementedError("plugins / training on the additional-embedding layers are not supported on the H100 hot path")
-                if rt.train_time:
-                    raise NotImplementedError("training the time embedding of a UNet with an additional (text_time) embedding is not supported")
+                    if not isinstance(p, nn.Linear):
+                        raise NotImplementedError("plugins on the additional-embedding layers are not supported on the H100 hot path")
+                train_add = any(q.requires_grad for lin in (ae.linear_1, ae.linear_2) for q in (lin.weight, lin.bias))
+                rt.add_unfused = rt.train_time or train_add
+            if rt.add_unfused:
+                # training (full fine-tune of an SDXL UNet): emb = silu(linear_2(e1) + add_embedding.linear_2(a1)) as two small
+                # linears with autograd nodes; the trained add-embedding operands are refreshed every step like the time MLP's
+                rt.add = SimpleNamespace(
+                    w1=ae.linear_1.weight.detach().to(torch.bfloat16).contiguous(), b1=ae.linear_1.bias.detach().float().clone(),
+                    w2=ae.linear_2.weight.detach().to(torch.bfloat16).contiguous(), b2=ae.linear_2.bias.detach().float().clone(),
+                    l1=[(ae.linear_1.weight, ae.linear_1.bias, 0, ae.linear_1.weight.shape[0])] if train_add else None,
+                    l2=[(ae.linear_2.weight, ae.linear_2.bias, 0, ae.linear_2.weight.shape[0])] if train_add else None)
+            elif hasattr(self, "add_embedding"):
+                # emb = time_embedding(t) + add_embedding(cat[text_embeds, sinusoid(time_ids)]): the two second linears are one
+                # skinny GEMM over the concatenated hidden vectors [e1 | a1] with W = [W2 | Wa2], b = b2 + ba2
                 rt.add = SimpleNamespace(
                     w1=ae.linear_1.weight.detach().to(torch.bfloat16).contiguous(), b1=ae.linear_1.bias.detach().float().contiguous(),
                     w2cat=torch.cat([te.linear_2.weight.detach(), ae.linear_2.weight.detach()], 1).to(torch.bfloat16).contiguous(),
@@ -499,12 +511,13 @@ class UNet2DConditionModel(nn.Module):
             rt.offs = offs
             rt.repack = _JobTable()
             rt.time_jobs = []
+
+            def job(kind, src, dst, rows, K, o0):
+                j = _lib.RepackJob()
+                j.src, j.dst0, j.dst1 = src.data_ptr(), dst.data_ptr(), None
+                j.kind, j.rows, j.K, j.o0, j.n_tot, j.flip = kind, rows, K, o0, 0, 0
+                return j
             if rt.train_time:
-                def job(kind, src, dst, rows, K, o0):
-                    j = _lib.RepackJob()
-                    j.src, j.dst0, j.dst1 = src.data_ptr(), dst.data_ptr(), None
-                    j.kind, j.rows, j.K, j.o0, j.n_tot, j.flip = kind, rows, K, o0, 0, 0
-                    return j
                 for lin, wdst, bdst in ((te.linear_1, rt.w1, rt.b1), (te.linear_2, rt.w2, rt.b2)):
                     rt.time_jobs += [job(3, lin.weight, wdst, lin.weight.shape[0], lin.weight.shape[1], 0),
                                      job(2, lin.bias, bdst, lin.bias.shape[0], 1, 0)]
@@ -518,6 +531,10 @@ class UNet2DConditionModel(nn.Module):
                     l1=[(te.linear_1.weight, te.linear_1.bias, 0, te.linear_1.weight.shape[0])],
                     l2=[(te.linear_2.weight, te.linear_2.bias, 0, te.linear_2.weight.shape[0])],
                     proj=[(self._temb_host(r).weight, self._temb_host(r).bias, a, b - a) for r, (a, b) in zip(resnets, offs)])
+            if rt.add_unfused and rt.add.l1 is not None:
+                for lin, wdst, bdst in ((ae.linear_1, rt.add.w1, rt.add.b1), (ae.linear_2, rt.add.w2, rt.add.b2)):
+                    rt.time_jobs += [job(3, lin.weight, wdst, lin.weight.shape[0], lin.weight.shape[1], 0),
+                                     job(2, lin.bias, bdst, lin.bias.shape[0], 1, 0)]
             rt.w_in = self.conv_in.weight.detach().float().permute(1, 2, 3, 0).contiguous()       # tap-major [Cin,3,3,Cout]
             rt.b_in = self.conv_in.bias.detach().float().contiguous()
             rt.w_out = self.conv_out.weight.detach().float().permute(2, 3, 0, 1).contiguous()     # tap-major [3,3,Cout,Cin]
@@ -525,6 +542,19 @@ class UNet2DConditionModel(nn.Module):
             rt.jobs = _JobTable()
             self.__dict__["_rt"] = rt
         return rt
+
+    def _add_input(self, added, B, dev) -> torch.Tensor:
+        """cat[text_embeds, sinusoid(time_ids)] [B, projection_class_embeddings_input_dim], fp32 (the add_embedding input)."""
+        te_, ids = added["text_embeds"], added["time_ids"]
+        cfg = self.config
+        P_, D_ = cfg.projection_class_embeddings_input_dim, cfg.addition_time_embed_dim
+        n_ids = ids.shape[-1]
+        if te_.shape[-1] + n_ids * D_ != P_:
+            raise ValueError(f"text_embeds ({te_.shape[-1]}) + time_ids ({n_ids} x {D_}) do not add up to {P_}")
+        addin = torch.empty((B, P_), dtype=torch.float32, device=dev)
+        addin[:, :te_.shape[-1]].copy_(te_)                           # boundary copy; the sinusoids are written next to it
+        ops.sinusoid(ids.to(dev, torch.float32).reshape(-1).contiguous(), D_, n_ids, addin, te_.shape[-1])
+        return addin
 
     def forward(self, sample: torch.Tensor, timestep, encoder_hidden_states: torch.Tensor,
                 encoder_attention_mask: Optional[torch.Tensor] = None, return_dict: bool = True, **kwargs):
@@ -569,7 +599,15 @@ class UNet2DConditionModel(nn.Module):
         if t.dim() == 0:
             t = t[None]
         t = t.expand(B).to(torch.float32).contiguous()
-        if rt.train_time:
+        if rt.add_unfused:
+            x0 = torch.empty((B, self.time_proj.num_channels), dtype=torch.float32, device=dev)
+            ops.sinusoid(t, self.time_proj.num_channels, 1, x0, 0)
+            lists = rt.train_lists if rt.train_time else None
+            e1 = ops.small_linear(x0, rt.w1, rt.b1, True, lists and lists.l1)
+            a1 = ops.small_linear(self._add_input(added, B, dev), rt.add.w1, rt.add.b1, True, rt.add.l1)
+            z = ops.small_linear(e1, rt.w2, rt.b2, False, lists and lists.l2) + ops.small_linear(a1, rt.add.w2, rt.add.b2, False, rt.add.l2)
+            emb = ops.silu(z)
+        elif rt.train_time:
             x0 = torch.empty((B, self.time_proj.num_channels), dtype=torch.float32, device=dev)
             ops.sinusoid(t, self.time_proj.num_channels, 1, x0, 0)
             e1 = ops.small_linear(x0, rt.w1, rt.b1, True, rt.train_lists.l1)
@@ -579,19 +617,12 @@ class UNet2DConditionModel(nn.Module):
             emb = ops.skinny_linear(e1, rt.w2, rt.b2, 0, True)           # silu(linear_2(.)): every consumer applies SiLU first
         else:
             e1 = ops.skinny_linear(t, rt.w1, rt.b1, 2, True)
-            te_, ids = added["text_embeds"], added["time_ids"]
-            cfg = self.config
-            P_, D_ = cfg.projection_class_embeddings_input_dim, cfg.addition_time_embed_dim
-            n_ids = ids.shape[-1]
-            if te_.shape[-1] + n_ids * D_ != P_:
-                raise ValueError(f"text_embeds ({te_.shape[-1]}) + time_ids ({n_ids} x {D_}) do not add up to {P_}")
-            addin = torch.empty((B, P_), dtype=torch.float32, device=dev)
-            addin[:, :te_.shape[-1]].copy_(te_)                           # boundary copy; the sinusoids are written next to it
-            ops.sinusoid(ids.to(dev, torch.float32).reshape(-1).contiguous(), D_, n_ids, addin, te_.shape[-1])
-            a1 = ops.skinny_linear(addin, rt.add.w1, rt.add.b1, 0, True)  # silu(add_embedding.linear_1(.))
+            a1 = ops.skinny_linear(self._add_input(added, B, dev), rt.add.w1, rt.add.b1, 0, True)  # silu(add_embedding.linear_1(.))
             emb = ops.skinny_linear(torch.cat([e1, a1], 1), rt.add.w2cat, rt.add.b2sum, 0, True)   # silu(linear_2(e1) + add.linear_2(a1))
-        if rt.train_time:
-            temb_all = ops.small_linear(emb, rt.wp, rt.bp, False, rt.train_lists.proj)
+        if rt.train_time or rt.add_unfused:
+            # an autograd node whenever emb carries a gradient: the trained add_embedding needs dL/demb even when every
+            # time_emb_proj is frozen
+            temb_all = ops.small_linear(emb, rt.wp, rt.bp, False, rt.train_lists.proj if rt.train_time else None)
         else:
             temb_all = ops.skinny_linear(emb, rt.wp, rt.bp, 0, False)    # all 22 time_emb_proj layers at once
         temb_list = [temb_all[:, a:b] for a, b in rt.offs]

@@ -1218,6 +1218,30 @@ class SmallLinearFn(torch.autograd.Function):
         return None, None, None, None, None, dx
 
 
+class SiluFn(torch.autograd.Function):
+    """y = silu(z) on fp32 rows: the summed time and additional embeddings of a text_time UNet whose embeddings are trained."""
+
+    @staticmethod
+    def forward(ctx, z: torch.Tensor):
+        z = z.float().contiguous()
+        y = torch.empty_like(z)
+        call("hcp_silu_f32", z.data_ptr(), None, z.numel(), y.data_ptr(), stream_ptr())
+        ctx.save_for_backward(z)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        (z,) = ctx.saved_tensors
+        dy = dy.float().contiguous()
+        dz = torch.empty_like(z)
+        call("hcp_silu_f32", z.data_ptr(), dy.data_ptr(), z.numel(), dz.data_ptr(), stream_ptr())
+        return dz
+
+
+def silu(z: torch.Tensor) -> torch.Tensor:
+    return SiluFn.apply(z)
+
+
 def small_linear(x, w_bf16, bias, silu, train=None):
     anchor = train[0][0] if train else None
     return SmallLinearFn.apply(w_bf16, bias, silu, train, anchor, x)

@@ -5,13 +5,15 @@ the hot path: build the UNet (cfg `model.unet`, the reference's injection seam t
 training) and `lora_unet:` lists through `make_hcpdiff` (train_ac.py:324-359), then run `train.train_steps` optimizer steps with
 the H100 engine and save `ckpts/unet-<step>.safetensors` every `train.save_step` in the reference checkpoint format
 (train_ac.py:523-544).  Honoured `train.*` keys: `gradient_accumulation_steps`, `max_grad_norm`, `scale_lr`, `optimizer.{lr,
-weight_decay, betas, eps}`, `scheduler.{name, num_warmup_steps, num_training_steps, scheduler_kwargs}` (one_cycle / constant /
+weight_decay, betas, eps}` for `torch.optim.AdamW` (the default `_target_`) or the constructor keys of
+`transformers.optimization.Adafactor` (reference cfgs/train/examples/FT_sdxl.yaml), `scheduler.{name, num_warmup_steps, num_training_steps, scheduler_kwargs}` (one_cycle / constant /
 constant_with_warmup), `loss.criterion` (`torch.nn.MSELoss` or `hcpdiff.loss.MinSNRLoss`-family `_target_` + `gamma`), `cfg_scale`
 (DreamArtist), `resume.{ckpt_path.unet, start_step}`; `model.ema` (`decay_max`, `inv_gamma`, `power`).
 
 Out of the hot path and therefore NOT here: datasets / buckets / captions, the CLIP text encoder, VAE, loggers, DeepSpeed /
 Colossal-AI trainers.  Inputs are the synthetic latents / text embeddings of SURVEY.md 8d (`data.synthetic`), or tensors saved
-in a .pt file (`data.path`: {'latents': [N,4,h,w], 'encoder_hidden_states': [N,L,768]}).
+in a .pt file (`data.path`: {'latents': [N,4,h,w], 'encoder_hidden_states': [N,L,768]}, plus 'text_embeds' / 'time_ids' for an
+SDXL ('text_time') UNet, whose synthetic time ids are (H, W, 0, 0, H, W) in pixels).
 
 Launch data-parallel with torchrun (one process per GPU); gradients are all-reduced over NCCL, every replica starts from rank
 0's parameters (DDP's construction-time broadcast), the learning rate is scaled by batch x world x accumulation when
@@ -27,6 +29,7 @@ import time
 import torch
 import torch.distributed as dist
 
+from . import adafactor
 from .ckpt_manager import CkptManagerPKL, CkptManagerSafe, auto_manager
 from .engine import LoraTrainStep
 from .utils.cfg_net_tools import load_lora_state, make_hcpdiff
@@ -51,6 +54,32 @@ def loss_from_cfg(loss_cfg):
     raise NotImplementedError(f"train.loss.criterion {target!r} is not supported on the H100 hot path")
 
 
+def optimizer_from_cfg(opt_cfg):
+    """`train.optimizer` -> (engine optimizer, Adafactor options or None).  No `_target_` or torch.optim.AdamW: AdamW from `lr /
+    weight_decay / betas / eps`; transformers.optimization.Adafactor: its constructor keys with transformers' defaults (a manual
+    `lr` with `relative_step: True` is refused, as transformers refuses it)."""
+    target = str((opt_cfg or {}).get("_target_", "torch.optim.AdamW"))
+    name = target.rsplit(".", 1)[-1]
+    if name == "AdamW" and target.startswith("torch."):
+        return "adamw", None
+    if name == "Adafactor" and target.startswith("transformers."):
+        kw = {k: v for k, v in opt_cfg.items() if k not in ("_target_", "_partial_")}
+        if "eps" in kw:
+            kw["eps"] = tuple(kw["eps"])
+        return "adafactor", adafactor.check_options(kw)
+    raise NotImplementedError(f"train.optimizer._target_={target!r}: torch.optim.AdamW or transformers.optimization.Adafactor")
+
+
+class _LrOnly(torch.optim.Optimizer):
+    """Stand-in for an optimizer without momentum or betas (Adafactor): the schedulers see what they would see on it."""
+
+    def __init__(self, groups):
+        super().__init__(groups, {"lr": groups[0]["lr"]})
+
+    def step(self, closure=None):
+        return None
+
+
 def make_scheduler(cfg, step_fn: LoraTrainStep):
     """Reference get_scheduler_with_name (hcpdiff/utils/net_utils.py:22-82) driven on a stand-in optimizer with the engine's groups:
     the real torch schedulers produce the numbers, `step()` copies lr (and OneCycleLR's cycled beta1) to the device."""
@@ -60,7 +89,11 @@ def make_scheduler(cfg, step_fn: LoraTrainStep):
     warm, total = int(cfg.get("num_warmup_steps", 0)), int(cfg.get("num_training_steps", 1))
     kwargs = dict(cfg.get("scheduler_kwargs") or {})
     dummy = [torch.nn.Parameter(torch.zeros(1)) for _ in step_fn.segments]
-    opt = torch.optim.AdamW([{"params": [d], "lr": s["base_lr"]} for d, s in zip(dummy, step_fn.segments)], betas=tuple(step_fn.betas))
+    adamw = step_fn.optimizer == "adamw"
+    if adamw:
+        opt = torch.optim.AdamW([{"params": [d], "lr": s["base_lr"]} for d, s in zip(dummy, step_fn.segments)], betas=tuple(step_fn.betas))
+    else:                                       # Adafactor has no betas: OneCycleLR's cycle_momentum fails as it does in torch
+        opt = _LrOnly([{"params": [d], "lr": s["base_lr"]} for d, s in zip(dummy, step_fn.segments)])
     if name == "one_cycle":
         sched = torch.optim.lr_scheduler.OneCycleLR(opt, max_lr=[s["base_lr"] for s in step_fn.segments], steps_per_epoch=total, epochs=1,
                                                     pct_start=warm / max(total, 1), **kwargs)
@@ -73,7 +106,7 @@ def make_scheduler(cfg, step_fn: LoraTrainStep):
 
     def push():
         for i, g in enumerate(opt.param_groups):
-            step_fn.set_hyper(i, lr=float(g["lr"]), beta1=float(g["betas"][0]))
+            step_fn.set_hyper(i, lr=float(g["lr"]), beta1=float(g["betas"][0]) if adamw else None)
 
     def step():
         opt.step()              # keeps torch's "optimizer.step() before lr_scheduler.step()" contract on the stand-in
@@ -119,6 +152,7 @@ class Trainer:
         accum = int(tr.get("gradient_accumulation_steps", 1))
         lr_scale = bs * self.world * accum if tr.get("scale_lr", False) else 1
         opt_cfg = tr.get("optimizer") or {}
+        opt_name, af_opts = optimizer_from_cfg(opt_cfg)
         groups, self.lora = make_hcpdiff(self.unet, cfgs.get("unet"), cfgs.get("lora_unet"), default_lr=float(opt_cfg.get("lr", 1e-4)))
         groups = [{"params": g["params"], "lr": float(g["lr"]) * lr_scale} for g in groups if len(g["params"])]
         resume = tr.get("resume")
@@ -141,7 +175,8 @@ class Trainer:
                                      betas=tuple(opt_cfg.get("betas", (0.9, 0.999))), eps=float(opt_cfg.get("eps", 1e-8)),
                                      max_grad_norm=float(tr.get("max_grad_norm", 1.0)), use_cuda_graph=bool(tr.get("cuda_graph", True)),
                                      grad_accum_steps=accum, loss=loss_from_cfg(tr.get("loss")), ema=ema,
-                                     cfg_scale=None if cfg_scale in (None, "1.0", 1.0) else str(cfg_scale))
+                                     cfg_scale=None if cfg_scale in (None, "1.0", 1.0) else str(cfg_scale),
+                                     optimizer=opt_name, optimizer_kwargs=af_opts)
         self.step_fn.sync_params(src=0)
         self.sched_step = make_scheduler(tr.get("scheduler"), self.step_fn)
         self.bs, self.accum = bs, accum
@@ -157,10 +192,15 @@ class Trainer:
     def _load_data(self, seed: int):
         d = self.cfgs.data
         g = torch.Generator().manual_seed(1234 + self.rank)
+        cfg = self.unet.config
+        self.text_time = getattr(cfg, "addition_embed_type", None) == "text_time"
+        self.text_embeds = self.time_ids = None
         if d.get("path"):
             blob = torch.load(d.path, map_location="cpu")
             self.latents, self.ehs = blob["latents"].float(), blob["encoder_hidden_states"].float()
             self.ehs_neg = blob.get("negative_hidden_states")
+            if self.text_time:
+                self.text_embeds, self.time_ids = blob["text_embeds"].float(), blob["time_ids"].float()
         else:
             n = int(d.get("num_samples", 64))
             s = int(self.unet.config.sample_size)
@@ -168,6 +208,12 @@ class Trainer:
             self.latents = torch.randn((n, self.unet.config.in_channels, s, s), generator=gd)
             self.ehs = torch.randn((n, int(d.get("tokens", 77)), self.unet.config.cross_attention_dim), generator=gd)
             self.ehs_neg = torch.randn((n, int(d.get("tokens", 77)), self.unet.config.cross_attention_dim), generator=gd)
+            if self.text_time:                                   # pooled text embedding ~ N(0,1); (H, W, 0, 0, H, W) in pixels
+                n_ids = 6
+                self.text_embeds = torch.randn((n, cfg.projection_class_embeddings_input_dim - n_ids * cfg.addition_time_embed_dim),
+                                               generator=gd)
+                px = float(s * 8)
+                self.time_ids = torch.tensor([[px, px, 0.0, 0.0, px, px]]).repeat(n, 1)
         self.gen = g
 
     def next_batch(self):
@@ -178,7 +224,10 @@ class Trainer:
             ehs = torch.cat([neg, ehs], 0)
         noise = torch.randn(lat.shape, generator=self.gen)
         t = torch.randint(0, 1000, (self.bs,), generator=self.gen, dtype=torch.int64)
-        return [x.pin_memory() for x in (lat, noise, t, ehs)]
+        batch = [x.pin_memory() for x in (lat, noise, t, ehs)]
+        if self.text_time:
+            batch.append({"text_embeds": self.text_embeds[idx].pin_memory(), "time_ids": self.time_ids[idx].pin_memory()})
+        return batch
 
     def save(self, step: int):
         base_trained = any(p.requires_grad for n, p in self.unet.named_parameters() if "lora_block_" not in n)

@@ -333,6 +333,37 @@ int hcp_adamw_flat(float* p, const float* g, float* m, float* v, int64_t n, cons
 int hcp_adamw_flat_dev(float* p, const float* g, float* m, float* v, int64_t n, const float* hyper_device, float grad_scale,
                        const float* sumsq_device, float max_norm, int* step_device, hcp_stream_t stream);
 
+/* Adafactor (transformers.optimization.Adafactor.step) over the flat buffer, per tensor of the module's shape.  A tensor with two or
+ * more dims is factored over its last two: view [P, R, C], exp_avg_sq_row [P, R] at state+row, exp_avg_sq_col [P, C] at state+col.
+ * A 1-D tensor has exp_avg_sq [numel] at state+row, and is walked as P = 1, R = ceil(numel / 256), C = 256. */
+typedef struct {
+    int64_t offset;     /* first element in p, g and exp_avg */
+    int64_t numel;
+    int64_t P, R, C;
+    int64_t row, col;   /* state offsets (col = -1 when not factored) */
+    int64_t rowpart;    /* work offset of the partial row sums [P*R, nct] (used when nct > 1) */
+    int64_t colpart;    /* work offset of the partial column sums [nrch, P*C] (used when nrch > 1) */
+    int64_t rmean;      /* work offset of mean_R(exp_avg_sq_row) [P] (factored) */
+    int32_t factored, group;
+    int32_t nct, nrch;  /* column tiles of 256 (wide rows) and row chunks of 256 of the tensor's items */
+    int32_t item0, nitems;  /* the tensor's range in the item list */
+} hcp_adafactor_tensor;
+/* One CTA of 256 threads: slabs [p0, p1), columns [c0, c1) (c1 - c0 <= 256; columns of 256 / (c1 - c0) slabs side by side), rows
+ * [r0, r1) (at most 256, starting at a multiple of 256; wide column tiles start at a multiple of 256).  Factor items (pass b): mode 0
+ * one CTA for slab p0, mode 1 one thread per slab of [p0, p1). */
+typedef struct {
+    int32_t tensor, p0, p1, c0, c1, r0, r1, mode;
+} hcp_adafactor_item;
+/* hyper_device: fp32 [ngroups, 8] = {lr, eps1, eps2, clip_threshold, decay_rate, beta1, weight_decay, flags} with flags = 1
+ * scale_parameter | 2 relative_step | 4 warmup_init | 8 beta1 set; steps_device int32 [ngroups] (incremented here).  work: fp32,
+ * [2 * nitems] tile partial sums followed by the per-tensor scratch the table points at.  exp_avg (flat, like p) may be NULL when
+ * no group sets beta1.  The gradient is g * grad_scale, clipped to max_norm with the device-side sumsq (as hcp_adamw_flat_dev).
+ * Five launches whatever the tensor count; no host synchronisation (CUDA-graph capturable). */
+int hcp_adafactor_flat(float* p, const float* g, float* state, float* exp_avg, float* work, const hcp_adafactor_tensor* tensors_device,
+                       const hcp_adafactor_item* items_device, int64_t nitems, const hcp_adafactor_item* factor_items_device,
+                       int64_t nfactor_items, const float* hyper_device, int* steps_device, int32_t ngroups, float grad_scale,
+                       const float* sumsq_device, float max_norm, hcp_stream_t stream);
+
 /* SNR-weighted eps loss (reference hcpdiff/loss/min_snr_loss.py:5-52): loss_sum += mean_i(w(t_b) (pred_i - target_i)^2),
  * dpred_i = 2 w d grad_scale / n;  snr = acp/(1-acp);  mode 0 MinSNRLoss w = min(gamma/snr, 1), 1 SoftMinSNRLoss, 2 KDiffMinSNRLoss,
  * 3 EDMLoss.  t int64 [n / per_image]. */

@@ -1,8 +1,10 @@
 """BASELINE config 4 on one H100: SDXL-base UNet (2.57 B parameters, random init), LoRA rank 16 on every attn / ff Linear and on the
 resnet / sampler convolutions (locon), batch 2, 1024x1024 (128x128 latent), 77 tokens x 2048.  Prints one JSON line with the step
 time.  Not the benchmark contract (bench.py measures config 2); a reference point for the SDXL rows of DESIGN.md.
+`--full-ft` trains every parameter of the UNet instead (reference cfgs/train/examples/FT_sdxl.yaml), with `--optimizer adamw` or
+`adafactor` (relative_step False, lr 1e-6, weight_decay 1e-3 as there); the line then also gives the optimizer's own time per step.
 
-  python tools/bench_sdxl.py [--batch 2] [--steps 5] [--no-locon]
+  python tools/bench_sdxl.py [--batch 2] [--steps 5] [--no-locon] [--full-ft --optimizer adafactor]
 """
 import argparse
 import json
@@ -23,6 +25,8 @@ ap.add_argument("--steps", type=int, default=5)
 ap.add_argument("--latent", type=int, default=128)
 ap.add_argument("--rank", type=int, default=16)
 ap.add_argument("--no-locon", action="store_true")
+ap.add_argument("--full-ft", action="store_true")
+ap.add_argument("--optimizer", choices=("adamw", "adafactor"), default="adamw")
 args = ap.parse_args()
 
 torch.manual_seed(0)
@@ -44,12 +48,20 @@ with torch.no_grad():
         else:
             p.zero_()
 unet.requires_grad_(False).eval()
-layers = [r"re:.*\.attn.?$", r"re:.*\.ff$"]
-if not args.no_locon:
-    layers += [r"re:.*\.resnets\.\d+\.conv[12]$", r"re:.*\.conv_shortcut$", r"re:.*samplers\.0\.conv$"]
-groups, lora = make_hcpdiff(unet, None, [{"rank": args.rank, "dropout": 0.0, "layers": layers}])
+if args.full_ft:
+    groups, lora = make_hcpdiff(unet, [{"lr": 1e-6, "layers": [""]}], None)
+    workload = f"SDXL-base UNet full fine-tune, {args.optimizer}"
+else:
+    layers = [r"re:.*\.attn.?$", r"re:.*\.ff$"]
+    if not args.no_locon:
+        layers += [r"re:.*\.resnets\.\d+\.conv[12]$", r"re:.*\.conv_shortcut$", r"re:.*samplers\.0\.conv$"]
+    groups, lora = make_hcpdiff(unet, None, [{"rank": args.rank, "dropout": 0.0, "layers": layers}])
+    workload = f"SDXL-base UNet LoRA r={args.rank} attn+ff" + ("" if args.no_locon else "+conv (locon)")
 params = [p for g in groups for p in g["params"]]
-step = LoraTrainStep(unet, params)
+if args.optimizer == "adafactor":
+    step = LoraTrainStep(unet, groups, optimizer="adafactor", optimizer_kwargs={"relative_step": False, "weight_decay": 1e-3})
+else:
+    step = LoraTrainStep(unet, groups if args.full_ft else params)
 B, S = args.batch, args.latent
 lat, noise = torch.randn(B, 4, S, S), torch.randn(B, 4, S, S)
 t, ehs = torch.randint(0, 1000, (B,)), torch.randn(B, 77, 2048)
@@ -66,8 +78,18 @@ for _ in range(args.steps):
 e1.record()
 torch.cuda.synchronize()
 ms = e0.elapsed_time(e1) / args.steps
-print(json.dumps({"workload": f"SDXL-base UNet LoRA r={args.rank} attn+ff" + ("" if args.no_locon else "+conv (locon)") +
-                              f", bs={B}, {S * 8}x{S * 8}", "ms_per_step": ms, "images_per_s": B / ms * 1e3,
-                  "lora_params": sum(p.numel() for p in params), "launches_per_step": step.launches_per_step,
+# the optimizer graph alone (clip + optimizer + EMA + zero_grad).  It ends by zeroing the gradient buffer, so these replays run on
+# zero gradients (the same memory traffic as a real step) and move the parameters and optimizer state after the timed steps.
+opt_reps = 5
+e0.record()
+for _ in range(opt_reps):
+    step._graph_opt.replay()
+e1.record()
+torch.cuda.synchronize()
+opt_ms = e0.elapsed_time(e1) / opt_reps
+props = torch.cuda.get_device_properties(0)
+print(json.dumps({"workload": workload + f", bs={B}, {S * 8}x{S * 8}", "ms_per_step": ms, "images_per_s": B / ms * 1e3,
+                  "optimizer_ms": opt_ms, ("trained_params" if args.full_ft else "lora_params"): sum(p.numel() for p in params),
+                  "optimizer_state_bytes": step.optimizer_state_bytes, "launches_per_step": step.launches_per_step,
                   "loss": float(step.loss.cpu()), "build_s": round(build_s, 1),
-                  "max_mem_gb": round(torch.cuda.max_memory_allocated() / 2 ** 30, 1)}))
+                  "max_mem_gb": round(torch.cuda.max_memory_allocated() / 2 ** 30, 1), "gpu": props.name}))
