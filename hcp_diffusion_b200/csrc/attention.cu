@@ -21,6 +21,10 @@
 //   dQ_i += dS K over all 128 kv rows of the CTA (dS^T of both warpgroups staged in shared memory as one MN-major operand; the
 //   warpgroups take turns per query tile), reduced into an fp32 buffer with vector red.global: one contribution per CTA, so a
 //   short kv range (<= 2 tiles) sums dQ in an order-independent way.
+// Causal variants (kCausal, Lq == Lkv: query row i sees kv columns <= i; CLIP's text encoder): the forward stops at the last kv
+// tile that meets its 128 query rows and masks by global row / column index; the backward starts its query loop at the first
+// 64-row tile that reaches its kv rows, and a CTA of a split query range with no tile left exits without writing.  The
+// non-causal instantiations compile to the same code as without the parameter.
 #include <stdlib.h>
 #include "common.cuh"
 #include "host_util.h"
@@ -68,7 +72,7 @@ struct AttnFwdCfg {
     static constexpr int SMEM_BYTES = Q_BYTES + 2 * STAGES * KV_BYTES + 256 + 1024;
 };
 
-template <int NB, int KVT>
+template <int NB, int KVT, bool kCausal>
 __global__ void __launch_bounds__(kAttnThreads, 1) attn_fwd_kernel(const __grid_constant__ AttnFwdParams p) {
     using Cfg = AttnFwdCfg<NB, KVT>;
     constexpr int STAGES = Cfg::STAGES;
@@ -85,7 +89,8 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attn_fwd_kernel(const __grid_
 
     const int warp = warp_id_uniform(), lane = threadIdx.x & 31;
     const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
-    const int nkv = (p.Lkv + KVT - 1) / KVT;
+    // causal: kv tiles past the CTA's last query row are masked entirely and never loaded
+    const int nkv = kCausal ? min((p.Lkv + KVT - 1) / KVT, (qt * 128 + 128 + KVT - 1) / KVT) : (p.Lkv + KVT - 1) / KVT;
 
     if (threadIdx.x == 0) {
         mbar_init(q_full, 1);
@@ -142,6 +147,7 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attn_fwd_kernel(const __grid_
         wgmma_fence_acc(s);
         // ---- online softmax (log2 domain)
         float mx[2] = {-INFINITY, -INFINITY};
+        const bool diag = kCausal && kv0 + KVT > qt * 128;       // the tile reaches above the CTA's first query row
 #pragma unroll
         for (int c8 = 0; c8 < KVT / 8; ++c8) {
 #pragma unroll
@@ -152,6 +158,7 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attn_fwd_kernel(const __grid_
                 for (int hh = 0; hh < 2; ++hh) {
                     float v = s[4 * c8 + 2 * hh + e] * sl2 + bv;
                     v = (col < ncols) ? v : -INFINITY;
+                    if (diag && kv0 + col > qt * 128 + row0 + 8 * hh) v = -INFINITY;   // column 0 is always kept: m is finite
                     s[4 * c8 + 2 * hh + e] = v;
                     mx[hh] = fmaxf(mx[hh], v);
                 }
@@ -238,7 +245,7 @@ struct AttnBwdCfg {
     static constexpr int SMEM_BYTES = 2 * KV_BYTES + 2 * STAGES * Q_BYTES + 2 * DS_BYTES + 256 + 1024;
 };
 
-template <int NB>
+template <int NB, bool kCausal>
 __global__ void __launch_bounds__(kAttnThreads, 1) attn_bwd_kernel(const __grid_constant__ AttnBwdParams p) {
     using Cfg = AttnBwdCfg<NB>;
     constexpr int STAGES = Cfg::STAGES;
@@ -262,7 +269,10 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attn_bwd_kernel(const __grid_
     const int h = blockIdx.y, b = blockIdx.z;
     const int nq = (p.Lq + 63) / 64;
     const int per = 2 * (((nq + 1) / 2 + p.qsplit - 1) / p.qsplit);     // whole 128-row units per split (plan_qsplit)
-    const int i0 = qs * per, i1 = min(nq, i0 + per);
+    // causal: query tiles before 2 * kt end above the CTA's first kv row (P = 0 there).  A split with no tile left contributes
+    // nothing: it exits before touching memory, so the fp32 dQ / dK / dV sums get no extra (zero) terms.
+    const int i0 = kCausal ? max(qs * per, 2 * kt) : qs * per, i1 = min(nq, qs * per + per);
+    if (kCausal && i0 >= i1) return;
 
     if (threadIdx.x == 0) {
         mbar_init(kv_full, 1);
@@ -338,6 +348,7 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attn_bwd_kernel(const __grid_
         wgmma_fence_acc(dp);
         // ---- P^T, dS^T = scale * P^T (dP^T - delta) as bf16 A fragments (K = q); dS^T also to shared memory for dQ
         uint32_t pa[4][4], da[4][4];
+        const bool diag = kCausal && i < 2 * kt + 2;             // the query tile starts inside the CTA's kv rows
 #pragma unroll
         for (int kk = 0; kk < 4; ++kk) {
             // per-column (query) statistics of the four columns of this k-step this thread holds
@@ -357,7 +368,8 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attn_bwd_kernel(const __grid_
                 float pv[2], dsv[2];
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
-                    const float pe = kv_ok[hh] ? fast_exp2(s[idx + e] * sl2 + kvb[hh] - lq[c + e]) : 0.f;
+                    float pe = kv_ok[hh] ? fast_exp2(s[idx + e] * sl2 + kvb[hh] - lq[c + e]) : 0.f;
+                    if (diag && kvw + r0 + 8 * hh > i * 64 + 16 * kk + 8 * (r >> 1) + cq + e) pe = 0.f;
                     pv[e] = pe;
                     dsv[e] = scale * pe * (dp[idx + e] - dq_[c + e]);
                 }
@@ -530,31 +542,31 @@ static int check_common(int64_t B, int64_t H, int64_t Lq, int64_t Lkv, int64_t d
     return HCP_OK;
 }
 
-template <int NB, int KVT>
+template <int NB, int KVT, bool kCausal>
 static int launch_attn_fwd(const AttnFwdParams& p, dim3 grid, cudaStream_t stream) {
     using Cfg = AttnFwdCfg<NB, KVT>;
     static bool configured = false;
     if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(attn_fwd_kernel<NB, KVT>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
+        cudaError_t e = cudaFuncSetAttribute(attn_fwd_kernel<NB, KVT, kCausal>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
         if (e != cudaSuccess) return set_cuda_error(e, "cudaFuncSetAttribute(attn_fwd)");
         configured = true;
     }
-    launch_k(attn_fwd_kernel<NB, KVT>, grid, dim3(kAttnThreads), Cfg::SMEM_BYTES, stream, p);
+    launch_k(attn_fwd_kernel<NB, KVT, kCausal>, grid, dim3(kAttnThreads), Cfg::SMEM_BYTES, stream, p);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return set_cuda_error(e, "attn_fwd launch");
     return HCP_OK;
 }
 
-template <int NB>
+template <int NB, bool kCausal>
 static int launch_attn_bwd(const AttnBwdParams& p, dim3 grid, cudaStream_t stream) {
     using Cfg = AttnBwdCfg<NB>;
     static bool configured = false;
     if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(attn_bwd_kernel<NB>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
+        cudaError_t e = cudaFuncSetAttribute(attn_bwd_kernel<NB, kCausal>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
         if (e != cudaSuccess) return set_cuda_error(e, "cudaFuncSetAttribute(attn_bwd)");
         configured = true;
     }
-    launch_k(attn_bwd_kernel<NB>, grid, dim3(kAttnThreads), Cfg::SMEM_BYTES, stream, p);
+    launch_k(attn_bwd_kernel<NB, kCausal>, grid, dim3(kAttnThreads), Cfg::SMEM_BYTES, stream, p);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return set_cuda_error(e, "attn_bwd launch");
     return HCP_OK;
@@ -564,10 +576,12 @@ static int launch_attn_bwd(const AttnBwdParams& p, dim3 grid, cudaStream_t strea
 
 using namespace hcp;
 
-extern "C" int hcp_attn_fwd_bf16(const hcp_attn_args* a, hcp_stream_t stream_) {
+template <bool kCausal>
+static int attn_fwd(const hcp_attn_args* a, hcp_stream_t stream_) {
     if (!a || !a->q || !a->k || !a->v || !a->o) return set_error(HCP_ERR_INVALID, "attn_fwd: null pointer");
     int rc = check_common(a->B, a->H, a->Lq, a->Lkv, a->d);
     if (rc) return rc;
+    if (kCausal && a->Lq != a->Lkv) return set_error(HCP_ERR_INVALID, "attn_fwd_causal: Lq must equal Lkv");
     const int nb = (int)((a->d + 63) / 64);
     // kv tile: 128 rows, 64 when the O accumulator of d > 128 leaves no registers for a 128-column S tile
     const uint32_t kvt = nb == 3 ? 64 : 128;
@@ -584,10 +598,13 @@ extern "C" int hcp_attn_fwd_bf16(const hcp_attn_args* a, hcp_stream_t stream_) {
     p.lse = a->lse;
     const dim3 grid((unsigned)((a->Lq + 127) / 128), (unsigned)a->H, (unsigned)a->B);
     cudaStream_t stream = (cudaStream_t)stream_;
-    if (nb == 1) return launch_attn_fwd<1, 128>(p, grid, stream);
-    if (nb == 2) return launch_attn_fwd<2, 128>(p, grid, stream);
-    return launch_attn_fwd<3, 64>(p, grid, stream);
+    if (nb == 1) return launch_attn_fwd<1, 128, kCausal>(p, grid, stream);
+    if (nb == 2) return launch_attn_fwd<2, 128, kCausal>(p, grid, stream);
+    return launch_attn_fwd<3, 64, kCausal>(p, grid, stream);
 }
+
+extern "C" int hcp_attn_fwd_bf16(const hcp_attn_args* a, hcp_stream_t stream) { return attn_fwd<false>(a, stream); }
+extern "C" int hcp_attn_fwd_causal_bf16(const hcp_attn_args* a, hcp_stream_t stream) { return attn_fwd<true>(a, stream); }
 
 // CTAs per kv tile along the query dimension: when the (kv tile, head, image) CTAs fill less than one wave, the query range is split
 // so that about two CTAs per SM run; the partial dK / dV sums then go through an fp32 buffer
@@ -610,11 +627,13 @@ extern "C" size_t hcp_attn_bwd_workspace_bytes(int64_t B, int64_t H, int64_t Lq,
     return n * sizeof(float);
 }
 
-extern "C" int hcp_attn_bwd_bf16(const hcp_attn_bwd_args* a, hcp_stream_t stream_) {
+template <bool kCausal>
+static int attn_bwd(const hcp_attn_bwd_args* a, hcp_stream_t stream_) {
     if (!a || !a->q || !a->k || !a->v || !a->o || !a->dout || !a->lse || !a->dq || !a->dk || !a->dv || !a->workspace)
         return set_error(HCP_ERR_INVALID, "attn_bwd: null pointer");
     int rc = check_common(a->B, a->H, a->Lq, a->Lkv, a->d);
     if (rc) return rc;
+    if (kCausal && a->Lq != a->Lkv) return set_error(HCP_ERR_INVALID, "attn_bwd_causal: Lq must equal Lkv");
     if (a->workspace_bytes < hcp_attn_bwd_workspace_bytes(a->B, a->H, a->Lq, a->Lkv, a->d))
         return set_error(HCP_ERR_INVALID, "attn_bwd: workspace too small");
     if ((a->ldo % 8) != 0 || (a->lddo % 8) != 0 || (a->lddq % 8) != 0) return set_error(HCP_ERR_INVALID, "attn_bwd: leading dimensions must be multiples of 8");
@@ -657,7 +676,8 @@ extern "C" int hcp_attn_bwd_bf16(const hcp_attn_bwd_args* a, hcp_stream_t stream
     // output column slices of 64 (one box): dK / dV / dQ accumulators of a slice stay in registers; S and dP are recomputed per slice
     for (int col0 = 0; col0 < a->d; col0 += 64) {
         p.col0 = col0;
-        rc = nb == 1 ? launch_attn_bwd<1>(p, grid, stream) : nb == 2 ? launch_attn_bwd<2>(p, grid, stream) : launch_attn_bwd<3>(p, grid, stream);
+        rc = nb == 1 ? launch_attn_bwd<1, kCausal>(p, grid, stream) : nb == 2 ? launch_attn_bwd<2, kCausal>(p, grid, stream)
+                     : launch_attn_bwd<3, kCausal>(p, grid, stream);
         if (rc) return rc;
     }
     {
@@ -674,3 +694,6 @@ extern "C" int hcp_attn_bwd_bf16(const hcp_attn_bwd_args* a, hcp_stream_t stream
     if (e != cudaSuccess) return set_cuda_error(e, "attn_bwd post launch");
     return HCP_OK;
 }
+
+extern "C" int hcp_attn_bwd_bf16(const hcp_attn_bwd_args* a, hcp_stream_t stream) { return attn_bwd<false>(a, stream); }
+extern "C" int hcp_attn_bwd_causal_bf16(const hcp_attn_bwd_args* a, hcp_stream_t stream) { return attn_bwd<true>(a, stream); }

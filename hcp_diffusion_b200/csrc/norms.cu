@@ -929,6 +929,102 @@ __global__ void geglu_bwd_kernel(const __nv_bfloat16* __restrict__ u, const __nv
 }
 
 // =============================================================================================
+// quick-GELU (CLIP MLP): y = x * sigmoid(1.702 x);  dx = dy * (s + 1.702 x s (1 - s))
+// =============================================================================================
+__device__ __forceinline__ float qgelu_sig(float x) { return 1.f / (1.f + __expf(-1.702f * x)); }
+
+__global__ void quick_gelu_fwd_kernel(const __nv_bfloat16* __restrict__ x, int64_t n8, __nv_bfloat16* __restrict__ y) {
+    pdl_trigger();
+    pdl_wait();
+    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;   // one thread per 8 elements
+    if (i >= n8) return;
+    const uint4 ux = reinterpret_cast<const uint4*>(x)[i];
+    const uint32_t xx[4] = {ux.x, ux.y, ux.z, ux.w};
+    uint32_t o[4];
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+        const float2 v = unpack_bf16x2(xx[e]);
+        o[e] = pack_bf16x2(v.x * qgelu_sig(v.x), v.y * qgelu_sig(v.y));
+    }
+    reinterpret_cast<uint4*>(y)[i] = make_uint4(o[0], o[1], o[2], o[3]);
+}
+__global__ void quick_gelu_bwd_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ dy, int64_t n8,
+                                      __nv_bfloat16* __restrict__ dx) {
+    pdl_trigger();
+    pdl_wait();
+    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (i >= n8) return;
+    const uint4 ux = reinterpret_cast<const uint4*>(x)[i], ud = reinterpret_cast<const uint4*>(dy)[i];
+    const uint32_t xx[4] = {ux.x, ux.y, ux.z, ux.w}, dd[4] = {ud.x, ud.y, ud.z, ud.w};
+    uint32_t o[4];
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+        const float2 v = unpack_bf16x2(xx[e]), d = unpack_bf16x2(dd[e]);
+        const float s0 = qgelu_sig(v.x), s1 = qgelu_sig(v.y);
+        o[e] = pack_bf16x2(d.x * (s0 + 1.702f * v.x * s0 * (1.f - s0)), d.y * (s1 + 1.702f * v.y * s1 * (1.f - s1)));
+    }
+    reinterpret_cast<uint4*>(dx)[i] = make_uint4(o[0], o[1], o[2], o[3]);
+}
+
+// =============================================================================================
+// fp32 sum of up to kSumSrcs bf16 arrays, in source order: the fan-in of the text embedding's gradient over the cross-attentions
+// =============================================================================================
+constexpr int kSumSrcs = 32;
+struct SumSrcs { const __nv_bfloat16* p[kSumSrcs]; };
+
+__global__ void sum_bf16_f32_kernel(const __grid_constant__ SumSrcs s, int nsrc, int64_t n8, int accumulate, float* __restrict__ out) {
+    pdl_trigger();
+    pdl_wait();
+    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;   // one thread per 8 elements
+    if (i >= n8) return;
+    float acc[8];
+    float4* o = reinterpret_cast<float4*>(out) + 2 * i;
+    if (accumulate) {
+        const float4 a = o[0], b = o[1];
+        acc[0] = a.x; acc[1] = a.y; acc[2] = a.z; acc[3] = a.w; acc[4] = b.x; acc[5] = b.y; acc[6] = b.z; acc[7] = b.w;
+    } else {
+#pragma unroll
+        for (int e = 0; e < 8; ++e) acc[e] = 0.f;
+    }
+    for (int k = 0; k < nsrc; ++k) {
+        const uint4 u = reinterpret_cast<const uint4*>(s.p[k])[i];
+        const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const float2 f = unpack_bf16x2(w[e]);
+            acc[2 * e] += f.x;
+            acc[2 * e + 1] += f.y;
+        }
+    }
+    o[0] = make_float4(acc[0], acc[1], acc[2], acc[3]);
+    o[1] = make_float4(acc[4], acc[5], acc[6], acc[7]);
+}
+
+// =============================================================================================
+// token + position embedding gather (CLIPTextEmbeddings): out[r] = bf16(tok[clamp(ids[r])] + pos[clamp(pos_ids[l] or l)]),
+// r = b * L + l.  Ids outside the tables read the nearest valid row; they are never read out of bounds.
+// =============================================================================================
+__global__ void embed_gather_kernel(const int64_t* __restrict__ ids, const int64_t* __restrict__ pos_ids, const float* __restrict__ tok,
+                                    int64_t V, const float* __restrict__ pos, int64_t P, int64_t rows, int L, int C,
+                                    __nv_bfloat16* __restrict__ out) {
+    pdl_trigger();
+    pdl_wait();
+    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;   // one thread per 8 outputs
+    const int nv = C / 8;
+    if (i >= rows * nv) return;
+    const int64_t r = i / nv;
+    const int c = (int)(i % nv) * 8;
+    const int l = (int)(r % L);
+    const int64_t t = min(max(ids[r], (int64_t)0), V - 1);
+    const int64_t pr = min(max(pos_ids ? pos_ids[l] : (int64_t)l, (int64_t)0), P - 1);
+    const float4* a = reinterpret_cast<const float4*>(tok + t * C + c);
+    const float4* b = reinterpret_cast<const float4*>(pos + pr * C + c);
+    const float4 a0 = a[0], a1 = a[1], b0 = b[0], b1 = b[1];
+    *reinterpret_cast<uint4*>(out + r * C + c) = make_uint4(pack_bf16x2(a0.x + b0.x, a0.y + b0.y), pack_bf16x2(a0.z + b0.z, a0.w + b0.w),
+                                                            pack_bf16x2(a1.x + b1.x, a1.y + b1.y), pack_bf16x2(a1.z + b1.z, a1.w + b1.w));
+}
+
+// =============================================================================================
 // nearest 2x upsample (NHWC) and its backward (sum of the 2x2 block)
 // =============================================================================================
 __global__ void upsample2x_fwd_kernel(const __nv_bfloat16* __restrict__ x, int B, int H, int W, int C, __nv_bfloat16* __restrict__ y) {
@@ -1107,6 +1203,52 @@ extern "C" int hcp_geglu_bwd_bf16(const void* u, const void* dh, int64_t M, int6
     launch_k(geglu_bwd_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, (cudaStream_t)stream_, (const __nv_bfloat16*)u, (const __nv_bfloat16*)dh, M,
                                                                                    (int)F, (__nv_bfloat16*)du);
     LAUNCH_CHECK("geglu_bwd launch");
+    return HCP_OK;
+}
+extern "C" int hcp_quick_gelu_fwd_bf16(const void* x, int64_t M, int64_t F, void* y, hcp_stream_t stream_) {
+    if (!x || !y || M < 0 || F % 8 != 0) return set_error(HCP_ERR_INVALID, "quick_gelu_fwd");
+    const int64_t n8 = M * (F / 8);
+    if (n8 == 0) return HCP_OK;
+    launch_k(quick_gelu_fwd_kernel, dim3((unsigned)((n8 + 255) / 256)), dim3(256), 0, (cudaStream_t)stream_, (const __nv_bfloat16*)x, n8,
+             (__nv_bfloat16*)y);
+    LAUNCH_CHECK("quick_gelu_fwd launch");
+    return HCP_OK;
+}
+extern "C" int hcp_quick_gelu_bwd_bf16(const void* x, const void* dy, int64_t M, int64_t F, void* dx, hcp_stream_t stream_) {
+    if (!x || !dy || !dx || M < 0 || F % 8 != 0) return set_error(HCP_ERR_INVALID, "quick_gelu_bwd");
+    const int64_t n8 = M * (F / 8);
+    if (n8 == 0) return HCP_OK;
+    launch_k(quick_gelu_bwd_kernel, dim3((unsigned)((n8 + 255) / 256)), dim3(256), 0, (cudaStream_t)stream_, (const __nv_bfloat16*)x,
+             (const __nv_bfloat16*)dy, n8, (__nv_bfloat16*)dx);
+    LAUNCH_CHECK("quick_gelu_bwd launch");
+    return HCP_OK;
+}
+extern "C" int hcp_sum_bf16_to_f32(const void* const* srcs, int64_t nsrc, int64_t n, float* out, hcp_stream_t stream_) {
+    if (!srcs || !out || nsrc <= 0 || n % 8 != 0) return set_error(HCP_ERR_INVALID, "sum_bf16_to_f32: need sources and n % 8 == 0");
+    for (int64_t k = 0; k < nsrc; ++k)
+        if (!srcs[k]) return set_error(HCP_ERR_INVALID, "sum_bf16_to_f32: null source");
+    const int64_t n8 = n / 8;
+    if (n8 == 0) return HCP_OK;
+    for (int64_t k0 = 0; k0 < nsrc; k0 += kSumSrcs) {
+        SumSrcs s;
+        memset(&s, 0, sizeof(s));
+        const int cnt = (int)(nsrc - k0 < kSumSrcs ? nsrc - k0 : kSumSrcs);
+        for (int k = 0; k < cnt; ++k) s.p[k] = (const __nv_bfloat16*)srcs[k0 + k];
+        launch_k(sum_bf16_f32_kernel, dim3((unsigned)((n8 + 255) / 256)), dim3(256), 0, (cudaStream_t)stream_, s, cnt, n8, (int)(k0 > 0), out);
+        LAUNCH_CHECK("sum_bf16_to_f32 launch");
+    }
+    return HCP_OK;
+}
+extern "C" int hcp_embed_gather_bf16(const int64_t* ids, const int64_t* pos_ids, const float* tok_emb, int64_t V, const float* pos_emb,
+                                     int64_t P, int64_t B, int64_t L, int64_t C, void* out, hcp_stream_t stream_) {
+    if (!ids || !tok_emb || !pos_emb || !out) return set_error(HCP_ERR_INVALID, "embed_gather: null pointer");
+    if (V <= 0 || P <= 0 || B <= 0 || L <= 0 || C <= 0 || C % 8 != 0)
+        return set_error(HCP_ERR_INVALID, "embed_gather: empty table or C not a multiple of 8");
+    if (!pos_ids && L > P) return set_error(HCP_ERR_INVALID, "embed_gather: sequence longer than the position table");
+    const int64_t n = B * L * (C / 8);
+    launch_k(embed_gather_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, (cudaStream_t)stream_, ids, pos_ids, tok_emb, V, pos_emb, P,
+             B * L, (int)L, (int)C, (__nv_bfloat16*)out);
+    LAUNCH_CHECK("embed_gather launch");
     return HCP_OK;
 }
 extern "C" int hcp_upsample2x_fwd_bf16(const void* x, int64_t B, int64_t H, int64_t W, int64_t C, void* y, hcp_stream_t stream_) {

@@ -26,6 +26,7 @@ from torch import nn
 
 from . import _lib, adafactor, ops
 from ._lib import call, stream_ptr
+from .models.clip import encode_prompt
 
 SNR_LOSS_MODES = {"min_snr": 0, "soft_min_snr": 1, "kdiff_min_snr": 2, "edm": 3,
                   "MinSNRLoss": 0, "SoftMinSNRLoss": 1, "KDiffMinSNRLoss": 2, "EDMLoss": 3}
@@ -175,14 +176,33 @@ class LoraTrainStep:
     (transformers.optimization.Adafactor; `optimizer_kwargs` takes its constructor keys with its defaults -- `lr`, `eps`,
     `clip_threshold`, `decay_rate`, `beta1`, `weight_decay`, `scale_parameter`, `relative_step`, `warmup_init` -- and a group's own
     'lr' / 'weight_decay' win over them).  Adafactor keeps factored second moments per tensor of the module's shape (state sized by
-    adafactor.state_numel), plus one flat first-moment buffer only when `beta1` is set."""
+    adafactor.state_numel), plus one flat first-moment buffer only when `beta1` is set.
+
+    `text_encoder`: a `models.CLIPTextModel` whose LoRA adapters train together with the UNet's (the reference's `lora_text_encoder`,
+    `TEUnetWrapper`); its adapter parameters must be among `params` (their own groups), so they share the flat buffer: one all-reduce,
+    one global-norm clip over both models, the same optimizer and EMA.  `step()` then takes int64 token ids [B, 77 R] in place of the
+    text embedding, and the text encoder runs forward and backward inside the same graph.  `text_encoder_opts`: {'n_repeats',
+    'clip_skip', 'clip_final_norm'} of `models.encode_prompt`."""
 
     def __init__(self, unet: nn.Module, params: Union[Iterable[nn.Parameter], Sequence[dict]], lr: float = 1e-4, betas=(0.9, 0.999),
                  eps: float = 1e-8, weight_decay: float = 1e-2, max_grad_norm: float = 1.0, use_cuda_graph: bool = True,
                  process_group: Optional[dist.ProcessGroup] = None, side_stream: bool = True, grad_accum_steps: int = 1,
                  loss: Union[None, str, dict] = None, ema: Optional[dict] = None, cfg_scale=None, num_train_timesteps: int = 1000,
-                 optimizer: str = "adamw", optimizer_kwargs: Optional[dict] = None):
+                 optimizer: str = "adamw", optimizer_kwargs: Optional[dict] = None, text_encoder: Optional[nn.Module] = None,
+                 text_encoder_opts: Optional[dict] = None):
         self.unet = unet
+        self.te, self.te_opts = text_encoder, None
+        if text_encoder is not None:
+            if cfg_scale is not None:
+                raise NotImplementedError("cfg_scale (DreamArtist batch doubling) together with a trained text encoder is not supported")
+            if getattr(getattr(unet, "config", None), "addition_embed_type", None) == "text_time":
+                raise NotImplementedError("an SDXL (text_time) UNet together with a trained text encoder is not supported")
+            opts = dict(text_encoder_opts or {})
+            unknown = set(opts) - {"n_repeats", "clip_skip", "clip_final_norm"}
+            if unknown:
+                raise ValueError(f"text_encoder_opts: unknown keys {sorted(unknown)}")
+            self.te_opts = {"n_repeats": int(opts.get("n_repeats", 1)), "clip_skip": int(opts.get("clip_skip", 0)),
+                            "clip_final_norm": bool(opts.get("clip_final_norm", True))}
         if optimizer not in ("adamw", "adafactor"):
             raise ValueError(f"optimizer {optimizer!r}: one of 'adamw', 'adafactor'")
         self.optimizer = optimizer
@@ -205,6 +225,11 @@ class LoraTrainStep:
             g["params"] = [p for p in dict.fromkeys(g["params"]) if id(p) not in seen]
             seen.update(id(p) for p in g["params"])
             flat_list += g["params"]
+        if text_encoder is not None:
+            missing = [n for n, p in text_encoder.named_parameters() if p.requires_grad and id(p) not in seen]
+            if missing:
+                raise ValueError(f"text-encoder parameters {missing[:3]}... are trainable but not in `params`: pass the "
+                                 "lora_text_encoder groups too (they share the flat buffer, the clip and the optimizer)")
         self.flat = FlatParams(flat_list)
         dev = self.flat.data.device
         self.m = self.v = None
@@ -351,6 +376,8 @@ class LoraTrainStep:
         x_in, t_in = x_t, t
         if self.cfg_ctx is not None:                       # DreamArtistPTContext.pre: 'b c h w -> (pn b) c h w', timesteps.repeat(2)
             x_in, t_in = torch.cat([x_t, x_t], 0), torch.cat([t, t], 0)
+        if self.te is not None:                            # TEUnetWrapper.forward: ehs = TE(ids) with its adapters in the graph
+            ehs = encode_prompt(self.te, ehs, **self.te_opts)
         pred = (self.unet(x_in, t_in, ehs, added_cond_kwargs=added) if added is not None else self.unet(x_in, t_in, ehs)).sample
         if self.cfg_ctx is not None:
             pred = _CfgMixFn.apply(pred, t, *self.cfg_ctx)
@@ -403,7 +430,7 @@ class LoraTrainStep:
     def step(self, latents: torch.Tensor, noise: torch.Tensor, t: torch.Tensor, ehs: torch.Tensor,
              added_cond_kwargs: Optional[Dict[str, torch.Tensor]] = None) -> torch.Tensor:
         """One micro-step: latents/noise fp32 [B,4,H,W], t int64 [B], ehs fp32 [B,L,ctx] ([2B,L,ctx] = [negative | positive] with
-        `cfg_scale`) (host-pinned or device); `added_cond_kwargs` ({'text_embeds' [B,P], 'time_ids' [B,6]}) for SDXL UNets
+        `cfg_scale`), or int64 token ids [B, 77 R] with a `text_encoder` (host-pinned or device); `added_cond_kwargs` ({'text_embeds' [B,P], 'time_ids' [B,6]}) for SDXL UNets
         (reference wrapper.py:66).  The optimizer runs on every `grad_accum_steps`-th call.  Returns the device loss tensor
         (shape [1]) of this micro-batch; reading it is the caller's D2H."""
         dev = self.flat.data.device
@@ -458,7 +485,8 @@ class LoraTrainStep:
         dev = self.flat.data.device
         self._static = {
             "latents": latents.to(dev).float().contiguous().clone(), "noise": noise.to(dev).float().contiguous().clone(),
-            "t": t.to(dev).long().contiguous().clone(), "ehs": ehs.to(dev).float().contiguous().clone(),
+            "t": t.to(dev).long().contiguous().clone(),
+            "ehs": (ehs.to(dev).long() if self.te is not None else ehs.to(dev).float()).contiguous().clone(),
             "added": None if added is None else {k: v.to(dev).float().contiguous().clone() for k, v in added.items()},
         }
         s = self._static

@@ -123,7 +123,8 @@ class Attention(nn.Module):
         return [g.kv, g.q, g.out] if self.is_cross else [g.qkv, g.out]
 
     def run(self, x: torch.Tensor, residual: torch.Tensor, context, kv_bias: Optional[torch.Tensor]) -> torch.Tensor:
-        """`context`: the text embedding [B, Lc, ctx] or a `_HoistedKV` holding the k/v projections computed ahead of time."""
+        """`context`: the text embedding [B, Lc, ctx], a `_PerAttnContext` (one alias per cross-attention, when the embedding carries
+        a gradient) or a `_HoistedKV` holding the k/v projections computed ahead of time."""
         g = self._groups()
         C_ = self.inner_dim
         if not self.is_cross:
@@ -131,9 +132,23 @@ class Attention(nn.Module):
             o = ops.attention(self.heads, C_, (0, C_, 2 * C_), qkv, None, None)
         else:
             q = g.q([x])
-            kv = context.take(self) if isinstance(context, _HoistedKV) else g.kv([context])   # [B, Lc, 2C]
+            if isinstance(context, _HoistedKV):
+                kv = context.take(self)
+            else:
+                kv = g.kv([context.take(self) if isinstance(context, _PerAttnContext) else context])   # [B, Lc, 2C]
             o = ops.attention(self.heads, C_, (0, 0, C_), q, kv, kv_bias)
         return g.out([o], residual=residual)
+
+
+class _PerAttnContext:
+    """The text embedding as one alias per cross-attention (ops.context_fanout): the k/v dgrads of the attentions come back as
+    separate gradients and are summed in fp32 (the reference's per-use autocast casts of the fp32 embedding)."""
+
+    def __init__(self, ehs: torch.Tensor, attns: Sequence["Attention"]):
+        self.ctx = dict(zip((id(a) for a in attns), ops.context_fanout(ehs, len(attns))))
+
+    def take(self, attn: "Attention") -> torch.Tensor:
+        return self.ctx.pop(id(attn))
 
 
 class _HoistedKV:
@@ -141,15 +156,16 @@ class _HoistedKV:
     (they depend on nothing but the text embedding, and autograd runs their backward -- incl. the LoRA-gradient kernels -- on
     the same side stream).  `take` makes the main stream wait for them once, at the first consumer."""
 
-    def __init__(self, ctx: torch.Tensor, attns: Sequence["Attention"]):
+    def __init__(self, ctx, attns: Sequence["Attention"]):
+        """`ctx`: the bf16 text embedding, or a `_PerAttnContext` when it carries a gradient."""
         self.ctx = ctx
         main = torch.cuda.current_stream()
-        self.side = ops.fork_side(ctx)
+        self.side = ops.fork_side(*(ctx.ctx.values() if isinstance(ctx, _PerAttnContext) else (ctx,)))
         self.joined = False
         self.kv = {}
         with torch.cuda.stream(self.side):
             for a in attns:
-                t = a._groups().kv([ctx])
+                t = a._groups().kv([ctx.take(a) if isinstance(ctx, _PerAttnContext) else ctx])
                 t.record_stream(main)               # produced on the side stream, consumed (and later freed) on the main one
                 self.kv[id(a)] = t
 
@@ -634,13 +650,18 @@ class UNet2DConditionModel(nn.Module):
                 temb_list[i] = temb_list[i] + d * b.alpha
         tembs = iter(temb_list)
 
-        ctx = ops.cast_bf16(encoder_hidden_states)
+        attn2s = [m.attn2 for m in self.modules() if isinstance(m, BasicTransformerBlock)]
+        if encoder_hidden_states.requires_grad and torch.is_grad_enabled():
+            # d(ehs): every cross-attention's k/v dgrad (merged LoRA included) summed in fp32; without a gradient nothing changes
+            ctx = _PerAttnContext(encoder_hidden_states, attn2s)
+        else:
+            ctx = ops.cast_bf16(encoder_hidden_states)
         kv_bias = None
         if encoder_attention_mask is not None:
             kv_bias = ((1.0 - encoder_attention_mask.to(torch.float32)) * -10000.0).contiguous()
 
         if ops.side_enabled():
-            ctx = _HoistedKV(ctx, [m.attn2 for m in self.modules() if isinstance(m, BasicTransformerBlock)])
+            ctx = _HoistedKV(ctx, attn2s)
 
         h = ops.conv_in(sample, rt.w_in, rt.b_in,                        # bf16 [B, H*W, C0]
                         train=(self.conv_in.weight, self.conv_in.bias) if rt.train_in else None)

@@ -983,10 +983,10 @@ def layer_norm(gamma, beta, eps, x):
 class AttentionFn(torch.autograd.Function):
     """softmax(q k^T * scale + bias) v over heads laid out as column blocks.
     q_src [B,Lq,ldq] holds q at column q_off; kv_src [B,Lkv,ldkv] holds k at k_off and v at v_off (q_src may be kv_src:
-    the fused QKV projection output)."""
+    the fused QKV projection output).  `causal` (Lq == Lkv): query row i attends to kv columns <= i (CLIP's text encoder)."""
 
     @staticmethod
-    def forward(ctx, heads: int, C_: int, offs: Tuple[int, int, int], kv_bias: Optional[torch.Tensor], q_src: torch.Tensor,
+    def forward(ctx, heads: int, C_: int, offs: Tuple[int, int, int], causal: bool, kv_bias: Optional[torch.Tensor], q_src: torch.Tensor,
                 kv_src: Optional[torch.Tensor]):
         q_src = _chk(q_src, "attention q")
         same = kv_src is None
@@ -1005,15 +1005,15 @@ class AttentionFn(torch.autograd.Function):
         a.scale = scale
         a.kv_bias = ptr(kv_bias)
         a.o, a.ldo, a.lse = o.data_ptr(), C_, lse.data_ptr()
-        call("hcp_attn_fwd_bf16", C.byref(a), stream_ptr())
+        call("hcp_attn_fwd_causal_bf16" if causal else "hcp_attn_fwd_bf16", C.byref(a), stream_ptr())
         ctx.save_for_backward(q_src, kvt, o, lse, kv_bias)
-        ctx.cfg = (heads, C_, offs, same, scale)
+        ctx.cfg = (heads, C_, offs, same, scale, causal)
         return o
 
     @staticmethod
     def backward(ctx, do):
         q_src, kvt, o, lse, kv_bias = ctx.saved_tensors
-        heads, C_, offs, same, scale = ctx.cfg
+        heads, C_, offs, same, scale, causal = ctx.cfg
         do = _chk(do, "attention grad")
         B, Lq, ldq = q_src.shape
         _, Lkv, ldkv = kvt.shape
@@ -1034,12 +1034,12 @@ class AttentionFn(torch.autograd.Function):
         a.dk, a.lddk = dkv.data_ptr() + 2 * offs[1], ldkv
         a.dv, a.lddv = dkv.data_ptr() + 2 * offs[2], ldkv
         a.workspace, a.workspace_bytes = ws.data_ptr(), wsb
-        call("hcp_attn_bwd_bf16", C.byref(a), stream_ptr())
-        return None, None, None, None, dq_src, (None if same else dkv)
+        call("hcp_attn_bwd_causal_bf16" if causal else "hcp_attn_bwd_bf16", C.byref(a), stream_ptr())
+        return None, None, None, None, None, dq_src, (None if same else dkv)
 
 
-def attention(heads: int, C_: int, offs, q_src, kv_src=None, kv_bias=None):
-    return AttentionFn.apply(heads, C_, tuple(offs), kv_bias, q_src, kv_src)
+def attention(heads: int, C_: int, offs, q_src, kv_src=None, kv_bias=None, causal: bool = False):
+    return AttentionFn.apply(heads, C_, tuple(offs), bool(causal), kv_bias, q_src, kv_src)
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -1066,6 +1066,49 @@ class GegluFn(torch.autograd.Function):
         du = torch.empty_like(u)
         call("hcp_geglu_bwd_bf16", u.data_ptr(), dh.data_ptr(), M, F2 // 2, du.data_ptr(), stream_ptr())
         return du
+
+
+class QuickGeluFn(torch.autograd.Function):
+    """y = x * sigmoid(1.702 x) (CLIP MLP activation), bf16 [..., F]."""
+
+    @staticmethod
+    def forward(ctx, x):
+        x = _chk(x, "quick_gelu input")
+        F_ = x.shape[-1]
+        y = torch.empty_like(x)
+        call("hcp_quick_gelu_fwd_bf16", x.data_ptr(), x.numel() // F_, F_, y.data_ptr(), stream_ptr())
+        ctx.save_for_backward(x)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        (x,) = ctx.saved_tensors
+        dy = _chk(dy, "quick_gelu grad")
+        F_ = x.shape[-1]
+        dx = torch.empty_like(x)
+        call("hcp_quick_gelu_bwd_bf16", x.data_ptr(), dy.data_ptr(), x.numel() // F_, F_, dx.data_ptr(), stream_ptr())
+        return dx
+
+
+def embed_tokens(ids: torch.Tensor, tok_emb: torch.Tensor, pos_emb: torch.Tensor, pos_ids: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """bf16 [B, L, C] = tok_emb[ids] + pos_emb[pos_ids or arange(L)] (fp32 tables, int64 ids on the device; ids outside the tables
+    are clamped to the nearest row, see hcp_embed_gather_bf16).  No gradient: the embedding tables are frozen."""
+    if ids.dtype != torch.int64 or not ids.is_cuda or ids.dim() != 2:
+        raise _lib.HcpError(f"embed_tokens: expected CUDA int64 ids [B, L], got {ids.dtype} {tuple(ids.shape)} on {ids.device}")
+    if tok_emb.dtype != torch.float32 or pos_emb.dtype != torch.float32:
+        raise _lib.HcpError("embed_tokens: the embedding tables must be fp32")
+    ids = ids.contiguous()
+    tok, pos = tok_emb.detach().contiguous(), pos_emb.detach().contiguous()
+    B, L = ids.shape
+    C_ = tok.shape[1]
+    if pos_ids is not None:
+        pos_ids = pos_ids.to(ids.device, torch.int64).reshape(-1).contiguous()
+        if pos_ids.numel() != L:
+            raise _lib.HcpError(f"embed_tokens: position_ids must hold {L} entries (one row shared by the batch)")
+    out = torch.empty((B, L, C_), dtype=BF16, device=ids.device)
+    call("hcp_embed_gather_bf16", ids.data_ptr(), ptr(pos_ids), tok.data_ptr(), tok.shape[0], pos.data_ptr(), pos.shape[0], B, L, C_,
+         out.data_ptr(), stream_ptr())
+    return out
 
 
 class Upsample2xFn(torch.autograd.Function):
@@ -1259,6 +1302,37 @@ def skinny_linear(x: torch.Tensor, w_bf16: torch.Tensor, bias: Optional[torch.Te
 def sinusoid(x: torch.Tensor, dim: int, per_row: int, out: torch.Tensor, col0: int) -> None:
     """out[m // per_row, col0 + (m % per_row) * dim + j] = sinusoidal embedding (cos | sin) of x[m]; out fp32 2-D, x fp32 [M]."""
     call("hcp_sinusoid_f32", x.data_ptr(), x.numel(), dim, per_row, out.data_ptr() + 4 * col0, out.stride(0), stream_ptr())
+
+
+class ContextFanoutFn(torch.autograd.Function):
+    """The text embedding for `n` cross-attentions when it carries a gradient: n bf16 aliases of one cast (no copy: the k/v
+    projection GEMMs only read it), so that each consumer's input gradient arrives here separately and the n of them are summed in
+    fp32 by one kernel (hcp_sum_bf16_to_f32), in a fixed order -- autograd would add them pairwise in bf16.  The reference casts its fp32
+    embedding per use under autocast and accumulates the per-use gradients in fp32.  The gradient has the input's dtype: fp32 for an
+    fp32 embedding; for a bf16 one (the text encoder's output) the fp32 sum is rounded once."""
+
+    @staticmethod
+    def forward(ctx, n: int, x: torch.Tensor):
+        ctx.in_dtype = x.dtype
+        y = x.contiguous() if x.dtype == BF16 else cast_bf16(x)
+        ctx.set_materialize_grads(False)
+        return tuple(y.view_as(y) for _ in range(n))        # distinct outputs: one gradient slot per consumer
+
+    @staticmethod
+    def backward(ctx, *grads):
+        gs = [_chk(g, "context grad") for g in grads if g is not None]
+        if not gs:
+            return None, None
+        acc = torch.empty(gs[0].shape, dtype=torch.float32, device=gs[0].device)
+        srcs = (C.c_void_p * len(gs))(*[g.data_ptr() for g in gs])
+        call("hcp_sum_bf16_to_f32", srcs, len(gs), acc.numel(), acc.data_ptr(), stream_ptr())
+        if ctx.in_dtype == BF16:
+            return None, cast_bf16(acc)
+        return None, acc if ctx.in_dtype == torch.float32 else acc.to(ctx.in_dtype)
+
+
+def context_fanout(x: torch.Tensor, n: int):
+    return ContextFanoutFn.apply(n, x)
 
 
 def cast_bf16(x: torch.Tensor) -> torch.Tensor:

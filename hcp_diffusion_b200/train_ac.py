@@ -10,7 +10,14 @@ weight_decay, betas, eps}` for `torch.optim.AdamW` (the default `_target_`) or t
 constant_with_warmup), `loss.criterion` (`torch.nn.MSELoss` or `hcpdiff.loss.MinSNRLoss`-family `_target_` + `gamma`), `cfg_scale`
 (DreamArtist), `resume.{ckpt_path.unet, start_step}`; `model.ema` (`decay_max`, `inv_gamma`, `power`).
 
-Out of the hot path and therefore NOT here: datasets / buckets / captions, the CLIP text encoder, VAE, loggers, DeepSpeed /
+Text encoder (SD1.x CLIP): `lora_text_encoder` items train LoRA on it next to the UNet (reference train_ac.py:61,335):
+`model.text_encoder` (instantiable, default CLIP-L) with weights from `model.text_encoder_init`, `model.clip_skip`,
+`model.clip_final_norm`, `model.tokenizer_repeats`; `ckpts/text_encoder-<step>` is saved next to `unet-<step>` and
+`resume.ckpt_path.TE` is loaded.  A `text_encoder:` full fine-tune list, a non-null `tokenizer_pt.train` and DreamArtist++ items in
+`lora_text_encoder` raise NotImplementedError.  The ids are given (no tokenizer): `data.path` holds 'input_ids' [N, 77 R], or
+synthetic prompts are BOS 49406, random tokens, EOS 49407 padding.
+
+Out of the hot path and therefore NOT here: datasets / buckets / captions, a tokenizer, VAE, loggers, DeepSpeed /
 Colossal-AI trainers.  Inputs are the synthetic latents / text embeddings of SURVEY.md 8d (`data.synthetic`), or tensors saved
 in a .pt file (`data.path`: {'latents': [N,4,h,w], 'encoder_hidden_states': [N,L,768]}, plus 'text_embeds' / 'time_ids' for an
 SDXL ('text_time') UNet, whose synthetic time ids are (H, W, 0, 0, H, W) in pixels).
@@ -155,6 +162,10 @@ class Trainer:
         opt_name, af_opts = optimizer_from_cfg(opt_cfg)
         groups, self.lora = make_hcpdiff(self.unet, cfgs.get("unet"), cfgs.get("lora_unet"), default_lr=float(opt_cfg.get("lr", 1e-4)))
         groups = [{"params": g["params"], "lr": float(g["lr"]) * lr_scale} for g in groups if len(g["params"])]
+        self.te, self.te_lora, te_opts = self._build_text_encoder(cfgs)
+        if self.te is not None:
+            te_groups, self.te_lora = make_hcpdiff(self.te, None, cfgs.get("lora_text_encoder"), default_lr=1e-5)
+            groups += [{"params": g["params"], "lr": float(g["lr"]) * lr_scale} for g in te_groups if len(g["params"])]
         resume = tr.get("resume")
         self.start_step = 0
         if resume:
@@ -165,6 +176,10 @@ class Trainer:
                 if "lora" in sd:
                     load_lora_state(self.lora, sd["lora"])           # INTO the blocks being trained (see load_lora_state)
                     self.unet.load_state_dict(sd["lora"], strict=False)   # raw-key checkpoints (plugin_from_raw), as the reference does
+            for path in ((resume.get("ckpt_path", {}) or {}).get("TE", []) or []) if self.te is not None else []:
+                sd = auto_manager(path).load_ckpt(path)
+                if "lora" in sd:
+                    load_lora_state(self.te_lora, sd["lora"])
             self.start_step = int(resume.get("start_step", 0) or 0)
         ema_cfg = cfgs.model.get("ema")
         ema = None
@@ -176,7 +191,7 @@ class Trainer:
                                      max_grad_norm=float(tr.get("max_grad_norm", 1.0)), use_cuda_graph=bool(tr.get("cuda_graph", True)),
                                      grad_accum_steps=accum, loss=loss_from_cfg(tr.get("loss")), ema=ema,
                                      cfg_scale=None if cfg_scale in (None, "1.0", 1.0) else str(cfg_scale),
-                                     optimizer=opt_name, optimizer_kwargs=af_opts)
+                                     optimizer=opt_name, optimizer_kwargs=af_opts, text_encoder=self.te, text_encoder_opts=te_opts)
         self.step_fn.sync_params(src=0)
         self.sched_step = make_scheduler(tr.get("scheduler"), self.step_fn)
         self.bs, self.accum = bs, accum
@@ -189,6 +204,31 @@ class Trainer:
         ops.set_dropout_seed(seed + 7919 * (self.rank + 1))
         self._load_data(seed)
 
+    def _build_text_encoder(self, cfgs):
+        """(text encoder, None, encode_prompt options) when `lora_text_encoder` is set, else (None, None, None)."""
+        if cfgs.get("text_encoder"):
+            raise NotImplementedError("`text_encoder:` (full fine-tuning of the text encoder) is not supported; use lora_text_encoder")
+        tpt = cfgs.get("tokenizer_pt")
+        if tpt and tpt.get("train") is not None:
+            raise NotImplementedError("`tokenizer_pt.train` (prompt tuning / textual inversion) is not supported")
+        items = cfgs.get("lora_text_encoder")
+        if not items:
+            return None, None, None
+        for item in items:
+            if str(item.get("type", "lora")) != "lora":
+                raise NotImplementedError(f"lora_text_encoder item type {item.get('type')!r} (DreamArtist++ adapters) is not supported")
+        from .models import CLIPTextModel
+        te = cfgs.model.get("text_encoder")
+        te = instantiate(te) if isinstance(te, dict) else (te if te is not None else CLIPTextModel())
+        init = cfgs.model.get("text_encoder_init")
+        if init and init != "random":
+            sd = auto_manager(init).load_ckpt(init)
+            te.load_state_dict(sd.get("base", sd), strict=False)
+        te = te.to(self.device).requires_grad_(False).eval()
+        opts = {"n_repeats": int(cfgs.model.get("tokenizer_repeats", 1) or 1), "clip_skip": int(cfgs.model.get("clip_skip", 0) or 0),
+                "clip_final_norm": bool(cfgs.model.get("clip_final_norm", True))}
+        return te, None, opts
+
     def _load_data(self, seed: int):
         d = self.cfgs.data
         g = torch.Generator().manual_seed(1234 + self.rank)
@@ -197,7 +237,8 @@ class Trainer:
         self.text_embeds = self.time_ids = None
         if d.get("path"):
             blob = torch.load(d.path, map_location="cpu")
-            self.latents, self.ehs = blob["latents"].float(), blob["encoder_hidden_states"].float()
+            self.latents = blob["latents"].float()
+            self.ehs = blob["input_ids"].long() if self.te is not None else blob["encoder_hidden_states"].float()
             self.ehs_neg = blob.get("negative_hidden_states")
             if self.text_time:
                 self.text_embeds, self.time_ids = blob["text_embeds"].float(), blob["time_ids"].float()
@@ -208,6 +249,15 @@ class Trainer:
             self.latents = torch.randn((n, self.unet.config.in_channels, s, s), generator=gd)
             self.ehs = torch.randn((n, int(d.get("tokens", 77)), self.unet.config.cross_attention_dim), generator=gd)
             self.ehs_neg = torch.randn((n, int(d.get("tokens", 77)), self.unet.config.cross_attention_dim), generator=gd)
+            if self.te is not None:                              # prompts of 77-token chunks: BOS, random tokens, EOS padding
+                R = self.step_fn.te_opts["n_repeats"]
+                ids = torch.full((n * R, 77), 49407, dtype=torch.int64)
+                ids[:, 0] = 49406
+                lens = torch.randint(1, 76, (n * R,), generator=gd)
+                words = torch.randint(0, 49406, (n * R, 75), generator=gd)
+                keep = torch.arange(75)[None] < lens[:, None]
+                ids[:, 1:76] = torch.where(keep, words, ids[:, 1:76])
+                self.ehs = ids.reshape(n, 77 * R)
             if self.text_time:                                   # pooled text embedding ~ N(0,1); (H, W, 0, 0, H, W) in pixels
                 n_ids = 6
                 self.text_embeds = torch.randn((n, cfg.projection_class_embeddings_input_dim - n_ids * cfg.addition_time_embed_dim),
@@ -233,6 +283,9 @@ class Trainer:
         base_trained = any(p.requires_grad for n, p in self.unet.named_parameters() if "lora_block_" not in n)
         path = self.ckpt.save_model_with_lora(self.unet if base_trained else None, self.lora, "unet", step,
                                               ema_state=self.step_fn.ema_state() if self.step_fn.ema is not None else None)
+        if self.te is not None:
+            self.ckpt.save_model_with_lora(None, self.te_lora, "text_encoder", step,
+                                           ema_state=self.step_fn.ema_state() if self.step_fn.ema is not None else None)
         return path
 
     def train(self):

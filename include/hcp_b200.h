@@ -167,6 +167,13 @@ typedef struct hcp_attn_bwd_args {
 size_t hcp_attn_bwd_workspace_bytes(int64_t B, int64_t H, int64_t Lq, int64_t Lkv, int64_t d);
 int hcp_attn_bwd_bf16(const hcp_attn_bwd_args* args, hcp_stream_t stream);
 
+/* Causal self-attention: the same arguments with Lq == Lkv (else HCP_ERR_INVALID before any launch); query row i attends to kv
+ * columns <= i, kv_bias (if given) still adds on top.  The backward uses the same workspace size.
+ * Replaces: transformers CLIPAttention with CLIPTextTransformer's causal_attention_mask (text encoder self_attn, reference
+ *           cfgs/te_struct.txt; run every step when `lora_text_encoder` is set, hcpdiff/models/wrapper.py:14-30) and its backward. */
+int hcp_attn_fwd_causal_bf16(const hcp_attn_args* args, hcp_stream_t stream);
+int hcp_attn_bwd_causal_bf16(const hcp_attn_bwd_args* args, hcp_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------------
  * GroupNorm (+SiLU) over NHWC bf16, optionally over the channel concatenation [x1 | x2] (up-block skip
  * connections: the concat is never materialised un-normalised), forward and backward.
@@ -205,6 +212,25 @@ int hcp_layernorm_bwd_bf16(const void* x, const void* dy, const void* add, const
 /* GEGLU (cfgs/unet_struct.txt:27-30): u bf16 [M,2F] = [a | g];  h = a * gelu_erf(g);  du = [dh*gelu(g) | dh*a*gelu'(g)] */
 int hcp_geglu_fwd_bf16(const void* u, int64_t M, int64_t F, void* h, hcp_stream_t stream);
 int hcp_geglu_bwd_bf16(const void* u, const void* dh, int64_t M, int64_t F, void* du, hcp_stream_t stream);
+
+/* quick-GELU (transformers QuickGELUActivation, CLIPMLP.activation_fn, reference cfgs/te_struct.txt): x, y, dy, dx bf16 [M,F],
+ * F % 8 == 0;  y = x * sigmoid(1.702 x);  dx = dy * (s + 1.702 x s (1 - s)), s = sigmoid(1.702 x).  fp32 arithmetic. */
+int hcp_quick_gelu_fwd_bf16(const void* x, int64_t M, int64_t F, void* y, hcp_stream_t stream);
+int hcp_quick_gelu_bwd_bf16(const void* x, const void* dy, int64_t M, int64_t F, void* dx, hcp_stream_t stream);
+
+/* out fp32 [n] = srcs[0] + srcs[1] + ... + srcs[nsrc-1] (bf16 [n] each, n % 8 == 0), summed in fp32 in source order.
+ * Replaces: autograd's fp32 accumulation of the gradient of the fp32 text embedding, which the reference casts to bf16 separately for
+ *           every cross-attention under autocast (attn2.to_k / to_v, reference cfgs/unet_struct.txt:35-38; TEUnetWrapper.forward,
+ *           hcpdiff/models/wrapper.py:14-30). */
+int hcp_sum_bf16_to_f32(const void* const* srcs, int64_t nsrc, int64_t n, float* out, hcp_stream_t stream);
+
+/* Token + position embedding (transformers CLIPTextEmbeddings.forward, reference cfgs/te_struct.txt):
+ * out[b, l, :] = bf16(tok_emb[ids[b, l]] + pos_emb[pos_ids ? pos_ids[l] : l]).  ids int64 [B, L] and pos_ids int64 [L] (or NULL)
+ * live on the device, so the call can be captured in a CUDA graph; an id outside [0, V) (position outside [0, P)) is clamped to
+ * the nearest valid row -- the tables are never read out of bounds.  tok_emb fp32 [V, C], pos_emb fp32 [P, C], C % 8 == 0;
+ * without pos_ids, L <= P.  out bf16 [B, L, C]. */
+int hcp_embed_gather_bf16(const int64_t* ids, const int64_t* pos_ids, const float* tok_emb, int64_t V, const float* pos_emb, int64_t P,
+                          int64_t B, int64_t L, int64_t C, void* out, hcp_stream_t stream);
 
 /* nearest x2 upsample of NHWC bf16 [B,H,W,C] (Upsample2D, cfgs/unet_struct.txt:392) and its backward */
 int hcp_upsample2x_fwd_bf16(const void* x, int64_t B, int64_t H, int64_t W, int64_t C, void* y, hcp_stream_t stream);
