@@ -15,12 +15,14 @@
 //   online softmax       on the accumulator fragments (a row lives in the four lanes of a quad); exp2 with folded scale
 //   O += P V             wgmma RS: P (bf16) goes from the S registers straight into the A operand; V is used from its
 //                        row-major TMA box as an MN-major operand
-// Backward, one CTA per (128 kv rows, head, image, output column slice of 64) looping over 64-row query tiles; warpgroup g owns
-// kv rows [64g, 64g+64):
+// Backward, one CTA per (128 kv rows, head, image, output column slice of 64) looping over 64-row query tiles; two MMA warpgroups
+// and no producer warp (one thread issues the TMA loads), so that 255 registers per thread hold the live state without spills;
+// warpgroup g owns kv rows [64g, 64g+64):
 //   S^T = K Q^T, dP^T = V dO^T (registers) -> P^T, dS^T -> dV += P^T dO, dK += dS^T Q (wgmma RS, accumulators in registers),
-//   dQ_i += dS K over all 128 kv rows of the CTA (dS^T of both warpgroups staged in shared memory as one MN-major operand; the
-//   warpgroups take turns per query tile), reduced into an fp32 buffer with vector red.global: one contribution per CTA, so a
-//   short kv range (<= 2 tiles) sums dQ in an order-independent way.
+//   dQ_i += dS K over all 128 kv rows of the CTA (dS^T of both warpgroups staged in shared memory as one MN-major operand; warpgroup
+//   g computes output columns [32g, 32g+32) of the slice), reduced into an fp32 buffer with vector red.global: one contribution
+//   per CTA, so a short kv range (<= 2 tiles) sums dQ in an order-independent way.  lse and delta of a query tile arrive in shared
+//   memory with its Q / dO tiles (one 1-D bulk copy from a per-tile layout the prep kernel writes).
 // Causal variants (kCausal, Lq == Lkv: query row i sees kv columns <= i; CLIP's text encoder): the forward stops at the last kv
 // tile that meets its 128 query rows and masks by global row / column index; the backward starts its query loop at the first
 // 64-row tile that reaches its kv rows, and a CTA of a split query range with no tile left exits without writing.  The
@@ -32,7 +34,9 @@
 
 namespace hcp {
 
-constexpr int kAttnThreads = 288;          // warps 0-7: two MMA warpgroups, warp 8: TMA
+constexpr int kAttnThreads = 288;          // forward: warps 0-7: two MMA warpgroups, warp 8: TMA
+// backward: two MMA warpgroups and no producer warp -- at 8 warps (two per SM sub-partition) a thread may hold 255 registers
+constexpr int kAttnBwdThreads = 256;
 constexpr int BOX_BYTES = 128 * 128;       // one [128 rows x 64 cols] bf16 box
 constexpr float kLog2e = 1.4426950408889634f;
 constexpr float kLn2 = 0.6931471805599453f;
@@ -225,8 +229,7 @@ struct alignas(64) AttnBwdParams {
     int col0;                // output column slice [col0, col0 + 64) of this launch
     float scale, scale_log2;
     const float* kv_bias;
-    const float* lse;        // [B,H,Lq]
-    const float* delta;      // [B,H,Lq]  rowsum(dO * O)
+    const float* stats;      // [B,H,ceil(Lq/64),2,64]: per 64-row query tile lse * log2(e) (+inf past Lq), then rowsum(dO * O) (0 past Lq)
     float* dq_acc;           // [B,H,dq_ld/4,Lq,4] fp32
     int dq_ld;
     int qsplit;              // CTAs per kv tile along the query dimension
@@ -242,11 +245,12 @@ struct AttnBwdCfg {
     static constexpr int Q_BYTES = NB * QBOX;             // Q or dO: 64 rows
     static constexpr int STAGES = 2;
     static constexpr int DS_BYTES = 64 * 128;             // dS^T of one warpgroup: [64 kv][64 q] bf16 (the two are contiguous)
-    static constexpr int SMEM_BYTES = 2 * KV_BYTES + 2 * STAGES * Q_BYTES + 2 * DS_BYTES + 256 + 1024;
+    static constexpr int STAT_BYTES = 2 * 64 * 4;         // lse * log2(e) and delta of one query tile
+    static constexpr int SMEM_BYTES = 2 * KV_BYTES + 2 * STAGES * Q_BYTES + 2 * DS_BYTES + STAGES * STAT_BYTES + 256 + 1024;
 };
 
 template <int NB, bool kCausal>
-__global__ void __launch_bounds__(kAttnThreads, 1) attn_bwd_kernel(const __grid_constant__ AttnBwdParams p) {
+__global__ void __launch_bounds__(kAttnBwdThreads, 1) attn_bwd_kernel(const __grid_constant__ AttnBwdParams p) {
     using Cfg = AttnBwdCfg<NB>;
     constexpr int STAGES = Cfg::STAGES;
     extern __shared__ uint8_t smem_raw[];
@@ -256,15 +260,12 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attn_bwd_kernel(const __grid_
     uint8_t* sQ = sV + Cfg::KV_BYTES;                     // [STAGES]
     uint8_t* sdO = sQ + STAGES * Cfg::Q_BYTES;            // [STAGES]
     uint8_t* sDS = sdO + STAGES * Cfg::Q_BYTES;           // [2 warpgroups]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sDS + 2 * Cfg::DS_BYTES);
+    uint8_t* sStat = sDS + 2 * Cfg::DS_BYTES;             // [STAGES]
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sStat + STAGES * Cfg::STAT_BYTES);
     uint64_t* kv_full = bars;
     uint64_t* q_full = bars + 1;                          // [STAGES]
-    uint64_t* q_empty = bars + 1 + STAGES;                // [STAGES]
 
-    // Register-bound: 288 threads cap every thread at 168 registers, and S, dP, their bf16 fragments and the dV / dK / dQ accumulators
-    // do not fit; ptxas spills (~0.3 KB per thread) and serializes the wgmmas (C7512).  The thread-index form of the warp index below
-    // measured faster than warp_id_uniform() here (the latter spilled more).
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = warp_id_uniform(), lane = threadIdx.x & 31;
     const int kt = blockIdx.x / p.qsplit, qs = blockIdx.x % p.qsplit;
     const int h = blockIdx.y, b = blockIdx.z;
     const int nq = (p.Lq + 63) / 64;
@@ -273,41 +274,41 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attn_bwd_kernel(const __grid_
     // nothing: it exits before touching memory, so the fp32 dQ / dK / dV sums get no extra (zero) terms.
     const int i0 = kCausal ? max(qs * per, 2 * kt) : qs * per, i1 = min(nq, qs * per + per);
     if (kCausal && i0 >= i1) return;
+    const int64_t bh = (int64_t)b * p.H + h;
 
     if (threadIdx.x == 0) {
         mbar_init(kv_full, 1);
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&q_full[s], 1); mbar_init(&q_empty[s], 256); }
+        for (int s = 0; s < STAGES; ++s) mbar_init(&q_full[s], 1);
         fence_mbar_init();
     }
     __syncthreads();
     pdl_trigger();
     pdl_wait();
 
-    if (warp == 8) {
-        if (elect_one()) {
-            mbar_arrive_expect_tx(kv_full, 2 * Cfg::KV_BYTES);
-            for (int bx = 0; bx < NB; ++bx) {
-                tma_load_4d(sK + bx * BOX_BYTES, &p.tmK, kv_full, bx * 64, h, kt * 128, b);
-                tma_load_4d(sV + bx * BOX_BYTES, &p.tmV, kv_full, bx * 64, h, kt * 128, b);
-            }
-            for (int i = i0; i < i1; ++i) {
-                const int st = (i - i0) % STAGES;
-                mbar_wait(&q_empty[st], (((i - i0) / STAGES) & 1) ^ 1);
-                mbar_arrive_expect_tx(&q_full[st], 2 * Cfg::Q_BYTES);
-                for (int bx = 0; bx < NB; ++bx) {
-                    tma_load_4d(sQ + st * Cfg::Q_BYTES + bx * Cfg::QBOX, &p.tmQ, &q_full[st], bx * 64, h, i * 64, b);
-                    tma_load_4d(sdO + st * Cfg::Q_BYTES + bx * Cfg::QBOX, &p.tmdO, &q_full[st], bx * 64, h, i * 64, b);
-                }
-            }
+    // Thread 0 issues every load: K / V once, then Q, dO and the statistics of query tile i into stage (i - i0) % STAGES.  A stage is
+    // refilled after the end-of-iteration barrier of the tile that used it: both warpgroups' wgmmas on it have completed by then.
+    auto load_q = [&](int i) {
+        const int st = (i - i0) % STAGES;
+        mbar_arrive_expect_tx(&q_full[st], 2 * Cfg::Q_BYTES + Cfg::STAT_BYTES);
+        for (int bx = 0; bx < NB; ++bx) {
+            tma_load_4d(sQ + st * Cfg::Q_BYTES + bx * Cfg::QBOX, &p.tmQ, &q_full[st], bx * 64, h, i * 64, b);
+            tma_load_4d(sdO + st * Cfg::Q_BYTES + bx * Cfg::QBOX, &p.tmdO, &q_full[st], bx * 64, h, i * 64, b);
         }
-        return;
+        bulk_load(sStat + st * Cfg::STAT_BYTES, p.stats + (bh * nq + i) * 128, Cfg::STAT_BYTES, &q_full[st]);
+    };
+    if (threadIdx.x == 0) {
+        mbar_arrive_expect_tx(kv_full, 2 * Cfg::KV_BYTES);
+        for (int bx = 0; bx < NB; ++bx) {
+            tma_load_4d(sK + bx * BOX_BYTES, &p.tmK, kv_full, bx * 64, h, kt * 128, b);
+            tma_load_4d(sV + bx * BOX_BYTES, &p.tmV, kv_full, bx * 64, h, kt * 128, b);
+        }
+        for (int i = i0; i < min(i1, i0 + STAGES); ++i) load_q(i);
     }
 
     const int wg = warp >> 2;
     const int g = lane >> 2, cq = 2 * (lane & 3);
     const int r0 = (warp & 3) * 16 + g;                  // rows r0, r0 + 8 of this warpgroup's 64 kv rows
     const int kvw = kt * 128 + wg * 64;
-    const int64_t bh = (int64_t)b * p.H + h;
     const float sl2 = p.scale_log2, scale = p.scale;
     const int cbox = p.col0 / 64;                        // box holding the output column slice
     float kvb[2];
@@ -323,8 +324,12 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attn_bwd_kernel(const __grid_
     for (int i = 0; i < 32; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
     const uint64_t kdesc = make_smem_desc(smem_u32(sK) + wg * 64 * 128, 16, 1024);
     const uint64_t vdesc = make_smem_desc(smem_u32(sV) + wg * 64 * 128, 16, 1024);
-    // dQ: A = dS^T of all 128 kv rows read transposed, B = the 128 K rows, output columns of the slice (both MN-major)
-    const uint64_t kdesc_mn = make_smem_desc(smem_u32(sK) + cbox * BOX_BYTES, BOX_BYTES, 1024);
+    // dQ: A = dS^T of all 128 kv rows read transposed, B = the 128 K rows (both MN-major); warpgroup g computes the 32 output
+    // columns [32g, 32g + 32) of the slice.  The MN-major SWIZZLE_128B operand starts 64 bytes into its swizzle rows for g = 1: the
+    // swizzle is a function of the shared-memory address bits, so the 32-column half reads as a 64-column one does.
+    const int dq_col = p.col0 + 32 * wg;
+    const bool dq_cols = dq_col < p.d;                   // warpgroup-uniform: the half holds at least one column of the head
+    const uint64_t kdesc_mn = make_smem_desc(smem_u32(sK) + cbox * BOX_BYTES + wg * 64, BOX_BYTES, 1024);
     const uint32_t ds_base = smem_u32(sDS) + wg * Cfg::DS_BYTES;
     const uint64_t dsdesc = make_smem_desc(smem_u32(sDS), 2 * Cfg::DS_BYTES, 1024);
     mbar_wait(kv_full, 0);
@@ -332,6 +337,7 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attn_bwd_kernel(const __grid_
         const int st = (i - i0) % STAGES;
         mbar_wait(&q_full[st], ((i - i0) / STAGES) & 1);
         const uint32_t qb = smem_u32(sQ + st * Cfg::Q_BYTES), dob = smem_u32(sdO + st * Cfg::Q_BYTES);
+        const uint32_t statb = smem_u32(sStat + st * Cfg::STAT_BYTES);
         const uint64_t qdesc = make_smem_desc(qb, 16, 1024), dodesc = make_smem_desc(dob, 16, 1024);
         // ---- S^T = K Q^T, dP^T = V dO^T  (rows: kv, columns: q)
         float s[32], dp[32];
@@ -351,14 +357,15 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attn_bwd_kernel(const __grid_
         const bool diag = kCausal && i < 2 * kt + 2;             // the query tile starts inside the CTA's kv rows
 #pragma unroll
         for (int kk = 0; kk < 4; ++kk) {
-            // per-column (query) statistics of the four columns of this k-step this thread holds
+            // per-column (query) statistics of the four columns of this k-step this thread holds; a query row past Lq has lse = +inf,
+            // so P = exp2(-inf) = 0 there
             float lq[4], dq_[4];
 #pragma unroll
-            for (int c = 0; c < 4; ++c) {
-                const int q = i * 64 + 16 * kk + 8 * (c >> 1) + cq + (c & 1);
-                const bool ok = q < p.Lq;
-                lq[c] = ok ? __ldg(p.lse + bh * p.Lq + q) * kLog2e : INFINITY;   // masked query: P = exp2(-inf) = 0
-                dq_[c] = ok ? __ldg(p.delta + bh * p.Lq + q) : 0.f;
+            for (int c2 = 0; c2 < 2; ++c2) {
+                const uint32_t a = statb + (16 * kk + 8 * c2 + cq) * 4;
+                const float2 l2 = lds_f32x2(a), d2 = lds_f32x2(a + 64 * 4);
+                lq[2 * c2] = l2.x; lq[2 * c2 + 1] = l2.y;
+                dq_[2 * c2] = d2.x; dq_[2 * c2 + 1] = d2.y;
             }
 #pragma unroll
             for (int r = 0; r < 4; ++r) {
@@ -382,40 +389,36 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attn_bwd_kernel(const __grid_
         }
         fence_proxy_async_smem();
         asm volatile("bar.sync 1, 256;" ::: "memory");                   // dS^T of both warpgroups in shared memory
-        // ---- dV += P^T dO, dK += dS^T Q (slice columns; MN-major B); one warpgroup: dQ_i = dS K over the CTA's 128 kv rows
-        const bool dq_here = ((i - i0) & 1) == wg;
+        // ---- dV += P^T dO, dK += dS^T Q (slice columns; MN-major B); dQ_i = dS K over the CTA's 128 kv rows, this warpgroup's half
         const uint64_t dodesc_mn = make_smem_desc(dob + cbox * Cfg::QBOX, Cfg::QBOX, 1024);
         const uint64_t qdesc_mn = make_smem_desc(qb + cbox * Cfg::QBOX, Cfg::QBOX, 1024);
-        float dqa[32];
+        float dqa[16];
         wgmma_fence();
 #pragma unroll
         for (int kk = 0; kk < 4; ++kk) wgmma_rs<64, 1>(dv, pa[kk], desc_adv(dodesc_mn, kk * 128), 1u);
 #pragma unroll
         for (int kk = 0; kk < 4; ++kk) wgmma_rs<64, 1>(dk, da[kk], desc_adv(qdesc_mn, kk * 128), 1u);
-        wgmma_commit();
-        wgmma_wait<0>();                                 // P^T / dS^T registers free before the dQ accumulator is live
-        wgmma_fence_acc(dv);
-        wgmma_fence_acc(dk);
-        if (dq_here) {
-            wgmma_fence();
-            wgmma_ss<64, 1, 1>(dqa, dsdesc, kdesc_mn, 0u);
+        if (dq_cols) {
+            wgmma_ss<32, 1, 1>(dqa, dsdesc, kdesc_mn, 0u);
 #pragma unroll
-            for (int kk = 1; kk < 8; ++kk) wgmma_ss<64, 1, 1>(dqa, desc_adv(dsdesc, kk * 128), desc_adv(kdesc_mn, kk * 128), 1u);
+            for (int kk = 1; kk < 8; ++kk) wgmma_ss<32, 1, 1>(dqa, desc_adv(dsdesc, kk * 128), desc_adv(kdesc_mn, kk * 128), 1u);
         }
         wgmma_commit();
         wgmma_wait<0>();
+        wgmma_fence_acc(dv);
+        wgmma_fence_acc(dk);
         wgmma_fence_acc(dqa);
-        mbar_arrive(&q_empty[st]);
-        asm volatile("bar.sync 1, 256;" ::: "memory");                   // the dS^T tiles may be overwritten by the next query tile
-        if (!dq_here) continue;
-        // ---- dQ of the CTA's kv rows -> fp32 accumulator [B,H,dq_ld/4,Lq,4]
+        asm volatile("bar.sync 1, 256;" ::: "memory");   // stage st and the dS^T tiles are no longer read by either warpgroup
+        if (threadIdx.x == 0 && i + STAGES < i1) load_q(i + STAGES);
+        if (!dq_cols) continue;
+        // ---- dQ of the CTA's kv rows, this warpgroup's 32 columns -> fp32 accumulator [B,H,dq_ld/4,Lq,4]
 #pragma unroll
         for (int hh = 0; hh < 2; ++hh) {
             const int q = i * 64 + r0 + 8 * hh;
             if (q >= p.Lq) continue;
 #pragma unroll
-            for (int c8 = 0; c8 < 8; ++c8) {
-                const int col = p.col0 + 8 * c8 + cq;
+            for (int c8 = 0; c8 < 4; ++c8) {
+                const int col = dq_col + 8 * c8 + cq;
                 if (col < p.d) red_add_v2(p.dq_acc + ((bh * (p.dq_ld / 4) + col / 4) * p.Lq + q) * 4 + (col & 3), dqa[4 * c8 + 2 * hh], dqa[4 * c8 + 2 * hh + 1]);
             }
         }
@@ -443,12 +446,15 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attn_bwd_kernel(const __grid_
     }
 }
 
-// delta[b,h,q] = sum_e dO*O ; also zero-fills the fp32 dQ / dK,dV accumulators (when present).  One thread per (b,q,h): the
-// d elements of a head are contiguous (d % 8 == 0 -> 16-byte loads) and adjacent threads read adjacent heads of the same token
-// row, so a warp streams contiguous memory.
+// Per-query statistics of the backward, laid out per 64-row query tile so that the kernel fetches a tile's with one bulk copy:
+// stats[b,h,q/64] = {lse * log2(e) of its 64 rows, delta = sum_e dO*O of its 64 rows}; rows past Lq get lse = +inf (P = 0) and
+// delta = 0.  Also zero-fills the fp32 dQ / dK,dV accumulators (when present).  One thread per (b,q,h): the d elements of a head are
+// contiguous (d % 8 == 0 -> 16-byte loads) and adjacent threads read adjacent heads of the same token row, so a warp streams
+// contiguous memory.
 __global__ void __launch_bounds__(256) attn_bwd_prep_kernel(const __nv_bfloat16* __restrict__ O, int64_t ldo,
-                                                            const __nv_bfloat16* __restrict__ dO, int64_t lddo, int B, int H, int Lq,
-                                                            int d, float* __restrict__ delta, float* __restrict__ dq_acc,
+                                                            const __nv_bfloat16* __restrict__ dO, int64_t lddo,
+                                                            const float* __restrict__ lse, int B, int H, int Lq, int d,
+                                                            float* __restrict__ stats, float* __restrict__ dq_acc,
                                                             int64_t dq_n, float* __restrict__ dkv_acc, int64_t dkv_n) {
     pdl_trigger();
     pdl_wait();
@@ -462,14 +468,22 @@ __global__ void __launch_bounds__(256) attn_bwd_prep_kernel(const __nv_bfloat16*
         float4* z = reinterpret_cast<float4*>(dkv_acc);
         for (int64_t i = gtid; i < dkv_n / 4; i += nthreads) z[i] = make_float4(0.f, 0.f, 0.f, 0.f);
     }
-    const int64_t total = (int64_t)B * Lq * H;
+    const int nq = (Lq + 63) / 64;
+    const int64_t total = (int64_t)B * nq * 64 * H;
     if (gtid >= total) return;
     const int h = (int)(gtid % H);
     const int64_t bq = gtid / H;
-    const int q = (int)(bq % Lq);
-    const int b = (int)(bq / Lq);
-    const uint4* o = reinterpret_cast<const uint4*>(O + bq * ldo + (int64_t)h * d);
-    const uint4* g = reinterpret_cast<const uint4*>(dO + bq * lddo + (int64_t)h * d);
+    const int q = (int)(bq % (nq * 64));
+    const int b = (int)(bq / (nq * 64));
+    float* st = stats + (((int64_t)b * H + h) * nq + q / 64) * 128 + (q & 63);
+    if (q >= Lq) {
+        st[0] = INFINITY;
+        st[64] = 0.f;
+        return;
+    }
+    const int64_t row = (int64_t)b * Lq + q;
+    const uint4* o = reinterpret_cast<const uint4*>(O + row * ldo + (int64_t)h * d);
+    const uint4* g = reinterpret_cast<const uint4*>(dO + row * lddo + (int64_t)h * d);
     float acc = 0.f;
     for (int e = 0; e < d / 8; ++e) {
         const uint4 a = o[e], c = g[e];
@@ -479,7 +493,8 @@ __global__ void __launch_bounds__(256) attn_bwd_prep_kernel(const __nv_bfloat16*
         x = unpack_bf16x2(a.z); y = unpack_bf16x2(c.z); acc += x.x * y.x + x.y * y.y;
         x = unpack_bf16x2(a.w); y = unpack_bf16x2(c.w); acc += x.x * y.x + x.y * y.y;
     }
-    delta[((int64_t)b * H + h) * Lq + q] = acc;
+    st[0] = lse[((int64_t)b * H + h) * Lq + q] * kLog2e;
+    st[64] = acc;
 }
 
 // dQ bf16 [B, Lq, lddq] <- fp32 accumulator [B,H,dq_ld/4,Lq,4]
@@ -566,7 +581,7 @@ static int launch_attn_bwd(const AttnBwdParams& p, dim3 grid, cudaStream_t strea
         if (e != cudaSuccess) return set_cuda_error(e, "cudaFuncSetAttribute(attn_bwd)");
         configured = true;
     }
-    launch_k(attn_bwd_kernel<NB, kCausal>, grid, dim3(kAttnThreads), Cfg::SMEM_BYTES, stream, p);
+    launch_k(attn_bwd_kernel<NB, kCausal>, grid, dim3(kAttnBwdThreads), Cfg::SMEM_BYTES, stream, p);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return set_cuda_error(e, "attn_bwd launch");
     return HCP_OK;
@@ -622,7 +637,7 @@ static int plan_qsplit(int64_t B, int64_t H, int64_t Lq, int64_t Lkv) {
 
 extern "C" size_t hcp_attn_bwd_workspace_bytes(int64_t B, int64_t H, int64_t Lq, int64_t Lkv, int64_t d) {
     const int64_t dq_ld = (d + 3) / 4 * 4;
-    size_t n = (size_t)((B * H * Lq + 3) / 4 * 4) + (size_t)(B * H * Lq * dq_ld);   // delta (padded to 16 bytes) + dQ accumulator
+    size_t n = (size_t)(B * H * ((Lq + 63) / 64) * 128) + (size_t)(B * H * Lq * dq_ld);   // per-tile lse / delta + dQ accumulator
     if (plan_qsplit(B, H, Lq, Lkv) > 1) n += (size_t)(B * H * Lkv * 2 * dq_ld);
     return n * sizeof(float);
 }
@@ -639,17 +654,17 @@ static int attn_bwd(const hcp_attn_bwd_args* a, hcp_stream_t stream_) {
     if ((a->ldo % 8) != 0 || (a->lddo % 8) != 0 || (a->lddq % 8) != 0) return set_error(HCP_ERR_INVALID, "attn_bwd: leading dimensions must be multiples of 8");
     cudaStream_t stream = (cudaStream_t)stream_;
     const int dq_ld = (int)((a->d + 3) / 4 * 4);
-    float* delta = a->workspace;
-    float* dq_acc = a->workspace + (a->B * a->H * a->Lq + 3) / 4 * 4;
+    float* stats = a->workspace;
+    float* dq_acc = a->workspace + a->B * a->H * ((a->Lq + 63) / 64) * 128;
     const int qsplit = plan_qsplit(a->B, a->H, a->Lq, a->Lkv);
     const int64_t dkv_n = qsplit > 1 ? a->B * a->H * a->Lkv * 2 * dq_ld : 0;
     float* dkv_acc = qsplit > 1 ? dq_acc + a->B * a->H * a->Lq * dq_ld : nullptr;
     {
-        const int64_t total = a->B * a->Lq * a->H;
+        const int64_t total = a->B * ((a->Lq + 63) / 64 * 64) * a->H;
         const int threads = 256;
         const int64_t blocks = (total + threads - 1) / threads;
         launch_k(attn_bwd_prep_kernel, dim3((unsigned)blocks), dim3(threads), 0, stream, (const __nv_bfloat16*)a->o, a->ldo,
-                 (const __nv_bfloat16*)a->dout, a->lddo, (int)a->B, (int)a->H, (int)a->Lq, (int)a->d, delta,
+                 (const __nv_bfloat16*)a->dout, a->lddo, (const float*)a->lse, (int)a->B, (int)a->H, (int)a->Lq, (int)a->d, stats,
                  dq_acc, (int64_t)(a->B * a->H * a->Lq * dq_ld), dkv_acc, dkv_n);
     }
     AttnBwdParams p;
@@ -663,8 +678,7 @@ static int attn_bwd(const hcp_attn_bwd_args* a, hcp_stream_t stream_) {
     p.scale = a->scale;
     p.scale_log2 = a->scale * kLog2e;
     p.kv_bias = a->kv_bias;
-    p.lse = a->lse;
-    p.delta = delta;
+    p.stats = stats;
     p.dq_acc = dq_acc;
     p.dq_ld = dq_ld;
     p.qsplit = qsplit;

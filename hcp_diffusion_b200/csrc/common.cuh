@@ -140,6 +140,12 @@ __device__ __forceinline__ void tma_load_5d(void* smem, const CUtensorMap* m, ui
         "r"(c3), "r"(c4)
         : "memory");
 }
+// 1-D bulk copy of `bytes` (a multiple of 16; both addresses 16-byte aligned) from global to shared memory, completion on an mbarrier
+__device__ __forceinline__ void bulk_load(void* smem, const void* gmem, uint32_t bytes, uint64_t* bar) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 ::"r"(smem_u32(smem)), "l"(reinterpret_cast<uint64_t>(gmem)), "r"(bytes), "r"(smem_u32(bar))
+                 : "memory");
+}
 
 // ---------------------------------------------------------------------------------------------
 // wgmma shared-memory matrix descriptor (64 bit):
@@ -202,6 +208,11 @@ __device__ __forceinline__ float fast_exp2(float x) {
 __device__ __forceinline__ uint4 lds128(uint32_t a) {
     uint4 v;
     asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(a) : "memory");
+    return v;
+}
+__device__ __forceinline__ float2 lds_f32x2(uint32_t a) {
+    float2 v;
+    asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(a) : "memory");
     return v;
 }
 
