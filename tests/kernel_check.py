@@ -22,6 +22,18 @@ bf16 keeps 8 significand bits, so rounding an output alone costs up to 2^-9 = 2.
   LORA  LoRA factor gradients (fp32 atomics over       2.50e-3 / 2.59e-3 / 3.19e-3              6e-3 / 8e-3 / 1e-2
         bf16 rank products T / U)
   LSE   attention lse (fp32 natural log; absolute)     1.07e-3                                  3e-3
+
+The normalisation, weight-gradient and time-embedding kernels (tests/test_gpu_norm_wgrad_edges.py, same H100):
+
+  NORM    GroupNorm / LayerNorm y and dx (fp32         1.69e-3 / 2.15e-3 / 3.51e-3              4e-3 / 6e-3 / 9e-3
+          statistics, one bf16 rounding of the output)
+  STAT    GroupNorm / LayerNorm mean (in units of the  4.3e-8 (mean) / 5.5e-7 (rstd)             1.5e-6
+          standard deviation) and rstd (relative), fp32
+  F32SUM  fp32 sums of bf16 (or fp32) products: weight  6.00e-7 / 6.09e-7 / 7.27e-7              1.5e-6 / 1.5e-6 / 2e-6
+          gradients, column sums, affine gradients, the
+          small time-embedding linears, the boundary convolutions' fp32 outputs
+  F32SIN  the skinny linear on sinusoidal embeddings    6.05e-6 / 6.83e-6 / 1.01e-5              2e-5 / 2e-5 / 3e-5
+          of timesteps up to 999 (fp32 argument t * freq)
 """
 from dataclasses import dataclass
 
@@ -41,6 +53,10 @@ FWD = Tol(rel=6e-3, block=8e-3, maxabs=1.2e-2)
 GRAD = Tol(rel=6e-3, block=1e-2, maxabs=1.5e-2)
 LORA = Tol(rel=6e-3, block=8e-3, maxabs=1e-2)
 LSE_ABS = 3e-3
+NORM = Tol(rel=4e-3, block=6e-3, maxabs=9e-3)
+STAT = 1.5e-6
+F32SUM = Tol(rel=1.5e-6, block=1.5e-6, maxabs=2e-6)
+F32SIN = Tol(rel=2e-5, block=2e-5, maxabs=3e-5)
 
 
 def compare(name: str, got: torch.Tensor, ref: torch.Tensor, tol: Tol, block=(128, 128)) -> None:
@@ -74,18 +90,21 @@ def compare(name: str, got: torch.Tensor, ref: torch.Tensor, tol: Tol, block=(12
 
 
 class Canary:
-    """A bf16 buffer of `rows + 2 * pad` rows x `ld` columns prefilled with 0xFFFF; `view` is the rows x cols output rectangle that
-    starts `pad` rows down and `col0` columns in.  `check()` asserts that no element outside the rectangle changed, bit for bit."""
+    """A bf16 (or fp32: `dtype=torch.float32`, pattern 0xFFFFFFFF) buffer of `rows + 2 * pad` rows x `ld` columns prefilled with all
+    ones; `view` is the rows x cols output rectangle that starts `pad` rows down and `col0` columns in.  `check()` asserts that no
+    element outside the rectangle changed, bit for bit."""
 
-    def __init__(self, rows: int, cols: int, ld: int = 0, pad: int = 3, col0: int = 8, device="cuda"):
-        ld = ld or cols + 64
+    def __init__(self, rows: int, cols: int, ld: int = 0, pad: int = 3, col0: int = 8, device="cuda", dtype=torch.bfloat16):
+        ld = ld or (cols + 71) // 8 * 8
         assert col0 + cols <= ld and ld % 8 == 0 and col0 % 8 == 0
-        self.buf = torch.full((rows + 2 * pad, ld), CANARY, dtype=torch.int16, device=device).view(torch.bfloat16)
+        self.bits = torch.int16 if dtype == torch.bfloat16 else torch.int32
+        assert dtype in (torch.bfloat16, torch.float32)
+        self.buf = torch.full((rows + 2 * pad, ld), CANARY, dtype=self.bits, device=device).view(dtype)
         self.view = self.buf[pad:pad + rows, col0:col0 + cols]
         self.ld, self.rect = ld, (pad, pad + rows, col0, col0 + cols)
 
     def check(self, name: str) -> None:
-        bits = self.buf.view(torch.int16).clone()
+        bits = self.buf.view(self.bits).clone()
         r0, r1, c0, c1 = self.rect
         bits[r0:r1, c0:c1] = CANARY
         stray = int((bits != CANARY).sum())

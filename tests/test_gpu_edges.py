@@ -312,6 +312,11 @@ ATTN_CASES = [
     (2, 10, 4096, 4096, 64, True, 0), (2, 10, 4096, 77, 64, False, 0), (1, 20, 1024, 1024, 64, True, 64),
     # backward query splits on a 132-SM H100: two (order-independent dK / dV partials), 32 (fp32 partial sums of dK / dV)
     (1, 8, 256, 256, 64, True, 0), (1, 2, 4096, 256, 80, False, 0),
+    # dQ split by output column between the two warpgroups (32-column slices): d 96 (three full slices), 112 / 176 (a part-filled
+    # warpgroup-1 half after the first slice), 160 (SD1.5's deepest head dim: warpgroup 1 has no column in the third slice) at a
+    # query-split shape and as a 77-token cross-attention
+    (1, 2, 200, 200, 96, False, 0), (1, 2, 257, 257, 112, True, 64), (1, 8, 256, 256, 160, True, 0), (2, 4, 300, 77, 160, False, 8),
+    (1, 2, 129, 77, 176, False, 0),
 ]
 
 
@@ -320,7 +325,7 @@ def test_attention_edges(B, H, Lq, Lkv, d, fused, pad):
     check_attention(AttnProblem(B, H, Lq, Lkv, d, fused, pad), f"attn B{B} H{H} Lq{Lq} Lkv{Lkv} d{d}")
 
 
-@pytest.mark.parametrize("d", [64, 128])
+@pytest.mark.parametrize("d", [64, 128, 160])
 @pytest.mark.parametrize("kind", ["large_logits", "masked_first_tile", "one_key"])
 def test_attention_online_softmax_stress(kind, d):
     """Scores spanning about +-30 with a planted row maximum (~+45) in the first kv tile for odd query rows and in the last for even
