@@ -15,12 +15,12 @@
 //   online softmax       on the accumulator fragments (a row lives in the four lanes of a quad); exp2 with folded scale
 //   O += P V             wgmma RS: P (bf16) goes from the S registers straight into the A operand; V is used from its
 //                        row-major TMA box as an MN-major operand
-// Backward, one CTA per (128 kv rows, head, image, output column slice of 64) looping over 64-row query tiles; two MMA warpgroups
+// Backward, one CTA per (128 kv rows, head, image, output column slice of up to 64) looping over 64-row query tiles; two MMA warpgroups
 // and no producer warp (one thread issues the TMA loads), so that 255 registers per thread hold the live state without spills;
 // warpgroup g owns kv rows [64g, 64g+64):
 //   S^T = K Q^T, dP^T = V dO^T (registers) -> P^T, dS^T -> dV += P^T dO, dK += dS^T Q (wgmma RS, accumulators in registers),
-//   dQ_i += dS K over all 128 kv rows of the CTA (dS^T of both warpgroups staged in shared memory as one MN-major operand; warpgroup
-//   g computes output columns [32g, 32g+32) of the slice), reduced into an fp32 buffer with vector red.global: one contribution
+//   dQ_i += dS K over all 128 kv rows of the CTA (dS^T of both warpgroups staged in shared memory as one MN-major operand; the two
+//   warpgroups split the slice's columns), reduced into an fp32 buffer with vector red.global: one contribution
 //   per CTA, so a short kv range (<= 2 tiles) sums dQ in an order-independent way.  lse and delta of a query tile arrive in shared
 //   memory with its Q / dO tiles (one 1-D bulk copy from a per-tile layout the prep kernel writes).
 // Causal variants (kCausal, Lq == Lkv: query row i sees kv columns <= i; CLIP's text encoder): the forward stops at the last kv
@@ -249,10 +249,14 @@ struct AttnBwdCfg {
     static constexpr int SMEM_BYTES = 2 * KV_BYTES + 2 * STAGES * Q_BYTES + 2 * DS_BYTES + STAGES * STAT_BYTES + 256 + 1024;
 };
 
-template <int NB, bool kCausal>
+// W = columns of the output slice [col0, col0 + W) (a multiple of 8, at most 64): dV / dK run at N = W, and the dQ columns are split
+// DQ0 + DQ1 = W between the warpgroups, so that no MMA computes a column past the head.
+template <int NB, int W, bool kCausal>
 __global__ void __launch_bounds__(kAttnBwdThreads, 1) attn_bwd_kernel(const __grid_constant__ AttnBwdParams p) {
     using Cfg = AttnBwdCfg<NB>;
     constexpr int STAGES = Cfg::STAGES;
+    constexpr int DQ0 = (W + 15) / 16 * 8, DQ1 = W - DQ0;
+    static_assert(W % 8 == 0 && W >= 8 && W <= 64, "attn_bwd: slice width");
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* sK = smem;
@@ -319,17 +323,17 @@ __global__ void __launch_bounds__(kAttnBwdThreads, 1) attn_bwd_kernel(const __gr
         kv_ok[hh] = kv < p.Lkv;
         kvb[hh] = (p.kv_bias && kv_ok[hh]) ? p.kv_bias[(int64_t)b * p.Lkv + kv] * kLog2e : 0.f;
     }
-    float dv[32], dk[32];
+    float dv[W / 2], dk[W / 2];
 #pragma unroll
-    for (int i = 0; i < 32; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
+    for (int i = 0; i < W / 2; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
     const uint64_t kdesc = make_smem_desc(smem_u32(sK) + wg * 64 * 128, 16, 1024);
     const uint64_t vdesc = make_smem_desc(smem_u32(sV) + wg * 64 * 128, 16, 1024);
-    // dQ: A = dS^T of all 128 kv rows read transposed, B = the 128 K rows (both MN-major); warpgroup g computes the 32 output
-    // columns [32g, 32g + 32) of the slice.  The MN-major SWIZZLE_128B operand starts 64 bytes into its swizzle rows for g = 1: the
-    // swizzle is a function of the shared-memory address bits, so the 32-column half reads as a 64-column one does.
-    const int dq_col = p.col0 + 32 * wg;
-    const bool dq_cols = dq_col < p.d;                   // warpgroup-uniform: the half holds at least one column of the head
-    const uint64_t kdesc_mn = make_smem_desc(smem_u32(sK) + cbox * BOX_BYTES + wg * 64, BOX_BYTES, 1024);
+    // dQ: A = dS^T of all 128 kv rows read transposed, B = the 128 K rows (both MN-major); warpgroup 0 computes the first DQ0 columns
+    // of the slice, warpgroup 1 the DQ1 after them.  Warpgroup 1's MN-major SWIZZLE_128B operand starts 2 * DQ0 bytes (16, 32, 48 or
+    // 64) into its swizzle rows: the swizzle is a function of the shared-memory address bits, so it reads as one starting at a row does.
+    const int dq_col = p.col0 + (wg ? DQ0 : 0);
+    const bool dq_cols = wg == 0 || DQ1 > 0;             // warpgroup-uniform: the warpgroup has dQ columns
+    const uint64_t kdesc_mn = make_smem_desc(smem_u32(sK) + cbox * BOX_BYTES + (wg ? 2 * DQ0 : 0), BOX_BYTES, 1024);
     const uint32_t ds_base = smem_u32(sDS) + wg * Cfg::DS_BYTES;
     const uint64_t dsdesc = make_smem_desc(smem_u32(sDS), 2 * Cfg::DS_BYTES, 1024);
     mbar_wait(kv_full, 0);
@@ -392,36 +396,47 @@ __global__ void __launch_bounds__(kAttnBwdThreads, 1) attn_bwd_kernel(const __gr
         // ---- dV += P^T dO, dK += dS^T Q (slice columns; MN-major B); dQ_i = dS K over the CTA's 128 kv rows, this warpgroup's half
         const uint64_t dodesc_mn = make_smem_desc(dob + cbox * Cfg::QBOX, Cfg::QBOX, 1024);
         const uint64_t qdesc_mn = make_smem_desc(qb + cbox * Cfg::QBOX, Cfg::QBOX, 1024);
-        float dqa[16];
+        float dqa0[DQ0 / 2], dqa1[DQ1 > 0 ? DQ1 / 2 : 4];   // warpgroup 0's / 1's dQ columns (separate arrays: one aliased array
+                                                             // of two widths makes ptxas serialize the wgmmas, C7511)
         wgmma_fence();
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk) wgmma_rs<64, 1>(dv, pa[kk], desc_adv(dodesc_mn, kk * 128), 1u);
+        for (int kk = 0; kk < 4; ++kk) wgmma_rs<W, 1>(dv, pa[kk], desc_adv(dodesc_mn, kk * 128), 1u);
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk) wgmma_rs<64, 1>(dk, da[kk], desc_adv(qdesc_mn, kk * 128), 1u);
-        if (dq_cols) {
-            wgmma_ss<32, 1, 1>(dqa, dsdesc, kdesc_mn, 0u);
+        for (int kk = 0; kk < 4; ++kk) wgmma_rs<W, 1>(dk, da[kk], desc_adv(qdesc_mn, kk * 128), 1u);
+        if (wg == 0) {
+            wgmma_ss<DQ0, 1, 1>(dqa0, dsdesc, kdesc_mn, 0u);
 #pragma unroll
-            for (int kk = 1; kk < 8; ++kk) wgmma_ss<32, 1, 1>(dqa, desc_adv(dsdesc, kk * 128), desc_adv(kdesc_mn, kk * 128), 1u);
+            for (int kk = 1; kk < 8; ++kk) wgmma_ss<DQ0, 1, 1>(dqa0, desc_adv(dsdesc, kk * 128), desc_adv(kdesc_mn, kk * 128), 1u);
+        } else if constexpr (DQ1 > 0) {
+            wgmma_ss<DQ1, 1, 1>(dqa1, dsdesc, kdesc_mn, 0u);
+#pragma unroll
+            for (int kk = 1; kk < 8; ++kk) wgmma_ss<DQ1, 1, 1>(dqa1, desc_adv(dsdesc, kk * 128), desc_adv(kdesc_mn, kk * 128), 1u);
         }
         wgmma_commit();
         wgmma_wait<0>();
         wgmma_fence_acc(dv);
         wgmma_fence_acc(dk);
-        wgmma_fence_acc(dqa);
+        wgmma_fence_acc(dqa0);
+        wgmma_fence_acc(dqa1);
         asm volatile("bar.sync 1, 256;" ::: "memory");   // stage st and the dS^T tiles are no longer read by either warpgroup
         if (threadIdx.x == 0 && i + STAGES < i1) load_q(i + STAGES);
         if (!dq_cols) continue;
-        // ---- dQ of the CTA's kv rows, this warpgroup's 32 columns -> fp32 accumulator [B,H,dq_ld/4,Lq,4]
+        // ---- dQ of the CTA's kv rows, this warpgroup's columns -> fp32 accumulator [B,H,dq_ld/4,Lq,4]
+        auto reduce_dq = [&](const auto& dqa) {
+            constexpr int N = 2 * sizeof(dqa) / sizeof(float);
 #pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-            const int q = i * 64 + r0 + 8 * hh;
-            if (q >= p.Lq) continue;
+            for (int hh = 0; hh < 2; ++hh) {
+                const int q = i * 64 + r0 + 8 * hh;
+                if (q >= p.Lq) continue;
 #pragma unroll
-            for (int c8 = 0; c8 < 4; ++c8) {
-                const int col = dq_col + 8 * c8 + cq;
-                if (col < p.d) red_add_v2(p.dq_acc + ((bh * (p.dq_ld / 4) + col / 4) * p.Lq + q) * 4 + (col & 3), dqa[4 * c8 + 2 * hh], dqa[4 * c8 + 2 * hh + 1]);
+                for (int c8 = 0; c8 < N / 8; ++c8) {
+                    const int col = dq_col + 8 * c8 + cq;
+                    red_add_v2(p.dq_acc + ((bh * (p.dq_ld / 4) + col / 4) * p.Lq + q) * 4 + (col & 3), dqa[4 * c8 + 2 * hh], dqa[4 * c8 + 2 * hh + 1]);
+                }
             }
-        }
+        };
+        if (wg == 0) reduce_dq(dqa0);
+        else reduce_dq(dqa1);
     }
     // ---- dK / dV of this warpgroup's kv rows
 #pragma unroll
@@ -429,9 +444,8 @@ __global__ void __launch_bounds__(kAttnBwdThreads, 1) attn_bwd_kernel(const __gr
         if (!kv_ok[hh]) continue;
         const int kv = kvw + r0 + 8 * hh;
 #pragma unroll
-        for (int c8 = 0; c8 < 8; ++c8) {
+        for (int c8 = 0; c8 < W / 8; ++c8) {
             const int col = p.col0 + 8 * c8 + cq;
-            if (col >= p.d) continue;
             const float v0 = dv[4 * c8 + 2 * hh], v1 = dv[4 * c8 + 2 * hh + 1];
             const float k0 = dk[4 * c8 + 2 * hh], k1 = dk[4 * c8 + 2 * hh + 1];
             if (p.dkv_acc) {
@@ -572,19 +586,34 @@ static int launch_attn_fwd(const AttnFwdParams& p, dim3 grid, cudaStream_t strea
     return HCP_OK;
 }
 
-template <int NB, bool kCausal>
+template <int NB, int W, bool kCausal>
 static int launch_attn_bwd(const AttnBwdParams& p, dim3 grid, cudaStream_t stream) {
     using Cfg = AttnBwdCfg<NB>;
     static bool configured = false;
     if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(attn_bwd_kernel<NB, kCausal>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
+        cudaError_t e = cudaFuncSetAttribute(attn_bwd_kernel<NB, W, kCausal>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
         if (e != cudaSuccess) return set_cuda_error(e, "cudaFuncSetAttribute(attn_bwd)");
         configured = true;
     }
-    launch_k(attn_bwd_kernel<NB, kCausal>, grid, dim3(kAttnBwdThreads), Cfg::SMEM_BYTES, stream, p);
+    launch_k(attn_bwd_kernel<NB, W, kCausal>, grid, dim3(kAttnBwdThreads), Cfg::SMEM_BYTES, stream, p);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return set_cuda_error(e, "attn_bwd launch");
     return HCP_OK;
+}
+
+// one output column slice [col0, col0 + w), w = min(64, d - col0)
+template <int NB, bool kCausal>
+static int launch_attn_bwd_slice(const AttnBwdParams& p, int w, dim3 grid, cudaStream_t stream) {
+    switch (w) {
+    case 8: return launch_attn_bwd<NB, 8, kCausal>(p, grid, stream);
+    case 16: return launch_attn_bwd<NB, 16, kCausal>(p, grid, stream);
+    case 24: return launch_attn_bwd<NB, 24, kCausal>(p, grid, stream);
+    case 32: return launch_attn_bwd<NB, 32, kCausal>(p, grid, stream);
+    case 40: return launch_attn_bwd<NB, 40, kCausal>(p, grid, stream);
+    case 48: return launch_attn_bwd<NB, 48, kCausal>(p, grid, stream);
+    case 56: return launch_attn_bwd<NB, 56, kCausal>(p, grid, stream);
+    default: return launch_attn_bwd<NB, 64, kCausal>(p, grid, stream);
+    }
 }
 
 }  // namespace hcp
@@ -690,8 +719,9 @@ static int attn_bwd(const hcp_attn_bwd_args* a, hcp_stream_t stream_) {
     // output column slices of 64 (one box): dK / dV / dQ accumulators of a slice stay in registers; S and dP are recomputed per slice
     for (int col0 = 0; col0 < a->d; col0 += 64) {
         p.col0 = col0;
-        rc = nb == 1 ? launch_attn_bwd<1, kCausal>(p, grid, stream) : nb == 2 ? launch_attn_bwd<2, kCausal>(p, grid, stream)
-                     : launch_attn_bwd<3, kCausal>(p, grid, stream);
+        const int w = a->d - col0 < 64 ? (int)(a->d - col0) : 64;
+        rc = nb == 1 ? launch_attn_bwd_slice<1, kCausal>(p, w, grid, stream) : nb == 2 ? launch_attn_bwd_slice<2, kCausal>(p, w, grid, stream)
+                     : launch_attn_bwd_slice<3, kCausal>(p, w, grid, stream);
         if (rc) return rc;
     }
     {
