@@ -34,6 +34,18 @@ The normalisation, weight-gradient and time-embedding kernels (tests/test_gpu_no
           small time-embedding linears, the boundary convolutions' fp32 outputs
   F32SIN  the skinny linear on sinusoidal embeddings    6.05e-6 / 6.83e-6 / 1.01e-5              2e-5 / 2e-5 / 3e-5
           of timesteps up to 999 (fp32 argument t * freq)
+
+The Conv2d LoRA (LoCon) and DreamArtist++ convolution path (tests/test_gpu_lora_conv_edges.py, same H100):
+
+  FWD     the convolution with its LoRA K-segment       1.67e-3 / 1.69e-3 / 3.27e-3
+  F32SUM  dW_down (nine shifted-box launches), dW_up,   3.66e-7 / 3.88e-7 / 5.31e-7
+          d_rowbias
+  LORA    factor gradients end to end (U / T rounded    2.64e-3 / 2.92e-3 / 3.71e-3
+          to bf16), against the fp32 masters
+  LOCON   y and dX end to end against the fp32 masters  3.06e-3 / 3.10e-3 / 5.21e-3              8e-3 / 8e-3 / 1.2e-2
+          (T / U and the factors rounded to bf16 before
+          their MMAs), and dX = dgrad(dY, W) accumulated
+          in place with dgrad(U, W_down) (two roundings)
 """
 from dataclasses import dataclass
 
@@ -57,6 +69,7 @@ NORM = Tol(rel=4e-3, block=6e-3, maxabs=9e-3)
 STAT = 1.5e-6
 F32SUM = Tol(rel=1.5e-6, block=1.5e-6, maxabs=2e-6)
 F32SIN = Tol(rel=2e-5, block=2e-5, maxabs=3e-5)
+LOCON = Tol(rel=8e-3, block=8e-3, maxabs=1.2e-2)
 
 
 def compare(name: str, got: torch.Tensor, ref: torch.Tensor, tol: Tol, block=(128, 128)) -> None:

@@ -14,6 +14,7 @@ import torch
 import torch.nn.functional as F
 
 from kernel_check import FWD, GRAD, LORA, LSE_ABS, Canary, compare
+from lora_conv_plan import tile_n
 
 pytestmark = pytest.mark.gpu
 
@@ -60,13 +61,6 @@ def run_gemm(x, w, bias, rb, res, rows_per_group, out):
     N = w.shape[0]
     ops.gemm_raw([(x, K, K)], [(w, K, N, 0)], M, N, out.view, out.ld, bias=bias, rowbias=rb, rows_per_group=rows_per_group,
                  residual=res, ldr=res.stride(0))
-
-
-def tile_n(N):
-    """Column-tile width BN the GEMM / convolution kernel picks for N output columns (pick_bn in gemm.cu): the error blocks."""
-    if N <= 64 or (N % 64 == 0 and N < 256 and N % 128):
-        return 32 if N <= 32 else 64
-    return min((128, 160, 176), key=lambda c: ((N + c - 1) // c * c, -c))
 
 
 # A ragged last column tile in every BN instantiation (N 8 and 24: BN 32; 40 and 192: 64; 200: 128; 336: 176, the 320 + 16
