@@ -153,7 +153,7 @@ EXPORTS = [
     "hcp_wgrad_bf16", "hcp_wgrad_conv3x3_bf16", "hcp_colsum_bf16", "hcp_norm_affine_grad_bf16", "hcp_small_linear_bwd_f32", "hcp_silu_f32",
     "hcp_conv_in_wgrad_f32", "hcp_conv_out_wgrad_f32", "hcp_repack_weights", "hcp_adafactor_flat",
     "hcp_attn_fwd_causal_bf16", "hcp_attn_bwd_causal_bf16", "hcp_quick_gelu_fwd_bf16", "hcp_quick_gelu_bwd_bf16", "hcp_embed_gather_bf16",
-    "hcp_sum_bf16_to_f32",
+    "hcp_sum_bf16_to_f32", "hcp_gelu_fwd_bf16", "hcp_gelu_bwd_bf16",
 ]
 
 
@@ -192,6 +192,8 @@ def lib() -> C.CDLL:
             l.hcp_geglu_bwd_bf16.argtypes = [vp, vp, i64, i64, vp, vp]
             l.hcp_quick_gelu_fwd_bf16.argtypes = [vp, i64, i64, vp, vp]
             l.hcp_quick_gelu_bwd_bf16.argtypes = [vp, vp, i64, i64, vp, vp]
+            l.hcp_gelu_fwd_bf16.argtypes = [vp, i64, i64, vp, vp]
+            l.hcp_gelu_bwd_bf16.argtypes = [vp, vp, i64, i64, vp, vp]
             l.hcp_sum_bf16_to_f32.argtypes = [C.POINTER(C.c_void_p), i64, i64, vp, vp]
             l.hcp_embed_gather_bf16.argtypes = [vp, vp, vp, i64, vp, i64, i64, i64, i64, vp, vp]
             l.hcp_upsample2x_fwd_bf16.argtypes = [vp, i64, i64, i64, i64, vp, vp]

@@ -967,6 +967,42 @@ __global__ void quick_gelu_bwd_kernel(const __nv_bfloat16* __restrict__ x, const
 }
 
 // =============================================================================================
+// exact GELU (OpenCLIP-bigG MLP, transformers hidden_act='gelu'): y = 0.5 x (1 + erf(x / sqrt 2));
+// dx = dy * (Phi(x) + x phi(x))  -- gelu_f / gelu_grad, the same functions GEGLU uses
+// =============================================================================================
+__global__ void gelu_fwd_kernel(const __nv_bfloat16* __restrict__ x, int64_t n8, __nv_bfloat16* __restrict__ y) {
+    pdl_trigger();
+    pdl_wait();
+    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;   // one thread per 8 elements
+    if (i >= n8) return;
+    const uint4 ux = reinterpret_cast<const uint4*>(x)[i];
+    const uint32_t xx[4] = {ux.x, ux.y, ux.z, ux.w};
+    uint32_t o[4];
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+        const float2 v = unpack_bf16x2(xx[e]);
+        o[e] = pack_bf16x2(gelu_f(v.x), gelu_f(v.y));
+    }
+    reinterpret_cast<uint4*>(y)[i] = make_uint4(o[0], o[1], o[2], o[3]);
+}
+__global__ void gelu_bwd_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ dy, int64_t n8,
+                                __nv_bfloat16* __restrict__ dx) {
+    pdl_trigger();
+    pdl_wait();
+    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (i >= n8) return;
+    const uint4 ux = reinterpret_cast<const uint4*>(x)[i], ud = reinterpret_cast<const uint4*>(dy)[i];
+    const uint32_t xx[4] = {ux.x, ux.y, ux.z, ux.w}, dd[4] = {ud.x, ud.y, ud.z, ud.w};
+    uint32_t o[4];
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+        const float2 v = unpack_bf16x2(xx[e]), d = unpack_bf16x2(dd[e]);
+        o[e] = pack_bf16x2(d.x * gelu_grad(v.x), d.y * gelu_grad(v.y));
+    }
+    reinterpret_cast<uint4*>(dx)[i] = make_uint4(o[0], o[1], o[2], o[3]);
+}
+
+// =============================================================================================
 // fp32 sum of up to kSumSrcs bf16 arrays, in source order: the fan-in of the text embedding's gradient over the cross-attentions
 // =============================================================================================
 constexpr int kSumSrcs = 32;
@@ -1221,6 +1257,24 @@ extern "C" int hcp_quick_gelu_bwd_bf16(const void* x, const void* dy, int64_t M,
     launch_k(quick_gelu_bwd_kernel, dim3((unsigned)((n8 + 255) / 256)), dim3(256), 0, (cudaStream_t)stream_, (const __nv_bfloat16*)x,
              (const __nv_bfloat16*)dy, n8, (__nv_bfloat16*)dx);
     LAUNCH_CHECK("quick_gelu_bwd launch");
+    return HCP_OK;
+}
+extern "C" int hcp_gelu_fwd_bf16(const void* x, int64_t M, int64_t F, void* y, hcp_stream_t stream_) {
+    if (!x || !y || M < 0 || F % 8 != 0) return set_error(HCP_ERR_INVALID, "gelu_fwd");
+    const int64_t n8 = M * (F / 8);
+    if (n8 == 0) return HCP_OK;
+    launch_k(gelu_fwd_kernel, dim3((unsigned)((n8 + 255) / 256)), dim3(256), 0, (cudaStream_t)stream_, (const __nv_bfloat16*)x, n8,
+             (__nv_bfloat16*)y);
+    LAUNCH_CHECK("gelu_fwd launch");
+    return HCP_OK;
+}
+extern "C" int hcp_gelu_bwd_bf16(const void* x, const void* dy, int64_t M, int64_t F, void* dx, hcp_stream_t stream_) {
+    if (!x || !dy || !dx || M < 0 || F % 8 != 0) return set_error(HCP_ERR_INVALID, "gelu_bwd");
+    const int64_t n8 = M * (F / 8);
+    if (n8 == 0) return HCP_OK;
+    launch_k(gelu_bwd_kernel, dim3((unsigned)((n8 + 255) / 256)), dim3(256), 0, (cudaStream_t)stream_, (const __nv_bfloat16*)x,
+             (const __nv_bfloat16*)dy, n8, (__nv_bfloat16*)dx);
+    LAUNCH_CHECK("gelu_bwd launch");
     return HCP_OK;
 }
 extern "C" int hcp_sum_bf16_to_f32(const void* const* srcs, int64_t nsrc, int64_t n, float* out, hcp_stream_t stream_) {

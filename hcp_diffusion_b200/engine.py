@@ -26,7 +26,7 @@ from torch import nn
 
 from . import _lib, adafactor, ops
 from ._lib import call, stream_ptr
-from .models.clip import encode_prompt
+from .models.clip import SDXLTextEncoder, encode_prompt, encode_prompt_sdxl
 
 SNR_LOSS_MODES = {"min_snr": 0, "soft_min_snr": 1, "kdiff_min_snr": 2, "edm": 3,
                   "MinSNRLoss": 0, "SoftMinSNRLoss": 1, "KDiffMinSNRLoss": 2, "EDMLoss": 3}
@@ -182,7 +182,9 @@ class LoraTrainStep:
     `TEUnetWrapper`); its adapter parameters must be among `params` (their own groups), so they share the flat buffer: one all-reduce,
     one global-norm clip over both models, the same optimizer and EMA.  `step()` then takes int64 token ids [B, 77 R] in place of the
     text embedding, and the text encoder runs forward and backward inside the same graph.  `text_encoder_opts`: {'n_repeats',
-    'clip_skip', 'clip_final_norm'} of `models.encode_prompt`."""
+    'clip_skip', 'clip_final_norm'} of `models.encode_prompt`.  With an SDXL (text_time) UNet the text encoder is a
+    `models.SDXLTextEncoder` (SDXLTEUnetWrapper): `step()` takes ids [B, 2 x 77] and `added_cond_kwargs={'time_ids'}`, and
+    `text_embeds` is the encoder's projected pooled row (`models.encode_prompt_sdxl`; n_repeats 1)."""
 
     def __init__(self, unet: nn.Module, params: Union[Iterable[nn.Parameter], Sequence[dict]], lr: float = 1e-4, betas=(0.9, 0.999),
                  eps: float = 1e-8, weight_decay: float = 1e-2, max_grad_norm: float = 1.0, use_cuda_graph: bool = True,
@@ -191,18 +193,25 @@ class LoraTrainStep:
                  optimizer: str = "adamw", optimizer_kwargs: Optional[dict] = None, text_encoder: Optional[nn.Module] = None,
                  text_encoder_opts: Optional[dict] = None):
         self.unet = unet
-        self.te, self.te_opts = text_encoder, None
+        self.te, self.te_opts, self.sdxl = text_encoder, None, False
         if text_encoder is not None:
             if cfg_scale is not None:
                 raise NotImplementedError("cfg_scale (DreamArtist batch doubling) together with a trained text encoder is not supported")
-            if getattr(getattr(unet, "config", None), "addition_embed_type", None) == "text_time":
-                raise NotImplementedError("an SDXL (text_time) UNet together with a trained text encoder is not supported")
             opts = dict(text_encoder_opts or {})
             unknown = set(opts) - {"n_repeats", "clip_skip", "clip_final_norm"}
             if unknown:
                 raise ValueError(f"text_encoder_opts: unknown keys {sorted(unknown)}")
             self.te_opts = {"n_repeats": int(opts.get("n_repeats", 1)), "clip_skip": int(opts.get("clip_skip", 0)),
                             "clip_final_norm": bool(opts.get("clip_final_norm", True))}
+            self.sdxl = getattr(getattr(unet, "config", None), "addition_embed_type", None) == "text_time"
+            if self.sdxl != isinstance(text_encoder, SDXLTextEncoder):
+                raise NotImplementedError("an SDXL (text_time) UNet trains with an SDXLTextEncoder (its pooled bigG projection is "
+                                          "text_embeds), and an SDXLTextEncoder needs an SDXL UNet")
+            if self.sdxl and self.te_opts["n_repeats"] != 1:
+                raise NotImplementedError(
+                    "SDXL with n_repeats > 1 (tokenizer_repeats) is not supported: the reference pools bigG's text_embeds at the "
+                    "largest id of the raw tokenizer output before it is cut into 77-token chunks, which pre-chunked ids cannot "
+                    "express (the reference's SDXL config uses tokenizer_repeats: 1)")
         if optimizer not in ("adamw", "adafactor"):
             raise ValueError(f"optimizer {optimizer!r}: one of 'adamw', 'adafactor'")
         self.optimizer = optimizer
@@ -376,7 +385,10 @@ class LoraTrainStep:
         x_in, t_in = x_t, t
         if self.cfg_ctx is not None:                       # DreamArtistPTContext.pre: 'b c h w -> (pn b) c h w', timesteps.repeat(2)
             x_in, t_in = torch.cat([x_t, x_t], 0), torch.cat([t, t], 0)
-        if self.te is not None:                            # TEUnetWrapper.forward: ehs = TE(ids) with its adapters in the graph
+        if self.sdxl:                                      # SDXLTEUnetWrapper.forward: text_embeds = bigG's projected pooled row
+            ehs, text_embeds = encode_prompt_sdxl(self.te, ehs, self.te_opts["clip_skip"], self.te_opts["clip_final_norm"])
+            added = {**added, "text_embeds": text_embeds}
+        elif self.te is not None:                          # TEUnetWrapper.forward: ehs = TE(ids) with its adapters in the graph
             ehs = encode_prompt(self.te, ehs, **self.te_opts)
         pred = (self.unet(x_in, t_in, ehs, added_cond_kwargs=added) if added is not None else self.unet(x_in, t_in, ehs)).sample
         if self.cfg_ctx is not None:
@@ -431,9 +443,15 @@ class LoraTrainStep:
              added_cond_kwargs: Optional[Dict[str, torch.Tensor]] = None) -> torch.Tensor:
         """One micro-step: latents/noise fp32 [B,4,H,W], t int64 [B], ehs fp32 [B,L,ctx] ([2B,L,ctx] = [negative | positive] with
         `cfg_scale`), or int64 token ids [B, 77 R] with a `text_encoder` (host-pinned or device); `added_cond_kwargs` ({'text_embeds' [B,P], 'time_ids' [B,6]}) for SDXL UNets
-        (reference wrapper.py:66).  The optimizer runs on every `grad_accum_steps`-th call.  Returns the device loss tensor
+        (reference wrapper.py:66; {'time_ids'} only, with ids [B, 2 x 77], when an SDXLTextEncoder is trained).  The optimizer runs on every `grad_accum_steps`-th call.  Returns the device loss tensor
         (shape [1]) of this micro-batch; reading it is the caller's D2H."""
         dev = self.flat.data.device
+        if self.sdxl:
+            if not added_cond_kwargs or "time_ids" not in added_cond_kwargs:
+                raise ValueError("an SDXL UNet with a text encoder needs added_cond_kwargs={'time_ids': [B, 6]}")
+            if "text_embeds" in added_cond_kwargs:
+                raise ValueError("text_embeds is computed by the trained SDXL text encoder (bigG's projected pooled row): pass "
+                                 "added_cond_kwargs={'time_ids'} only")
         if not self.use_graph:
             added = None if added_cond_kwargs is None else {k: v.to(dev, non_blocking=True) for k, v in added_cond_kwargs.items()}
             self._forward_backward(latents.to(dev, non_blocking=True), noise.to(dev, non_blocking=True), t.to(dev, non_blocking=True),

@@ -517,7 +517,10 @@ class UNet2DConditionModel(nn.Module):
                 rt.add = SimpleNamespace(
                     w1=ae.linear_1.weight.detach().to(torch.bfloat16).contiguous(), b1=ae.linear_1.bias.detach().float().contiguous(),
                     w2cat=torch.cat([te.linear_2.weight.detach(), ae.linear_2.weight.detach()], 1).to(torch.bfloat16).contiguous(),
-                    b2sum=(te.linear_2.bias.detach() + ae.linear_2.bias.detach()).float().contiguous())
+                    b2sum=(te.linear_2.bias.detach() + ae.linear_2.bias.detach()).float().contiguous(),
+                    # the unfused operands, for a text_embeds that carries a gradient (a trained text encoder in front)
+                    w2=ae.linear_2.weight.detach().to(torch.bfloat16).contiguous(), b2=ae.linear_2.bias.detach().float().contiguous(),
+                    l1=None, l2=None)
             rt.wp = torch.cat([self._temb_host(r).weight.detach() for r in resnets], 0).to(torch.bfloat16).contiguous()
             rt.bp = torch.cat([self._temb_host(r).bias.detach() for r in resnets], 0).float().contiguous()
             offs, o = [], 0
@@ -615,7 +618,11 @@ class UNet2DConditionModel(nn.Module):
         if t.dim() == 0:
             t = t[None]
         t = t.expand(B).to(torch.float32).contiguous()
-        if rt.add_unfused:
+        # d(text_embeds) wanted (SDXL with a trained text encoder, whose pooled projection is text_embeds): the unfused path, whose
+        # add_embedding.linear_1 node produces dx; a frozen add_embedding stays frozen
+        te_grad = rt.add is not None and added["text_embeds"].requires_grad and torch.is_grad_enabled()
+        unfused = rt.add_unfused or te_grad
+        if unfused:
             x0 = torch.empty((B, self.time_proj.num_channels), dtype=torch.float32, device=dev)
             ops.sinusoid(t, self.time_proj.num_channels, 1, x0, 0)
             lists = rt.train_lists if rt.train_time else None
@@ -635,7 +642,7 @@ class UNet2DConditionModel(nn.Module):
             e1 = ops.skinny_linear(t, rt.w1, rt.b1, 2, True)
             a1 = ops.skinny_linear(self._add_input(added, B, dev), rt.add.w1, rt.add.b1, 0, True)  # silu(add_embedding.linear_1(.))
             emb = ops.skinny_linear(torch.cat([e1, a1], 1), rt.add.w2cat, rt.add.b2sum, 0, True)   # silu(linear_2(e1) + add.linear_2(a1))
-        if rt.train_time or rt.add_unfused:
+        if rt.train_time or unfused:
             # an autograd node whenever emb carries a gradient: the trained add_embedding needs dL/demb even when every
             # time_emb_proj is frozen
             temb_all = ops.small_linear(emb, rt.wp, rt.bp, False, rt.train_lists.proj if rt.train_time else None)

@@ -1090,6 +1090,28 @@ class QuickGeluFn(torch.autograd.Function):
         return dx
 
 
+class GeluFn(torch.autograd.Function):
+    """y = 0.5 x (1 + erf(x / sqrt 2)) (exact GELU, the OpenCLIP-bigG MLP activation), bf16 [..., F]."""
+
+    @staticmethod
+    def forward(ctx, x):
+        x = _chk(x, "gelu input")
+        F_ = x.shape[-1]
+        y = torch.empty_like(x)
+        call("hcp_gelu_fwd_bf16", x.data_ptr(), x.numel() // F_, F_, y.data_ptr(), stream_ptr())
+        ctx.save_for_backward(x)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        (x,) = ctx.saved_tensors
+        dy = _chk(dy, "gelu grad")
+        F_ = x.shape[-1]
+        dx = torch.empty_like(x)
+        call("hcp_gelu_bwd_bf16", x.data_ptr(), dy.data_ptr(), x.numel() // F_, F_, dx.data_ptr(), stream_ptr())
+        return dx
+
+
 def embed_tokens(ids: torch.Tensor, tok_emb: torch.Tensor, pos_emb: torch.Tensor, pos_ids: Optional[torch.Tensor] = None) -> torch.Tensor:
     """bf16 [B, L, C] = tok_emb[ids] + pos_emb[pos_ids or arange(L)] (fp32 tables, int64 ids on the device; ids outside the tables
     are clamped to the nearest row, see hcp_embed_gather_bf16).  No gradient: the embedding tables are frozen."""

@@ -15,7 +15,10 @@ Text encoder (SD1.x CLIP): `lora_text_encoder` items train LoRA on it next to th
 `model.clip_final_norm`, `model.tokenizer_repeats`; `ckpts/text_encoder-<step>` is saved next to `unet-<step>` and
 `resume.ckpt_path.TE` is loaded.  A `text_encoder:` full fine-tune list, a non-null `tokenizer_pt.train` and DreamArtist++ items in
 `lora_text_encoder` raise NotImplementedError.  The ids are given (no tokenizer): `data.path` holds 'input_ids' [N, 77 R], or
-synthetic prompts are BOS 49406, random tokens, EOS 49407 padding.
+synthetic prompts are BOS 49406, random tokens, EOS 49407 padding.  With an SDXL ('text_time') UNet the default text encoder is
+SDXL's pair (`models.SDXLTextEncoder`, CLIP-L + OpenCLIP-bigG, reference cfgs/train/examples/lora_sdxl.yaml): ids are [N, 2 x 77]
+(clip_B's chunk, then bigG's; synthetic bigG chunks carry the same words and are padded with id 0 after EOS, as SDXL's second
+tokenizer pads), `text_embeds` comes from the encoder and the data holds only 'time_ids'.
 
 Out of the hot path and therefore NOT here: datasets / buckets / captions, a tokenizer, VAE, loggers, DeepSpeed /
 Colossal-AI trainers.  Inputs are the synthetic latents / text embeddings of SURVEY.md 8d (`data.synthetic`), or tensors saved
@@ -217,9 +220,13 @@ class Trainer:
         for item in items:
             if str(item.get("type", "lora")) != "lora":
                 raise NotImplementedError(f"lora_text_encoder item type {item.get('type')!r} (DreamArtist++ adapters) is not supported")
-        from .models import CLIPTextModel
+        from .models import CLIPTextModel, SDXLTextEncoder
         te = cfgs.model.get("text_encoder")
-        te = instantiate(te) if isinstance(te, dict) else (te if te is not None else CLIPTextModel())
+        if isinstance(te, dict):
+            te = instantiate(te)
+        elif te is None:                         # the UNet's family decides: SDXL's CLIP-L + OpenCLIP-bigG pair, else CLIP-L
+            sdxl = getattr(self.unet.config, "addition_embed_type", None) == "text_time"
+            te = SDXLTextEncoder() if sdxl else CLIPTextModel()
         init = cfgs.model.get("text_encoder_init")
         if init and init != "random":
             sd = auto_manager(init).load_ckpt(init)
@@ -241,7 +248,9 @@ class Trainer:
             self.ehs = blob["input_ids"].long() if self.te is not None else blob["encoder_hidden_states"].float()
             self.ehs_neg = blob.get("negative_hidden_states")
             if self.text_time:
-                self.text_embeds, self.time_ids = blob["text_embeds"].float(), blob["time_ids"].float()
+                self.time_ids = blob["time_ids"].float()
+                if self.te is None:                              # with a text encoder, text_embeds is its pooled projection
+                    self.text_embeds = blob["text_embeds"].float()
         else:
             n = int(d.get("num_samples", 64))
             s = int(self.unet.config.sample_size)
@@ -258,10 +267,15 @@ class Trainer:
                 keep = torch.arange(75)[None] < lens[:, None]
                 ids[:, 1:76] = torch.where(keep, words, ids[:, 1:76])
                 self.ehs = ids.reshape(n, 77 * R)
+                if self.step_fn.sdxl:                            # the same words for bigG, whose tokenizer pads with id 0 after EOS
+                    ids_g = ids.clone()
+                    ids_g[:, 1:] = torch.where(torch.arange(1, 77)[None] <= lens[:, None] + 1, ids[:, 1:], 0)
+                    self.ehs = torch.cat([ids, ids_g], 1)
             if self.text_time:                                   # pooled text embedding ~ N(0,1); (H, W, 0, 0, H, W) in pixels
                 n_ids = 6
-                self.text_embeds = torch.randn((n, cfg.projection_class_embeddings_input_dim - n_ids * cfg.addition_time_embed_dim),
-                                               generator=gd)
+                if self.te is None:
+                    self.text_embeds = torch.randn((n, cfg.projection_class_embeddings_input_dim - n_ids * cfg.addition_time_embed_dim),
+                                                   generator=gd)
                 px = float(s * 8)
                 self.time_ids = torch.tensor([[px, px, 0.0, 0.0, px, px]]).repeat(n, 1)
         self.gen = g
@@ -276,7 +290,10 @@ class Trainer:
         t = torch.randint(0, 1000, (self.bs,), generator=self.gen, dtype=torch.int64)
         batch = [x.pin_memory() for x in (lat, noise, t, ehs)]
         if self.text_time:
-            batch.append({"text_embeds": self.text_embeds[idx].pin_memory(), "time_ids": self.time_ids[idx].pin_memory()})
+            added = {"time_ids": self.time_ids[idx].pin_memory()}
+            if self.text_embeds is not None:
+                added["text_embeds"] = self.text_embeds[idx].pin_memory()
+            batch.append(added)
         return batch
 
     def save(self, step: int):

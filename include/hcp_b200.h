@@ -218,6 +218,12 @@ int hcp_geglu_bwd_bf16(const void* u, const void* dh, int64_t M, int64_t F, void
 int hcp_quick_gelu_fwd_bf16(const void* x, int64_t M, int64_t F, void* y, hcp_stream_t stream);
 int hcp_quick_gelu_bwd_bf16(const void* x, const void* dy, int64_t M, int64_t F, void* dx, hcp_stream_t stream);
 
+/* exact GELU (transformers GELUActivation, hidden_act='gelu': the MLP of SDXL's second text encoder, OpenCLIP ViT-bigG/14): x, y, dy,
+ * dx bf16 [M,F], F % 8 == 0;  y = 0.5 x (1 + erf(x / sqrt 2));  dx = dy * (Phi(x) + x phi(x)) from the saved pre-activation x.
+ * fp32 arithmetic. */
+int hcp_gelu_fwd_bf16(const void* x, int64_t M, int64_t F, void* y, hcp_stream_t stream);
+int hcp_gelu_bwd_bf16(const void* x, const void* dy, int64_t M, int64_t F, void* dx, hcp_stream_t stream);
+
 /* out fp32 [n] = srcs[0] + srcs[1] + ... + srcs[nsrc-1] (bf16 [n] each, n % 8 == 0), summed in fp32 in source order.
  * Replaces: autograd's fp32 accumulation of the gradient of the fp32 text embedding, which the reference casts to bf16 separately for
  *           every cross-attention under autocast (attn2.to_k / to_v, reference cfgs/unet_struct.txt:35-38; TEUnetWrapper.forward,
