@@ -409,154 +409,6 @@ static int plan_splits(int64_t ctas, int64_t total_kb, int64_t N) {
     return s < 2 ? 1 : (int)s;
 }
 
-// =============================================================================================
-// LoRA gradients on the tensor pipe:  D[n, j] = sum_m X[m, n] * S[m, j]   (reduction over the M token rows)
-//   dW_down[j, k] = sum_m U[m, c0+j] x[m, k]          S = U = dY . (alpha B),  X = x
-//   dW_up[o, j]   = alpha * sum_m dY[m, o0+o] T[m, c0+j]   S = T = x . A^T,        X = dY
-// Both operands are read straight from their row-major [M, *] tensors as MN-major wgmma operands (TMA boxes of 64 columns x
-// 128 rows), so no transpose ever exists.  One CTA owns 128 columns of X and a slice of the rows (split-K); MMA warpgroup g
-// accumulates the 64 x 64 fp32 block of X columns [64g, 64g+64) and reduces it into the flat gradient buffer with atomics.
-// =============================================================================================
-constexpr int kLgThreads = 288;   // warps 0-7: two MMA warpgroups, warp 8: TMA
-constexpr int LG_STAGES = 3;
-constexpr int LG_STAGE_BYTES = 3 * 128 * 128;      // two X boxes + one S box
-constexpr int LG_SMEM_BYTES = LG_STAGES * LG_STAGE_BYTES + 256 + 1024;
-constexpr int LG_MAX_BLOCKS = 8;
-
-struct LGBlock {
-    int32_t n_lo, n_hi, c0, rank, transpose_out, dst_ld;
-    int32_t n_stride;        // element stride of the X-column index in the destination (1; 9 for the taps of a 3x3 W_down)
-    float scale;
-    float* dst;
-};
-// X operand = shifted im2col box of a 3x3 convolution (dW_down of a Conv2d LoRA): same boxes as the forward conv's A operand
-struct LGConv {
-    int32_t rank;            // 0: plain [M, ldx] matrix; 4 / 5: rank of the NHWC tensor map
-    int32_t bw, bh, bn, tiles_w, tiles_h;
-    int32_t c0_off, dw, dh, c2;
-};
-struct LGProblem {
-    int32_t n_begin, n_end, tiles_per_cta, nblocks, col_chunks, splits;
-    LGBlock blk[LG_MAX_BLOCKS];
-};
-struct alignas(64) LoraGradParams {
-    CUtensorMap tmX[2], tmS[2];        // up to two independent problems per launch (dW_down and dW_up of one group)
-    int32_t M, nprob;
-    LGProblem prob[2];
-    LGConv conv;
-};
-
-__global__ void __launch_bounds__(kLgThreads, 1) lora_grad_tc_kernel(const __grid_constant__ LoraGradParams p) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + LG_STAGES * LG_STAGE_BYTES);
-    uint64_t* empty_bar = full_bar + LG_STAGES;
-    const int warp = warp_id_uniform(), lane = threadIdx.x & 31;
-    // flat grid over (problem, column chunk, row split)
-    int bid = blockIdx.x, z = 0;
-    if (p.nprob == 2 && bid >= p.prob[0].col_chunks * p.prob[0].splits) { bid -= p.prob[0].col_chunks * p.prob[0].splits; z = 1; }
-    // The reduction epilogue walks `p.prob[z].blk[b]` with run-time z and b (dynamically indexed constant-bank loads): the MMA
-    // threads copy the descriptor to shared memory first; the producer only needs the scalars read here.
-    __shared__ LGProblem sq;
-    const LGProblem& q = z ? p.prob[1] : p.prob[0];
-    const CUtensorMap* tmX = z ? &p.tmX[1] : &p.tmX[0];
-    const CUtensorMap* tmS = z ? &p.tmS[1] : &p.tmS[0];
-    const int ncol0 = q.n_begin + (bid % q.col_chunks) * 128;
-    const int total_tiles = (p.M + 127) / 128;
-    const int t0 = (bid / q.col_chunks) * q.tiles_per_cta;
-    const int t1 = min(total_tiles, t0 + q.tiles_per_cta);
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < LG_STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 256); }
-        fence_mbar_init();
-    }
-    __syncthreads();
-    pdl_trigger();
-    pdl_wait();
-
-    if (warp == 8) {
-        if (elect_one()) {
-            int stage = 0; uint32_t phase = 0;
-            for (int t = t0; t < t1; ++t) {
-                mbar_wait(&empty_bar[stage], phase ^ 1);
-                mbar_arrive_expect_tx(&full_bar[stage], LG_STAGE_BYTES);
-                uint8_t* base = smem + stage * LG_STAGE_BYTES;
-                if (p.conv.rank == 0) {
-                    tma_load_2d(base, tmX, &full_bar[stage], ncol0, t * 128);
-                    tma_load_2d(base + 128 * 128, tmX, &full_bar[stage], ncol0 + 64, t * 128);
-                } else {
-                    const LGConv& cv = p.conv;
-                    int img0, h0 = 0, w0 = 0;
-                    if (cv.bn == 1) {
-                        const int per_img = cv.tiles_w * cv.tiles_h, r = t % per_img;
-                        img0 = t / per_img;
-                        h0 = (r / cv.tiles_w) * cv.bh;
-                        w0 = (r % cv.tiles_w) * cv.bw;
-                    } else {
-                        img0 = t * cv.bn;
-                    }
-                    for (int hf = 0; hf < 2; ++hf) {
-                        const int c = cv.c0_off + ncol0 + hf * 64;
-                        if (cv.rank == 4) tma_load_4d(base + hf * 128 * 128, tmX, &full_bar[stage], c, w0 + cv.dw, h0 + cv.dh, img0);
-                        else tma_load_5d(base + hf * 128 * 128, tmX, &full_bar[stage], c, w0 + cv.dw, cv.c2, h0 + cv.dh, img0);
-                    }
-                }
-                tma_load_2d(base + 2 * 128 * 128, tmS, &full_bar[stage], 0, t * 128);
-                if (++stage == LG_STAGES) { stage = 0; phase ^= 1; }
-            }
-        }
-        return;
-    }
-    {   // descriptor -> shared memory
-        const uint32_t* src = reinterpret_cast<const uint32_t*>(&q);
-        uint32_t* dst = reinterpret_cast<uint32_t*>(&sq);
-        for (int i = threadIdx.x; i < (int)(sizeof(LGProblem) / 4); i += 256) dst[i] = src[i];
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-    }
-    const int wg = warp >> 2;
-    float acc[32];
-#pragma unroll
-    for (int i = 0; i < 32; ++i) acc[i] = 0.f;
-    int stage = 0; uint32_t phase = 0;
-    for (int t = t0; t < t1; ++t) {
-        mbar_wait(&full_bar[stage], phase);
-        const uint32_t xb = smem_u32(smem + stage * LG_STAGE_BYTES) + wg * 128 * 128;   // this warpgroup's 64 X columns
-        const uint32_t sb = smem_u32(smem + stage * LG_STAGE_BYTES) + 2 * 128 * 128;
-        wgmma_fence();
-#pragma unroll
-        for (int ks = 0; ks < 8; ++ks)                                   // 16 token rows per k-step = 2048 B
-            wgmma_ss<64, 1, 1>(acc, make_smem_desc(xb + ks * 2048, 128 * 128, 1024), make_smem_desc(sb + ks * 2048, 128 * 128, 1024), 1u);
-        wgmma_commit();
-        wgmma_wait<0>();
-        mbar_arrive(&empty_bar[stage]);
-        if (++stage == LG_STAGES) { stage = 0; phase ^= 1; }
-    }
-    wgmma_fence_acc(acc);
-    if (t1 <= t0) return;
-    const LGProblem& qs = sq;
-    const int n_lo_row = ncol0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-        const int n = n_lo_row + 8 * h;                                  // column of X
-        if (n >= qs.n_end) continue;
-        for (int b = 0; b < qs.nblocks; ++b) {
-            const LGBlock& k = qs.blk[b];
-            if (n < k.n_lo || n >= k.n_hi) continue;
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-                const int jj = 8 * (i >> 1) + 2 * (lane & 3) + (i & 1);   // column of S
-                const int j = jj - k.c0;
-                if (j >= 0 && j < k.rank) {
-                    const float val = acc[4 * (i >> 1) + 2 * h + (i & 1)] * k.scale;
-                    float* dst = k.transpose_out ? k.dst + (int64_t)(n - k.n_lo) * k.dst_ld + j
-                                                 : k.dst + (int64_t)j * k.dst_ld + (int64_t)(n - k.n_lo) * k.n_stride;
-                    atomicAdd(dst, val);
-                }
-            }
-        }
-    }
-}
-
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
@@ -736,19 +588,12 @@ extern "C" int hcp_conv3x3_bf16(const hcp_conv3x3_args* a, hcp_stream_t stream_)
         oH = a->Hin * 2; oW = a->Win * 2;
         tH = a->Hin; tW = a->Win;   // one launch per output phase, tiles walk the dY grid
     }
-    // box: bw*bh*bn == 128
-    int bw, bh, bnimg;
-    if (tW >= 128) { bw = 128; bh = 1; bnimg = 1; if (tW % 128) return set_error(HCP_ERR_INVALID, "conv3x3: W"); }
-    else {
-        bw = (int)tW;
-        if (128 % bw) return set_error(HCP_ERR_INVALID, "conv3x3: W must divide 128");
-        bh = 128 / bw;
-        if (bh <= tH) { if (tH % bh) return set_error(HCP_ERR_INVALID, "conv3x3: H tiling"); bnimg = 1; }
-        else { bh = (int)tH; if (128 % (bw * bh)) return set_error(HCP_ERR_INVALID, "conv3x3: H*W must divide 128"); bnimg = 128 / (bw * bh); }
-    }
-    kp.bw = bw; kp.bh = bh; kp.bn = bnimg;
-    kp.tiles_w = (int)(tW / bw);
-    kp.tiles_h = (int)(tH / bh);
+    ConvBox box;
+    int rc = plan_conv_box(tH, tW, "conv3x3", box);
+    if (rc) return rc;
+    kp.bw = box.bw; kp.bh = box.bh; kp.bn = box.bn;
+    kp.tiles_w = box.tiles_w;
+    kp.tiles_h = box.tiles_h;
     kp.oW = (int)oW; kp.oH = (int)oH;
     kp.nseg = 1;
     kp.nkb[0] = (int)(Cin / BLOCK_K);
@@ -765,9 +610,8 @@ extern "C" int hcp_conv3x3_bf16(const hcp_conv3x3_args* a, hcp_stream_t stream_)
     kp.out = (__nv_bfloat16*)a->out;
     kp.ldo = a->Cout;
     kp.n_main = (int)a->Cout;
-    const int m_tiles = (bnimg == 1) ? (int)(a->B * kp.tiles_w * kp.tiles_h) : (int)((a->B + bnimg - 1) / bnimg);
+    const int m_tiles = (box.bn == 1) ? (int)(a->B * kp.tiles_w * kp.tiles_h) : (int)((a->B + box.bn - 1) / box.bn);
     const int b_box_rows = bn;
-    int rc;
     if (a->w_tiled) {          // k-block-major weights [9*Cin/64][Cout][64]
         uint64_t dims[3] = {BLOCK_K, (uint64_t)a->Cout, (uint64_t)(9 * Cin / BLOCK_K)};
         uint64_t strides[2] = {BLOCK_K * 2, (uint64_t)a->Cout * BLOCK_K * 2};
@@ -780,43 +624,14 @@ extern "C" int hcp_conv3x3_bf16(const hcp_conv3x3_args* a, hcp_stream_t stream_)
     if (rc) return rc;
     cudaStream_t stream = (cudaStream_t)stream_;
 
-    if (a->mode == 0 && a->stride == 1) {
-        kp.conv = 4;
-        uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)a->Win, (uint64_t)a->Hin, (uint64_t)a->B};
-        uint64_t strides[3] = {(uint64_t)Cin * 2, (uint64_t)a->Win * Cin * 2, (uint64_t)a->Hin * a->Win * Cin * 2};
-        uint32_t box[4] = {BLOCK_K, (uint32_t)bw, (uint32_t)bh, (uint32_t)bnimg};
-        rc = make_tmap_nd(&kp.tmA[0], a->x, 4, dims, strides, box);
-        if (rc) return rc;
+    if (a->mode == 0) {
+        kp.conv = a->stride == 1 ? 4 : 5;
+        if ((rc = make_tmap_nhwc(&kp.tmA[0], a->x, a->B, a->Hin, a->Win, Cin, a->stride, box))) return rc;
         kp.ntaps = 9;
         for (int kh = 0; kh < 3; ++kh)
             for (int kw = 0; kw < 3; ++kw) {
-                TapEntry& t = kp.taps[kh * 3 + kw];
-                t.c0_off = 0; t.dw = kw - 1; t.dh = kh - 1; t.c2 = 0;
-                t.wk_off = (int)((kh * 3 + kw) * Cin);
-            }
-        kp.sh = kp.sw = 1; kp.oh0 = kp.ow0 = 0;
-        if ((rc = conv_lora_segment(a, kp, b_box_rows))) return rc;
-        return run_gemm(bn, kp, m_tiles, (int64_t)9 * kp.nkb[0] + (kp.nseg > 1 ? kp.nkb[1] : 0), a->workspace, a->workspace_bytes, true, stream);
-    }
-    if (a->mode == 0 && a->stride == 2) {
-        // view x as [B][Hin/2][2][Win/2][2*Cin]: input row ih = 2*oh + kh - 1 -> (phase, index)
-        kp.conv = 5;
-        uint64_t dims[5] = {(uint64_t)(2 * Cin), (uint64_t)(a->Win / 2), 2, (uint64_t)(a->Hin / 2), (uint64_t)a->B};
-        uint64_t strides[4] = {(uint64_t)(2 * Cin) * 2, (uint64_t)a->Win * Cin * 2, (uint64_t)(2 * a->Win * Cin) * 2,
-                               (uint64_t)a->Hin * a->Win * Cin * 2};
-        uint32_t box[5] = {BLOCK_K, (uint32_t)bw, 1, (uint32_t)bh, (uint32_t)bnimg};
-        rc = make_tmap_nd(&kp.tmA[0], a->x, 5, dims, strides, box);
-        if (rc) return rc;
-        kp.ntaps = 9;
-        for (int kh = 0; kh < 3; ++kh)
-            for (int kw = 0; kw < 3; ++kw) {
-                TapEntry& t = kp.taps[kh * 3 + kw];
-                const int pw = (kw == 1) ? 0 : 1, ph = (kh == 1) ? 0 : 1;
-                t.c0_off = (int)(pw * Cin);
-                t.dw = (kw == 0) ? -1 : 0;
-                t.c2 = ph;
-                t.dh = (kh == 0) ? -1 : 0;
-                t.wk_off = (int)((kh * 3 + kw) * Cin);
+                const ConvTap t = conv_tap(kh, kw, a->stride, Cin);
+                kp.taps[kh * 3 + kw] = TapEntry{t.c0_off, t.dw, t.dh, t.c2, (int)((kh * 3 + kw) * Cin)};
             }
         kp.sh = kp.sw = 1; kp.oh0 = kp.ow0 = 0;
         if ((rc = conv_lora_segment(a, kp, b_box_rows))) return rc;
@@ -828,13 +643,7 @@ extern "C" int hcp_conv3x3_bf16(const hcp_conv3x3_args* a, hcp_stream_t stream_)
     // parity matches:  ph=0: kh=1 (dh=0);  ph=1: kh=0 (dh=+1), kh=2 (dh=0).   w[co][kh][kw][ci] here is the
     // dgrad weight = W_fwd[ci][kh][kw][co] (NOT flipped; the tap choice below does the bookkeeping).
     kp.conv = 4;
-    {
-        uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)a->Win, (uint64_t)a->Hin, (uint64_t)a->B};
-        uint64_t strides[3] = {(uint64_t)Cin * 2, (uint64_t)a->Win * Cin * 2, (uint64_t)a->Hin * a->Win * Cin * 2};
-        uint32_t box[4] = {BLOCK_K, (uint32_t)bw, (uint32_t)bh, (uint32_t)bnimg};
-        rc = make_tmap_nd(&kp.tmA[0], a->x, 4, dims, strides, box);
-        if (rc) return rc;
-    }
+    if ((rc = make_tmap_nhwc(&kp.tmA[0], a->x, a->B, a->Hin, a->Win, Cin, 1, box))) return rc;
     kp.sh = kp.sw = 2;
     for (int ph = 0; ph < 2; ++ph)
         for (int pw = 0; pw < 2; ++pw) {
@@ -856,148 +665,4 @@ extern "C" int hcp_conv3x3_bf16(const hcp_conv3x3_args* a, hcp_stream_t stream_)
             if (rc) return rc;
         }
     return HCP_OK;
-}
-
-static int lg_fill(LoraGradParams& p, int z, const void* S, int64_t lds, const void* X, int64_t ldx, int64_t M, int64_t n_begin,
-                   int64_t n_end, const hcp_lora_grad_block* blocks, int32_t nblocks, int target_ctas) {
-    if (!S || !X || !blocks || nblocks < 1 || nblocks > LG_MAX_BLOCKS) return set_error(HCP_ERR_INVALID, "lora_grad: 1..8 blocks per problem");
-    if (n_end <= n_begin || (ldx % 8) != 0 || (n_begin % 8) != 0 || lds < 64 || (lds % 8) != 0) return set_error(HCP_ERR_INVALID, "lora_grad: shape");
-    int rc = make_tmap_2d(&p.tmX[z], X, (uint64_t)ldx, (uint64_t)M, (uint64_t)ldx, 64, 128);
-    if (rc) return rc;
-    rc = make_tmap_2d(&p.tmS[z], S, 64, (uint64_t)M, (uint64_t)lds, 64, 128);     // the 64 columns of S this launch reduces
-    if (rc) return rc;
-    LGProblem& q = p.prob[z];
-    q.n_begin = (int)n_begin; q.n_end = (int)n_end; q.nblocks = nblocks;
-    q.col_chunks = (int)((n_end - n_begin + 127) / 128);
-    const int total_tiles = (int)((M + 127) / 128);
-    int splits = target_ctas / q.col_chunks;     // at most one wave of CTAs over all problems of the launch
-    if (splits < 1) splits = 1;
-    if (splits > total_tiles) splits = total_tiles;
-    q.tiles_per_cta = (total_tiles + splits - 1) / splits;
-    q.splits = (total_tiles + q.tiles_per_cta - 1) / q.tiles_per_cta;
-    for (int i = 0; i < nblocks; ++i) {
-        const hcp_lora_grad_block& k = blocks[i];
-        if (k.rank < 1 || k.c0 < 0 || k.c0 + k.rank > 64 || !k.dst) return set_error(HCP_ERR_INVALID, "lora_grad: block descriptor");
-        q.blk[i].n_lo = (int)k.n_lo; q.blk[i].n_hi = (int)k.n_hi; q.blk[i].c0 = k.c0; q.blk[i].rank = k.rank;
-        q.blk[i].transpose_out = k.transpose_out; q.blk[i].dst_ld = (int)k.dst_ld; q.blk[i].scale = k.scale; q.blk[i].dst = k.dst;
-        q.blk[i].n_stride = 1;
-    }
-    return HCP_OK;
-}
-
-static int lg_launch(LoraGradParams& p, cudaStream_t stream) {
-    static bool configured = false;
-    if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(lora_grad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, LG_SMEM_BYTES);
-        if (e != cudaSuccess) return set_cuda_error(e, "cudaFuncSetAttribute(lora_grad)");
-        configured = true;
-    }
-    int ctas = 0;
-    for (int z = 0; z < p.nprob; ++z) ctas += p.prob[z].col_chunks * p.prob[z].splits;
-    launch_k(lora_grad_tc_kernel, dim3(ctas), dim3(kLgThreads), LG_SMEM_BYTES, stream, p);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_cuda_error(e, "lora_grad launch");
-    return HCP_OK;
-}
-
-extern "C" int hcp_lora_grad(const void* S, int64_t lds, const void* X, int64_t ldx, int64_t M, int64_t n_begin, int64_t n_end,
-                             const hcp_lora_grad_block* blocks, int32_t nblocks, hcp_stream_t stream_) {
-    if (M <= 0) return set_error(HCP_ERR_INVALID, "lora_grad: M");
-    LoraGradParams p;
-    memset(&p, 0, sizeof(p));
-    p.M = (int)M; p.nprob = 1;
-    int rc = lg_fill(p, 0, S, lds, X, ldx, M, n_begin, n_end, blocks, nblocks, num_sms());
-    if (rc) return rc;
-    return lg_launch(p, (cudaStream_t)stream_);
-}
-
-// dW_down of a Conv2d LoRA: nine launches (one per tap) of the gradient kernel with the shifted NHWC box as X operand.
-extern "C" int hcp_lora_grad_conv3x3(const void* S, int64_t lds, const void* x, int64_t B, int64_t Hin, int64_t Win, int64_t Cin,
-                                     int32_t stride, const hcp_lora_grad_block* blocks, int32_t nblocks, hcp_stream_t stream_) {
-    if (!S || !x || !blocks || nblocks < 1 || nblocks > LG_MAX_BLOCKS) return set_error(HCP_ERR_INVALID, "lora_grad_conv: arguments");
-    if (Cin % 64 != 0 || (stride != 1 && stride != 2) || lds < 64 || (lds % 8) != 0) return set_error(HCP_ERR_INVALID, "lora_grad_conv: shape");
-    if (stride == 2 && ((Hin | Win) & 1)) return set_error(HCP_ERR_INVALID, "lora_grad_conv: odd extent with stride 2");
-    const int64_t oH = Hin / stride, oW = Win / stride;
-    int bw, bh, bnimg;                       // same 128-pixel tiles as hcp_conv3x3_bf16 (mode 0)
-    if (oW >= 128) { bw = 128; bh = 1; bnimg = 1; if (oW % 128) return set_error(HCP_ERR_INVALID, "lora_grad_conv: W"); }
-    else {
-        bw = (int)oW;
-        if (128 % bw) return set_error(HCP_ERR_INVALID, "lora_grad_conv: W must divide 128");
-        bh = 128 / bw;
-        if (bh <= oH) { if (oH % bh) return set_error(HCP_ERR_INVALID, "lora_grad_conv: H tiling"); bnimg = 1; }
-        else { bh = (int)oH; if (128 % (bw * bh)) return set_error(HCP_ERR_INVALID, "lora_grad_conv: H*W must divide 128"); bnimg = 128 / (bw * bh); }
-    }
-    LoraGradParams p;
-    memset(&p, 0, sizeof(p));
-    const int64_t M = B * oH * oW;
-    p.M = (int)M; p.nprob = 1;
-    int rc;
-    if (stride == 1) {
-        uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)Win, (uint64_t)Hin, (uint64_t)B};
-        uint64_t strides[3] = {(uint64_t)Cin * 2, (uint64_t)Win * Cin * 2, (uint64_t)Hin * Win * Cin * 2};
-        uint32_t box[4] = {64, (uint32_t)bw, (uint32_t)bh, (uint32_t)bnimg};
-        rc = make_tmap_nd(&p.tmX[0], x, 4, dims, strides, box);
-        p.conv.rank = 4;
-    } else {
-        uint64_t dims[5] = {(uint64_t)(2 * Cin), (uint64_t)(Win / 2), 2, (uint64_t)(Hin / 2), (uint64_t)B};
-        uint64_t strides[4] = {(uint64_t)(2 * Cin) * 2, (uint64_t)Win * Cin * 2, (uint64_t)(2 * Win * Cin) * 2, (uint64_t)Hin * Win * Cin * 2};
-        uint32_t box[5] = {64, (uint32_t)bw, 1, (uint32_t)bh, (uint32_t)bnimg};
-        rc = make_tmap_nd(&p.tmX[0], x, 5, dims, strides, box);
-        p.conv.rank = 5;
-    }
-    if (rc) return rc;
-    rc = make_tmap_2d(&p.tmS[0], S, 64, (uint64_t)M, (uint64_t)lds, 64, 128);
-    if (rc) return rc;
-    p.conv.bw = bw; p.conv.bh = bh; p.conv.bn = bnimg;
-    p.conv.tiles_w = (int)(oW / bw); p.conv.tiles_h = (int)(oH / bh);
-    LGProblem& q = p.prob[0];
-    q.n_begin = 0; q.n_end = (int)Cin; q.nblocks = nblocks;
-    q.col_chunks = (int)((Cin + 127) / 128);
-    const int total_tiles = (int)((M + 127) / 128);
-    int splits = num_sms() / q.col_chunks;
-    if (splits < 1) splits = 1;
-    if (splits > total_tiles) splits = total_tiles;
-    q.tiles_per_cta = (total_tiles + splits - 1) / splits;
-    q.splits = (total_tiles + q.tiles_per_cta - 1) / q.tiles_per_cta;
-    for (int kh = 0; kh < 3; ++kh)
-        for (int kw = 0; kw < 3; ++kw) {
-            if (stride == 1) { p.conv.c0_off = 0; p.conv.dw = kw - 1; p.conv.dh = kh - 1; p.conv.c2 = 0; }
-            else {          // input row 2*oh + kh - 1 -> (phase, index) of the [H/2][2][W/2][2C] view, as in the forward conv
-                p.conv.c0_off = (int)(((kw == 1) ? 0 : 1) * Cin);
-                p.conv.dw = (kw == 0) ? -1 : 0;
-                p.conv.c2 = (kh == 1) ? 0 : 1;
-                p.conv.dh = (kh == 0) ? -1 : 0;
-            }
-            for (int i = 0; i < nblocks; ++i) {
-                const hcp_lora_grad_block& k = blocks[i];
-                if (k.rank < 1 || k.c0 < 0 || k.c0 + k.rank > 64 || !k.dst) return set_error(HCP_ERR_INVALID, "lora_grad_conv: block descriptor");
-                q.blk[i].n_lo = 0; q.blk[i].n_hi = (int)Cin; q.blk[i].c0 = k.c0; q.blk[i].rank = k.rank;
-                q.blk[i].transpose_out = 0; q.blk[i].dst_ld = (int)(Cin * 9); q.blk[i].n_stride = 9;
-                q.blk[i].scale = k.scale; q.blk[i].dst = k.dst + (kh * 3 + kw);
-            }
-            rc = lg_launch(p, (cudaStream_t)stream_);
-            if (rc) return rc;
-        }
-    return HCP_OK;
-}
-
-// dW_down and dW_up of one LoRA group in ONE launch (two independent TN GEMMs over the same M token rows).
-extern "C" int hcp_lora_grad_pair(const void* U, const void* x, int64_t ldx, int64_t K, const hcp_lora_grad_block* down,
-                                  const void* T, const void* dy, int64_t lddy, int64_t N, const hcp_lora_grad_block* up,
-                                  int32_t nblocks, int64_t M, int64_t lds, hcp_stream_t stream_) {
-    if (M <= 0) return set_error(HCP_ERR_INVALID, "lora_grad_pair: M");
-    LoraGradParams p;
-    memset(&p, 0, sizeof(p));
-    p.M = (int)M; p.nprob = 2;
-    // split the SMs between the two problems in proportion to their column counts (one CTA per SM: 147 KB of smem each)
-    const int64_t ck = (K + 127) / 128, cn = (N + 127) / 128;
-    const int sms = num_sms();
-    int t0 = (int)((sms * ck + (ck + cn) / 2) / (ck + cn));
-    if (t0 < 1) t0 = 1;
-    if (t0 > sms - 1) t0 = sms - 1;
-    int rc = lg_fill(p, 0, U, lds, x, ldx, M, 0, K, down, nblocks, t0);
-    if (rc) return rc;
-    rc = lg_fill(p, 1, T, lds, dy, lddy, M, 0, N, up, nblocks, sms - t0);
-    if (rc) return rc;
-    return lg_launch(p, (cudaStream_t)stream_);
 }

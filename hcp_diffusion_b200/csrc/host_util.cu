@@ -102,6 +102,51 @@ int make_tmap_nd(CUtensorMap* out, const void* base, int rank, const uint64_t* d
     return HCP_OK;
 }
 
+int plan_conv_box(int64_t tH, int64_t tW, const char* who, ConvBox& box) {
+    char buf[96];
+    const char* why = nullptr;
+    box.bn = 1;
+    if (tW >= 128) {
+        box.bw = 128; box.bh = 1;
+        if (tW % 128) why = "W";
+    } else {
+        box.bw = (int)tW;
+        box.bh = 128 / box.bw;
+        if (128 % box.bw) why = "W must divide 128";
+        else if (box.bh <= tH) { if (tH % box.bh) why = "H tiling"; }
+        else {
+            box.bh = (int)tH;
+            if (128 % (box.bw * box.bh)) why = "H*W must divide 128";
+            else box.bn = 128 / (box.bw * box.bh);
+        }
+    }
+    if (why) {
+        snprintf(buf, sizeof(buf), "%s: %s", who, why);
+        return set_error(HCP_ERR_INVALID, buf);
+    }
+    box.tiles_w = (int)(tW / box.bw);
+    box.tiles_h = (int)(tH / box.bh);
+    return HCP_OK;
+}
+
+int make_tmap_nhwc(CUtensorMap* out, const void* x, int64_t B, int64_t H, int64_t W, int64_t C, int stride, const ConvBox& box) {
+    if (stride == 1) {
+        uint64_t dims[4] = {(uint64_t)C, (uint64_t)W, (uint64_t)H, (uint64_t)B};
+        uint64_t strides[3] = {(uint64_t)C * 2, (uint64_t)(W * C) * 2, (uint64_t)(H * W * C) * 2};
+        uint32_t bx[4] = {64, (uint32_t)box.bw, (uint32_t)box.bh, (uint32_t)box.bn};
+        return make_tmap_nd(out, x, 4, dims, strides, bx);
+    }
+    uint64_t dims[5] = {(uint64_t)(2 * C), (uint64_t)(W / 2), 2, (uint64_t)(H / 2), (uint64_t)B};
+    uint64_t strides[4] = {(uint64_t)(2 * C) * 2, (uint64_t)(W * C) * 2, (uint64_t)(2 * W * C) * 2, (uint64_t)(H * W * C) * 2};
+    uint32_t bx[5] = {64, (uint32_t)box.bw, 1, (uint32_t)box.bh, (uint32_t)box.bn};
+    return make_tmap_nd(out, x, 5, dims, strides, bx);
+}
+
+ConvTap conv_tap(int kh, int kw, int stride, int64_t C) {
+    if (stride == 1) return ConvTap{0, kw - 1, kh - 1, 0};
+    return ConvTap{(int32_t)((kw == 1 ? 0 : 1) * C), kw == 0 ? -1 : 0, kh == 0 ? -1 : 0, kh == 1 ? 0 : 1};
+}
+
 }  // namespace hcp
 
 extern "C" int hcp_version(void) { return 2; }

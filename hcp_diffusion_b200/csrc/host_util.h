@@ -28,6 +28,23 @@ inline int make_tmap_2d(CUtensorMap* out, const void* base, uint64_t inner, uint
     return make_tmap_nd(out, base, 2, dims, strides, box);
 }
 
+// Geometry of the 3x3 / pad 1 convolutions on NHWC bf16 activations (forward, dgrad and both weight-gradient kernels).
+// One 128-row M tile is a box of bw x bh pixels x bn images of the tile grid (tH x tW pixels per image): whole 128-pixel row pieces,
+// whole rows, or whole images.  The grid of such boxes is tiles_w x tiles_h per image (bn == 1) or ceil(B / bn) tiles (bn > 1).
+struct ConvBox {
+    int32_t bw, bh, bn, tiles_w, tiles_h;
+};
+// Plans the box of a tH x tW tile grid; on failure the error message starts with `who`.
+int plan_conv_box(int64_t tH, int64_t tW, const char* who, ConvBox& box);
+// TMA map of x [B, H, W, C] whose boxes are 64 channels x one ConvBox: 4-D for stride 1, for stride 2 the 5-D phase view
+// [B][H/2][2][W/2][2C] (input row 2*oh + kh - 1 and column 2*ow + kw - 1 become (phase, index) pairs of the view).
+int make_tmap_nhwc(CUtensorMap* out, const void* x, int64_t B, int64_t H, int64_t W, int64_t C, int stride, const ConvBox& box);
+// Shift of tap (kh, kw) in the map above: added to the channel, W, H coordinates of the box and, 5-D only, the H phase.
+struct ConvTap {
+    int32_t c0_off, dw, dh, c2;
+};
+ConvTap conv_tap(int kh, int kw, int stride, int64_t C);
+
 // Launch with programmatic stream serialization (PDL): the kernel may start while its predecessor on the stream drains; every
 // kernel of the library calls pdl_wait() (common.cuh) before touching global memory.  HCP_PDL=0 turns the attribute off.
 bool pdl_enabled();

@@ -24,25 +24,49 @@ namespace hcp {
 // D[j, n] += scale * sum_m S[m, j0 + j] * X[m, n0 + n]        (reduction over the M token / pixel rows)
 //   linear:  dW[o, k] : S = dY [M, N], X = x [M, K]
 //   conv3x3: dW[co, ci, kh, kw] : S = dY, X = x shifted by the tap (4-D / 5-D NHWC box, zero padding by TMA)
-// One CTA owns 128 columns of X and SN columns of S over a slice of the rows; MMA warpgroup g computes X columns [64g, 64g+64)
-// (wgmma M = 64, N = SN, K = 16 rows per instruction) and reduces its 64 x SN fp32 block into dst[j * ld_j + n * ld_n] with atomics.
+//   LoRA:    dW_down[j, k] = sum_m U[m, c0+j] x[m, k]  (S = U = dY . (alpha B), X = x, or the shifted box of a Conv2d LoRA)
+//            dW_up[o, j]   = alpha * sum_m dY[m, o0+o] T[m, c0+j]  (S = T = x . A^T, X = dY)
+// Both operands are read straight from their row-major [M, *] tensors as MN-major wgmma operands (TMA boxes of 64 columns x
+// 128 rows), so no transpose ever exists.  One CTA owns 128 columns of X and SN columns of S over a slice of the rows; MMA warpgroup
+// g computes X columns [64g, 64g+64) (wgmma M = 64, N = SN, K = 16 rows per instruction) and reduces its 64 x SN fp32 block into
+// the flat gradient buffer with atomics: dense, dst[j * ld_j + n * ld_n], or (kTable, SN = 64) through a table of up to 8 LoRA
+// blocks, each a rank range of the 64 S columns and an X column range with its own destination layout and scale.
 // =============================================================================================
 constexpr int kWgThreads = 288;   // warps 0-7: two MMA warpgroups, warp 8: TMA
+constexpr int LG_MAX_BLOCKS = 8;
 
+struct LGBlock {
+    int32_t n_lo, n_hi, c0, rank, transpose_out, dst_ld;
+    int32_t n_stride;        // element stride of the X-column index in the destination (1; 9 for the taps of a 3x3 W_down)
+    float scale;
+    float* dst;
+};
+struct LGTable {
+    int32_t nblocks;
+    LGBlock blk[LG_MAX_BLOCKS];
+};
+// X operand = shifted im2col box of a 3x3 convolution: the same boxes as the forward convolution's A operand
 struct WgConv {
     int32_t rank;            // 0: plain [M, ldx] matrix; 4 / 5: rank of the NHWC tensor map
-    int32_t bw, bh, bn, tiles_w, tiles_h;
-    int32_t c0_off, dw, dh, c2;
+    ConvBox box;
+    ConvTap tap;
 };
-struct alignas(64) WgradParams {
+struct WgProblem {
     CUtensorMap tmX, tmS;
-    int32_t M;
-    int32_t n_tiles, j_tiles, splits, tiles_per_cta;
-    int32_t n_cols, j_cols;          // valid X / S columns
+    int32_t n_begin, n_end;          // X columns [n_begin, n_end)
+    int32_t j_cols;                  // valid S columns (dense epilogue)
+    int32_t n_tiles, j_tiles, splits, tiles_per_cta, ctas;
+    // dense epilogue
     int64_t ld_j, ld_n;
     float scale;
     float* dst;
-    WgConv conv;
+    // table epilogue
+    LGTable tab;
+};
+struct alignas(64) WgradParams {
+    WgProblem prob[2];               // up to two independent problems per launch (dW_down and dW_up of one LoRA group)
+    int32_t M, nprob;
+    WgConv conv;                     // X geometry of the launch (a convolution launch carries one problem)
 };
 
 template <int SN>
@@ -54,8 +78,9 @@ struct WgCfg {
     static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 256 + 1024;
 };
 
-template <int SN>
+template <int SN, bool kTable>
 __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_constant__ WgradParams p) {
+    static_assert(!kTable || SN == 64, "the block table covers one 64-column slab of S");
     using Cfg = WgCfg<SN>;
     constexpr int STAGES = Cfg::STAGES;
     extern __shared__ uint8_t smem_raw[];
@@ -63,19 +88,22 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
     uint64_t* empty_bar = full_bar + STAGES;
     const int warp = warp_id_uniform(), lane = threadIdx.x & 31;
-    // flat grid over (row split, j tile, n tile): n fastest so that concurrent CTAs share the S tile in L2
-    const int bid = blockIdx.x;
-    const int nt = bid % p.n_tiles, jt = (bid / p.n_tiles) % p.j_tiles, sp = bid / (p.n_tiles * p.j_tiles);
-    const int ncol0 = nt * 128, jcol0 = jt * SN;
+    // flat grid over (problem, row split, j tile, n tile): n fastest so that concurrent CTAs share the S tile in L2.  Only the LoRA
+    // launches carry two problems; the dense variant keeps problem 0 a compile-time choice (90 instead of 94 registers at SN = 128).
+    int bid = blockIdx.x, z = 0;
+    if (kTable && p.nprob == 2 && bid >= p.prob[0].ctas) { bid -= p.prob[0].ctas; z = 1; }
+    const WgProblem& q = z ? p.prob[1] : p.prob[0];
+    const int nt = bid % q.n_tiles, jt = (bid / q.n_tiles) % q.j_tiles, sp = bid / (q.n_tiles * q.j_tiles);
+    const int ncol0 = q.n_begin + nt * 128, jcol0 = jt * SN;
     const int total_tiles = (p.M + 127) / 128;
-    const int t0 = sp * p.tiles_per_cta;
-    const int t1 = min(total_tiles, t0 + p.tiles_per_cta);
+    const int t0 = sp * q.tiles_per_cta;
+    const int t1 = min(total_tiles, t0 + q.tiles_per_cta);
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 256); }
         fence_mbar_init();
-        tma_prefetch_desc(&p.tmX);
-        tma_prefetch_desc(&p.tmS);
+        tma_prefetch_desc(&q.tmX);
+        tma_prefetch_desc(&q.tmS);
     }
     __syncthreads();
     pdl_trigger();
@@ -89,32 +117,42 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
                 mbar_arrive_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
                 uint8_t* base = smem + stage * Cfg::STAGE_BYTES;
                 if (p.conv.rank == 0) {
-                    tma_load_2d(base, &p.tmX, &full_bar[stage], ncol0, t * 128);
-                    tma_load_2d(base + 128 * 128, &p.tmX, &full_bar[stage], ncol0 + 64, t * 128);
+                    tma_load_2d(base, &q.tmX, &full_bar[stage], ncol0, t * 128);
+                    tma_load_2d(base + 128 * 128, &q.tmX, &full_bar[stage], ncol0 + 64, t * 128);
                 } else {
-                    const WgConv& cv = p.conv;
+                    const ConvBox& bx = p.conv.box;
+                    const ConvTap& tp = p.conv.tap;
                     int img0, h0 = 0, w0 = 0;
-                    if (cv.bn == 1) {
-                        const int per_img = cv.tiles_w * cv.tiles_h, r = t % per_img;
+                    if (bx.bn == 1) {
+                        const int per_img = bx.tiles_w * bx.tiles_h, r = t % per_img;
                         img0 = t / per_img;
-                        h0 = (r / cv.tiles_w) * cv.bh;
-                        w0 = (r % cv.tiles_w) * cv.bw;
+                        h0 = (r / bx.tiles_w) * bx.bh;
+                        w0 = (r % bx.tiles_w) * bx.bw;
                     } else {
-                        img0 = t * cv.bn;
+                        img0 = t * bx.bn;
                     }
                     for (int hf = 0; hf < 2; ++hf) {
-                        const int c = cv.c0_off + ncol0 + hf * 64;
-                        if (cv.rank == 4) tma_load_4d(base + hf * 128 * 128, &p.tmX, &full_bar[stage], c, w0 + cv.dw, h0 + cv.dh, img0);
-                        else tma_load_5d(base + hf * 128 * 128, &p.tmX, &full_bar[stage], c, w0 + cv.dw, cv.c2, h0 + cv.dh, img0);
+                        const int c = tp.c0_off + ncol0 + hf * 64;
+                        if (p.conv.rank == 4) tma_load_4d(base + hf * 128 * 128, &q.tmX, &full_bar[stage], c, w0 + tp.dw, h0 + tp.dh, img0);
+                        else tma_load_5d(base + hf * 128 * 128, &q.tmX, &full_bar[stage], c, w0 + tp.dw, tp.c2, h0 + tp.dh, img0);
                     }
                 }
 #pragma unroll
-                for (int q = 0; q < SN / 64; ++q)
-                    tma_load_2d(base + Cfg::X_BYTES + q * 128 * 128, &p.tmS, &full_bar[stage], jcol0 + q * 64, t * 128);
+                for (int s = 0; s < SN / 64; ++s)
+                    tma_load_2d(base + Cfg::X_BYTES + s * 128 * 128, &q.tmS, &full_bar[stage], jcol0 + s * 64, t * 128);
                 if (++stage == STAGES) { stage = 0; phase ^= 1; }
             }
         }
         return;
+    }
+    // The table epilogue walks `q.tab.blk[b]` with run-time z and b (dynamically indexed constant-bank loads): the MMA threads copy
+    // the table to shared memory first.
+    __shared__ LGTable stab;
+    if constexpr (kTable) {
+        const uint32_t* src = reinterpret_cast<const uint32_t*>(&q.tab);
+        uint32_t* dst = reinterpret_cast<uint32_t*>(&stab);
+        for (int i = threadIdx.x; i < (int)(sizeof(LGTable) / 4); i += 256) dst[i] = src[i];
+        asm volatile("bar.sync 1, 256;" ::: "memory");
     }
     const int wg = warp >> 2;
     float acc[SN / 2];
@@ -137,16 +175,40 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
     }
     wgmma_fence_acc(acc);
     if (t1 <= t0) return;
-    const float scale = p.scale;
+    const int n_row = ncol0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    if constexpr (kTable) {
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-        const int n = ncol0 + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;     // column of X
-        if (n >= p.n_cols) continue;
-        float* dcol = p.dst + (int64_t)n * p.ld_n;
+        for (int h = 0; h < 2; ++h) {
+            const int n = n_row + 8 * h;                                     // column of X
+            if (n >= q.n_end) continue;
+            for (int b = 0; b < stab.nblocks; ++b) {
+                const LGBlock& k = stab.blk[b];
+                if (n < k.n_lo || n >= k.n_hi) continue;
 #pragma unroll
-        for (int i = 0; i < SN / 4; ++i) {
-            const int j = jcol0 + 8 * (i >> 1) + 2 * (lane & 3) + (i & 1);          // column of S
-            if (j < p.j_cols) atomicAdd(dcol + (int64_t)j * p.ld_j, acc[4 * (i >> 1) + 2 * h + (i & 1)] * scale);
+                for (int i = 0; i < 16; ++i) {
+                    const int jj = 8 * (i >> 1) + 2 * (lane & 3) + (i & 1);   // column of S
+                    const int j = jj - k.c0;
+                    if (j >= 0 && j < k.rank) {
+                        const float val = acc[4 * (i >> 1) + 2 * h + (i & 1)] * k.scale;
+                        float* dst = k.transpose_out ? k.dst + (int64_t)(n - k.n_lo) * k.dst_ld + j
+                                                     : k.dst + (int64_t)j * k.dst_ld + (int64_t)(n - k.n_lo) * k.n_stride;
+                        atomicAdd(dst, val);
+                    }
+                }
+            }
+        }
+    } else {
+        const float scale = q.scale;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int n = n_row + 8 * h;                                     // column of X
+            if (n >= q.n_end) continue;
+            float* dcol = q.dst + (int64_t)n * q.ld_n;
+#pragma unroll
+            for (int i = 0; i < SN / 4; ++i) {
+                const int j = jcol0 + 8 * (i >> 1) + 2 * (lane & 3) + (i & 1);      // column of S
+                if (j < q.j_cols) atomicAdd(dcol + (int64_t)j * q.ld_j, acc[4 * (i >> 1) + 2 * h + (i & 1)] * scale);
+            }
         }
     }
 }
@@ -537,35 +599,86 @@ __global__ void __launch_bounds__(256) repack_kernel(const RepackJob* __restrict
     }
 }
 
-template <int SN>
-static int launch_wgrad(const WgradParams& p, int ctas, cudaStream_t stream) {
+template <int SN, bool kTable>
+static int launch_wgrad(const WgradParams& p, cudaStream_t stream) {
     using Cfg = WgCfg<SN>;
     static bool configured = false;
     if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(wgrad_tc_kernel<SN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
+        cudaError_t e = cudaFuncSetAttribute(wgrad_tc_kernel<SN, kTable>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
         if (e != cudaSuccess) return set_cuda_error(e, "cudaFuncSetAttribute(wgrad)");
         configured = true;
     }
-    launch_k(wgrad_tc_kernel<SN>, dim3(ctas), dim3(kWgThreads), Cfg::SMEM_BYTES, stream, p);
+    const int ctas = p.prob[0].ctas + (p.nprob == 2 ? p.prob[1].ctas : 0);
+    launch_k(wgrad_tc_kernel<SN, kTable>, dim3(ctas), dim3(kWgThreads), Cfg::SMEM_BYTES, stream, p);
     LAUNCH_CHECK("wgrad launch");
     return HCP_OK;
 }
 
-static int run_wgrad(WgradParams& p, int64_t j_cols, int64_t n_cols, cudaStream_t stream) {
-    const int sn = (j_cols > 64) ? 128 : 64;
-    p.n_tiles = (int)((n_cols + 127) / 128);
-    p.j_tiles = (int)((j_cols + sn - 1) / sn);
-    p.n_cols = (int)n_cols; p.j_cols = (int)j_cols;
-    const int total_tiles = (p.M + 127) / 128;
-    const int out_tiles = p.n_tiles * p.j_tiles;
-    int splits = (2 * num_sms() + out_tiles - 1) / out_tiles;    // about two waves of CTAs
+// `splits` CTAs (at least one 128-row tile each) share the rows of every output tile of the problem
+static void split_rows(WgProblem& q, int M, int splits) {
+    const int total_tiles = (M + 127) / 128;
     if (splits < 1) splits = 1;
     if (splits > total_tiles) splits = total_tiles;
-    p.tiles_per_cta = (total_tiles + splits - 1) / splits;
-    p.splits = (total_tiles + p.tiles_per_cta - 1) / p.tiles_per_cta;
-    const int ctas = out_tiles * p.splits;
-    if (sn == 128) return launch_wgrad<128>(p, ctas, stream);
-    return launch_wgrad<64>(p, ctas, stream);
+    q.tiles_per_cta = (total_tiles + splits - 1) / splits;
+    q.splits = (total_tiles + q.tiles_per_cta - 1) / q.tiles_per_cta;
+    q.ctas = q.n_tiles * q.j_tiles * q.splits;
+}
+
+// dense problem over S columns [0, j_cols) and X columns [0, n_cols): about two waves of CTAs
+static int run_wgrad(WgradParams& p, int64_t j_cols, int64_t n_cols, cudaStream_t stream) {
+    WgProblem& q = p.prob[0];
+    const int sn = (j_cols > 64) ? 128 : 64;
+    p.nprob = 1;
+    q.n_tiles = (int)((n_cols + 127) / 128);
+    q.j_tiles = (int)((j_cols + sn - 1) / sn);
+    q.n_end = (int)n_cols; q.j_cols = (int)j_cols;
+    const int out_tiles = q.n_tiles * q.j_tiles;
+    split_rows(q, p.M, (2 * num_sms() + out_tiles - 1) / out_tiles);
+    if (sn == 128) return launch_wgrad<128, false>(p, stream);
+    return launch_wgrad<64, false>(p, stream);
+}
+
+// X operand of a 3x3 / pad 1 convolution's weight gradient: the shifted boxes of the forward convolution, one row per output pixel
+static int conv_x(WgradParams& p, const void* x, int64_t B, int64_t Hin, int64_t Win, int64_t Cin, int stride, const char* who) {
+    const int64_t oH = Hin / stride, oW = Win / stride;
+    int rc = plan_conv_box(oH, oW, who, p.conv.box);
+    if (rc) return rc;
+    p.M = (int)(B * oH * oW);
+    p.conv.rank = stride == 1 ? 4 : 5;
+    return make_tmap_nhwc(&p.prob[0].tmX, x, B, Hin, Win, Cin, stride, p.conv.box);
+}
+
+// LoRA problem: the 64 S columns of one slab against X columns [n_begin, n_end) in 128-column chunks, `target_ctas` CTAs in all
+static void lg_problem(WgProblem& q, int M, int64_t n_begin, int64_t n_end, int target_ctas) {
+    q.n_begin = (int)n_begin; q.n_end = (int)n_end;
+    q.n_tiles = (int)((n_end - n_begin + 127) / 128);
+    q.j_tiles = 1;
+    split_rows(q, M, target_ctas / q.n_tiles);
+}
+
+static int lg_table(LGTable& t, const hcp_lora_grad_block* blocks, int32_t nblocks, const char* err) {
+    t.nblocks = nblocks;
+    for (int i = 0; i < nblocks; ++i) {
+        const hcp_lora_grad_block& k = blocks[i];
+        if (k.rank < 1 || k.c0 < 0 || k.c0 + k.rank > 64 || !k.dst) return set_error(HCP_ERR_INVALID, err);
+        t.blk[i].n_lo = (int)k.n_lo; t.blk[i].n_hi = (int)k.n_hi; t.blk[i].c0 = k.c0; t.blk[i].rank = k.rank;
+        t.blk[i].transpose_out = k.transpose_out; t.blk[i].dst_ld = (int)k.dst_ld; t.blk[i].scale = k.scale; t.blk[i].dst = k.dst;
+        t.blk[i].n_stride = 1;
+    }
+    return HCP_OK;
+}
+
+static int lg_fill(WgradParams& p, int z, const void* S, int64_t lds, const void* X, int64_t ldx, int64_t M, int64_t n_begin,
+                   int64_t n_end, const hcp_lora_grad_block* blocks, int32_t nblocks, int target_ctas) {
+    if (!S || !X || !blocks || nblocks < 1 || nblocks > LG_MAX_BLOCKS) return set_error(HCP_ERR_INVALID, "lora_grad: 1..8 blocks per problem");
+    if (n_end <= n_begin || (ldx % 8) != 0 || (n_begin % 8) != 0 || lds < 64 || (lds % 8) != 0) return set_error(HCP_ERR_INVALID, "lora_grad: shape");
+    WgProblem& q = p.prob[z];
+    int rc = make_tmap_2d(&q.tmX, X, (uint64_t)ldx, (uint64_t)M, (uint64_t)ldx, 64, 128);
+    if (rc) return rc;
+    rc = make_tmap_2d(&q.tmS, S, 64, (uint64_t)M, (uint64_t)lds, 64, 128);     // the 64 columns of S this launch reduces
+    if (rc) return rc;
+    lg_problem(q, p.M, n_begin, n_end, target_ctas);
+    return lg_table(q.tab, blocks, nblocks, "lora_grad: block descriptor");
 }
 
 }  // namespace hcp
@@ -578,10 +691,11 @@ extern "C" int hcp_wgrad_bf16(const void* S, int64_t lds, int64_t j_cols, const 
     if ((lds % 8) || (ldx % 8)) return set_error(HCP_ERR_INVALID, "wgrad: row pitches must be multiples of 8 elements");
     WgradParams p;
     memset(&p, 0, sizeof(p));
-    p.M = (int)M; p.scale = scale; p.dst = dst; p.ld_j = ld_j; p.ld_n = ld_n;
-    int rc = make_tmap_2d(&p.tmX, X, (uint64_t)n_cols, (uint64_t)M, (uint64_t)ldx, 64, 128);
+    WgProblem& q = p.prob[0];
+    p.M = (int)M; q.scale = scale; q.dst = dst; q.ld_j = ld_j; q.ld_n = ld_n;
+    int rc = make_tmap_2d(&q.tmX, X, (uint64_t)n_cols, (uint64_t)M, (uint64_t)ldx, 64, 128);
     if (rc) return rc;
-    rc = make_tmap_2d(&p.tmS, S, (uint64_t)j_cols, (uint64_t)M, (uint64_t)lds, 64, 128);
+    rc = make_tmap_2d(&q.tmS, S, (uint64_t)j_cols, (uint64_t)M, (uint64_t)lds, 64, 128);
     if (rc) return rc;
     return run_wgrad(p, j_cols, n_cols, (cudaStream_t)stream_);
 }
@@ -592,54 +706,84 @@ extern "C" int hcp_wgrad_conv3x3_bf16(const void* dy, int64_t Cout, const void* 
     if (!dy || !x || !dw) return set_error(HCP_ERR_INVALID, "wgrad_conv: null pointer");
     if (Cin % 64 != 0 || Cout % 8 != 0 || (stride != 1 && stride != 2)) return set_error(HCP_ERR_INVALID, "wgrad_conv: shape");
     if (stride == 2 && ((Hin | Win) & 1)) return set_error(HCP_ERR_INVALID, "wgrad_conv: odd extent with stride 2");
-    const int64_t oH = Hin / stride, oW = Win / stride;
-    int bw, bh, bnimg;                       // same 128-pixel tiles as hcp_conv3x3_bf16 (mode 0)
-    if (oW >= 128) { bw = 128; bh = 1; bnimg = 1; if (oW % 128) return set_error(HCP_ERR_INVALID, "wgrad_conv: W"); }
-    else {
-        bw = (int)oW;
-        if (128 % bw) return set_error(HCP_ERR_INVALID, "wgrad_conv: W must divide 128");
-        bh = 128 / bw;
-        if (bh <= oH) { if (oH % bh) return set_error(HCP_ERR_INVALID, "wgrad_conv: H tiling"); bnimg = 1; }
-        else { bh = (int)oH; if (128 % (bw * bh)) return set_error(HCP_ERR_INVALID, "wgrad_conv: H*W must divide 128"); bnimg = 128 / (bw * bh); }
-    }
     WgradParams p;
     memset(&p, 0, sizeof(p));
-    const int64_t M = B * oH * oW;
-    p.M = (int)M; p.scale = scale;
-    p.ld_j = Cin * 9; p.ld_n = 9;
-    int rc;
-    if (stride == 1) {
-        uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)Win, (uint64_t)Hin, (uint64_t)B};
-        uint64_t strides[3] = {(uint64_t)Cin * 2, (uint64_t)Win * Cin * 2, (uint64_t)Hin * Win * Cin * 2};
-        uint32_t box[4] = {64, (uint32_t)bw, (uint32_t)bh, (uint32_t)bnimg};
-        rc = make_tmap_nd(&p.tmX, x, 4, dims, strides, box);
-        p.conv.rank = 4;
-    } else {
-        uint64_t dims[5] = {(uint64_t)(2 * Cin), (uint64_t)(Win / 2), 2, (uint64_t)(Hin / 2), (uint64_t)B};
-        uint64_t strides[4] = {(uint64_t)(2 * Cin) * 2, (uint64_t)Win * Cin * 2, (uint64_t)(2 * Win * Cin) * 2, (uint64_t)Hin * Win * Cin * 2};
-        uint32_t box[5] = {64, (uint32_t)bw, 1, (uint32_t)bh, (uint32_t)bnimg};
-        rc = make_tmap_nd(&p.tmX, x, 5, dims, strides, box);
-        p.conv.rank = 5;
-    }
+    WgProblem& q = p.prob[0];
+    q.scale = scale; q.ld_j = Cin * 9; q.ld_n = 9;
+    int rc = conv_x(p, x, B, Hin, Win, Cin, stride, "wgrad_conv");
     if (rc) return rc;
-    rc = make_tmap_2d(&p.tmS, dy, (uint64_t)Cout, (uint64_t)M, (uint64_t)Cout, 64, 128);
+    rc = make_tmap_2d(&q.tmS, dy, (uint64_t)Cout, (uint64_t)p.M, (uint64_t)Cout, 64, 128);
     if (rc) return rc;
-    p.conv.bw = bw; p.conv.bh = bh; p.conv.bn = bnimg;
-    p.conv.tiles_w = (int)(oW / bw); p.conv.tiles_h = (int)(oH / bh);
     for (int kh = 0; kh < 3; ++kh)
         for (int kw = 0; kw < 3; ++kw) {
-            if (stride == 1) { p.conv.c0_off = 0; p.conv.dw = kw - 1; p.conv.dh = kh - 1; p.conv.c2 = 0; }
-            else {          // input row 2*oh + kh - 1 -> (phase, index) of the [H/2][2][W/2][2C] view, as in the forward conv
-                p.conv.c0_off = (int)(((kw == 1) ? 0 : 1) * Cin);
-                p.conv.dw = (kw == 0) ? -1 : 0;
-                p.conv.c2 = (kh == 1) ? 0 : 1;
-                p.conv.dh = (kh == 0) ? -1 : 0;
-            }
-            p.dst = dw + (kh * 3 + kw);
+            p.conv.tap = conv_tap(kh, kw, stride, Cin);
+            q.dst = dw + (kh * 3 + kw);
             rc = run_wgrad(p, Cout, Cin, (cudaStream_t)stream_);
             if (rc) return rc;
         }
     return HCP_OK;
+}
+
+extern "C" int hcp_lora_grad(const void* S, int64_t lds, const void* X, int64_t ldx, int64_t M, int64_t n_begin, int64_t n_end,
+                             const hcp_lora_grad_block* blocks, int32_t nblocks, hcp_stream_t stream_) {
+    if (M <= 0) return set_error(HCP_ERR_INVALID, "lora_grad: M");
+    WgradParams p;
+    memset(&p, 0, sizeof(p));
+    p.M = (int)M; p.nprob = 1;
+    int rc = lg_fill(p, 0, S, lds, X, ldx, M, n_begin, n_end, blocks, nblocks, num_sms());     // one wave of CTAs
+    if (rc) return rc;
+    return launch_wgrad<64, true>(p, (cudaStream_t)stream_);
+}
+
+// dW_down of a Conv2d LoRA: nine launches (one per tap) with the shifted NHWC box as X operand.
+extern "C" int hcp_lora_grad_conv3x3(const void* S, int64_t lds, const void* x, int64_t B, int64_t Hin, int64_t Win, int64_t Cin,
+                                     int32_t stride, const hcp_lora_grad_block* blocks, int32_t nblocks, hcp_stream_t stream_) {
+    if (!S || !x || !blocks || nblocks < 1 || nblocks > LG_MAX_BLOCKS) return set_error(HCP_ERR_INVALID, "lora_grad_conv: arguments");
+    if (Cin % 64 != 0 || (stride != 1 && stride != 2) || lds < 64 || (lds % 8) != 0) return set_error(HCP_ERR_INVALID, "lora_grad_conv: shape");
+    if (stride == 2 && ((Hin | Win) & 1)) return set_error(HCP_ERR_INVALID, "lora_grad_conv: odd extent with stride 2");
+    WgradParams p;
+    memset(&p, 0, sizeof(p));
+    WgProblem& q = p.prob[0];
+    p.nprob = 1;
+    int rc = conv_x(p, x, B, Hin, Win, Cin, stride, "lora_grad_conv");
+    if (rc) return rc;
+    rc = make_tmap_2d(&q.tmS, S, 64, (uint64_t)p.M, (uint64_t)lds, 64, 128);
+    if (rc) return rc;
+    lg_problem(q, p.M, 0, Cin, num_sms());
+    if ((rc = lg_table(q.tab, blocks, nblocks, "lora_grad_conv: block descriptor"))) return rc;
+    for (int i = 0; i < nblocks; ++i) {      // dW_down [r, Cin, 3, 3]: X column ci of tap t lands at dst[j * 9 Cin + 9 ci + t]
+        LGBlock& k = q.tab.blk[i];
+        k.n_lo = 0; k.n_hi = (int)Cin; k.transpose_out = 0; k.dst_ld = (int)(Cin * 9); k.n_stride = 9;
+    }
+    for (int kh = 0; kh < 3; ++kh)
+        for (int kw = 0; kw < 3; ++kw) {
+            p.conv.tap = conv_tap(kh, kw, stride, Cin);
+            for (int i = 0; i < nblocks; ++i) q.tab.blk[i].dst = blocks[i].dst + (kh * 3 + kw);
+            rc = launch_wgrad<64, true>(p, (cudaStream_t)stream_);
+            if (rc) return rc;
+        }
+    return HCP_OK;
+}
+
+// dW_down and dW_up of one LoRA group in ONE launch (two independent TN GEMMs over the same M token rows).
+extern "C" int hcp_lora_grad_pair(const void* U, const void* x, int64_t ldx, int64_t K, const hcp_lora_grad_block* down,
+                                  const void* T, const void* dy, int64_t lddy, int64_t N, const hcp_lora_grad_block* up,
+                                  int32_t nblocks, int64_t M, int64_t lds, hcp_stream_t stream_) {
+    if (M <= 0) return set_error(HCP_ERR_INVALID, "lora_grad_pair: M");
+    WgradParams p;
+    memset(&p, 0, sizeof(p));
+    p.M = (int)M; p.nprob = 2;
+    // split the SMs between the two problems in proportion to their column counts (one CTA per SM: 147 KB of smem each)
+    const int64_t ck = (K + 127) / 128, cn = (N + 127) / 128;
+    const int sms = num_sms();
+    int t0 = (int)((sms * ck + (ck + cn) / 2) / (ck + cn));
+    if (t0 < 1) t0 = 1;
+    if (t0 > sms - 1) t0 = sms - 1;
+    int rc = lg_fill(p, 0, U, lds, x, ldx, M, 0, K, down, nblocks, t0);
+    if (rc) return rc;
+    rc = lg_fill(p, 1, T, lds, dy, lddy, M, 0, N, up, nblocks, sms - t0);
+    if (rc) return rc;
+    return launch_wgrad<64, true>(p, (cudaStream_t)stream_);
 }
 
 extern "C" int hcp_colsum_bf16(const void* x, int64_t ld, int64_t M, int64_t N, int64_t rows_per_group, float scale, float* out,

@@ -247,6 +247,34 @@ def conv3x3_raw(x: torch.Tensor, w: torch.Tensor, B: int, Hin: int, Win: int, Ci
 # ----------------------------------------------------------------------------------------------------------------------
 # packed weights
 # ----------------------------------------------------------------------------------------------------------------------
+def lora_columns(blocks) -> int:
+    """Give each LoRA block of a pack its first rank column `c0`: blocks sit side by side, and one that would cross a 64-column
+    boundary (or is wider than 64) starts a new slab.  Returns the columns in use, alignment gaps included."""
+    c = 0
+    for b in blocks:
+        if b.rank > 64 or (c % 64) + b.rank > 64:
+            c = (c + 63) // 64 * 64
+        b.c0 = c
+        c += b.rank
+    return c
+
+
+def lora_slabs(blocks, R: int):
+    """[(slab index, [(block, first rank row j0, rows, first column inside the slab)])] of R rank columns: the pieces each launch of
+    the gradient kernel reduces (up to 8 per launch)."""
+    out = []
+    for q in range(R // 64):
+        lo, hi = 64 * q, 64 * q + 64
+        pieces = []
+        for b in blocks:
+            a, e = max(lo, b.c0), min(hi, b.c0 + b.rank)
+            if a < e:
+                pieces.append((b, a - b.c0, e - a, a - lo))
+        if pieces:
+            out.append((q, pieces))
+    return out
+
+
 class LoraBlockRef:
     """One LoRA block inside a fused linear group (see hcp_lora_job in include/hcp_b200.h).
     `branch`: None (applies to every row) or 'p' / 'n' -- DreamArtist++ adapters, reference DAPPPatchContainer.forward
@@ -330,15 +358,10 @@ class LinearPack:
 
     def attach_lora(self, blocks: List[LoraBlockRef]) -> None:
         self.lora = blocks
-        c = 0
         for b in blocks:
             if b.in_dim != self.K:
                 raise _lib.HcpError(f"LoRA block input width {b.in_dim} does not match the layer ({self.K})")
-            if b.rank > 64 or (c % 64) + b.rank > 64:
-                c = (c + 63) // 64 * 64
-            b.c0 = c
-            c += b.rank
-        self.r_tot = c
+        self.r_tot = c = lora_columns(blocks)
         self.R = (c + 63) // 64 * 64
         if self.R > 1024:
             raise _lib.HcpError(f"LoRA ranks of one fused linear group sum to {c} (> 1024 columns)")
@@ -399,20 +422,6 @@ class LinearPack:
                 A, BlT = (self.A, self.BlT) if br is None else (self.A_br[br], self.BlT_br[br])
                 j.A, j.AT, j.Bl, j.BlT = A.data_ptr(), self.AT.data_ptr(), self.Bl.data_ptr(), BlT.data_ptr()
                 out.append(j)
-        return out
-
-    def slabs(self):
-        """[(slab index, [(block, first rank row j0, rows, first column inside the slab)])] for the gradient kernel."""
-        out = []
-        for q in range(self.R // 64):
-            lo, hi = 64 * q, 64 * q + 64
-            pieces = []
-            for b in self.lora:
-                a, e = max(lo, b.c0), min(hi, b.c0 + b.rank)
-                if a < e:
-                    pieces.append((b, a - b.c0, e - a, a - lo))
-            if pieces:
-                out.append((q, pieces))
         return out
 
 
@@ -476,15 +485,11 @@ class ConvPack:
 
     def attach_lora(self, blocks: List[ConvLoraRef]) -> None:
         self.lora = blocks
-        c = 0
         for b in blocks:
             if b.w_down.shape[1] != self.Cin or tuple(b.w_down.shape[2:]) != (3, 3) or b.w_up.shape[0] != self.Cout:
                 raise _lib.HcpError("Conv2d LoRA block does not match its 3x3 host convolution")
-            if b.rank > 64 or (c % 64) + b.rank > 64:
-                c = (c + 63) // 64 * 64
-            b.c0 = c
-            c += b.rank
-        self.r_tot, self.R = c, (c + 63) // 64 * 64
+        self.r_tot = c = lora_columns(blocks)
+        self.R = (c + 63) // 64 * 64
         dev = self.W.device
         z = lambda *shape: torch.zeros(shape, dtype=BF16, device=dev)   # noqa: E731
         self.dapp = any(b.branch is not None for b in blocks)
@@ -519,19 +524,6 @@ class ConvPack:
             j.flip = 1 if self.stride == 1 else 0
             j.wt, j.wd = (self.Wt_br[b.branch] if self.dapp else self.Wt).data_ptr(), self.Wdl.data_ptr()
             out.append(j)
-        return out
-
-    def slabs(self):
-        out = []
-        for q in range(self.R // 64):
-            lo, hi = 64 * q, 64 * q + 64
-            pieces = []
-            for b in self.lora:
-                a, e = max(lo, b.c0), min(hi, b.c0 + b.rank)
-                if a < e:
-                    pieces.append((b, a - b.c0, e - a, a - lo))
-            if pieces:
-                out.append((q, pieces))
         return out
 
 
@@ -630,7 +622,7 @@ class FusedLinearFn(torch.autograd.Function):
 
     @staticmethod
     def _lora_grads(pack, xs, ks, T, U, dy, M, N, R):
-        for q, pieces in pack.slabs():
+        for q, pieces in lora_slabs(pack.lora, pack.R):
             for p0 in range(0, len(pieces), 8):
                 chunk = pieces[p0:p0 + 8]
                 nb = len(chunk)
@@ -827,7 +819,7 @@ class Conv3x3Fn(torch.autograd.Function):
                 Mh = M // 2
                 for half, br in ((0, "n"), (1, "p")):
                     gemm_raw([(_RowView(dy, half * Mh * N), N, N)], [(pack.BlT_br[br], N, R, 0)], Mh, R, _RowView(U, half * Mh * R), R)
-            for q, pieces in pack.slabs():
+            for q, pieces in lora_slabs(pack.lora, pack.R):
                 for p0 in range(0, len(pieces), 8):
                     chunk = pieces[p0:p0 + 8]
                     nb = len(chunk)

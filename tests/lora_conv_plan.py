@@ -5,10 +5,11 @@ path a case takes and the tiles its errors are measured over.
   tile_n        pick_bn (gemm.cu): column-tile width BN of the GEMM / convolution kernel
   split_plan    plan_splits + run_gemm + hcp_splitk_workspace_bytes (gemm.cu) for a convolution with total_k = 9 Cin + R: the number
                 of K-splits, k-blocks per split, and the split that holds the LoRA K-segment's k-blocks
-  conv_box      the 128-pixel box (bw x bh pixels x bnimg images) of hcp_conv3x3_bf16 and hcp_lora_grad_conv3x3
+  conv_box      plan_conv_box (host_util.cu): the 128-pixel box (bw x bh pixels x bnimg images) of every 3x3 convolution kernel:
+                hcp_conv3x3_bf16 (mode 0), hcp_wgrad_conv3x3_bf16 and hcp_lora_grad_conv3x3
   lora_grad_plan  hcp_lora_grad_conv3x3's grid: 128-column chunks of Cin and the row split of the 128-row tiles
-  lora_layout   ConvPack.attach_lora (ops.py): the first rank column c0 of each block, r_tot and the 64-padded R
-  slabs         ConvPack.slabs: the pieces of each 64-column slab the gradient kernels reduce, 8 per launch
+  lora_layout   lora_columns (ops.py, both packs' attach_lora): the first rank column c0 of each block, r_tot and the 64-padded R
+  slabs         lora_slabs (ops.py): the pieces of each 64-column slab the gradient kernel reduces, 8 per launch
 """
 H100_SMS = 132          # H100 SXM; the GPU tests re-plan with the live SM count
 BLOCK_K = 64
@@ -31,7 +32,7 @@ def plan_splits(ctas, total_kb, N, sms=H100_SMS):
 
 
 def conv_box(B, H, W, stride):
-    """128-pixel box of a mode-0 convolution (or of the dW_down kernel) on an H x W input."""
+    """128-pixel box of a mode-0 convolution, and of both weight-gradient kernels, on an H x W input (plan_conv_box in host_util.cu)."""
     oH, oW = H // stride, W // stride
     if oW >= 128:
         assert oW % 128 == 0
@@ -89,7 +90,7 @@ def lora_layout(ranks):
 
 
 def slabs(ranks):
-    """[(slab, [(block index, first rank row j0, rows, first column inside the slab)])], as ConvPack.slabs."""
+    """[(slab, [(block index, first rank row j0, rows, first column inside the slab)])], as lora_slabs in ops.py."""
     c0s, _, R = lora_layout(ranks)
     out = []
     for q in range(R // 64):

@@ -6,9 +6,12 @@ cases reach every branch of every planner; the GPU tests use the same functions 
                 channels, V 16-byte vectors per pixel row, 64 or 32 pixel lanes), two-pass 8-vector kernels `gn8`, two-pass pair kernels `gn`
   ln_plan       launch_layernorm (norms.cu): NVPL 16-byte vectors per lane, the software-pipelined variant, rows per warp
   wgrad_plan    run_wgrad (wgrad.cu): S-column tile SN and the number of row splits
-  conv_wgrad_plan  hcp_wgrad_conv3x3_bf16 (wgrad.cu): the 128-pixel box bw x bh x bnimg images
+  conv_box      plan_conv_box (host_util.cu): the 128-pixel box bw x bh x bnimg images of hcp_wgrad_conv3x3_bf16, which every 3x3
+                convolution kernel shares; restated once, in tests/lora_conv_plan.py
 """
 import math
+
+from lora_conv_plan import conv_box  # noqa: F401
 
 H100_SMS = 132          # H100 SXM; the GPU tests re-plan with the live SM count
 
@@ -66,21 +69,6 @@ def small_linear_dx_plan(M, N, K):
     while n_chunk < N and kb * -(-N // n_chunk) > 592:
         n_chunk *= 2
     return {"n_chunk": n_chunk, "row_blocks": -(-M // 16)}
-
-
-def conv_wgrad_plan(B, Hin, Win, stride):
-    oH, oW = Hin // stride, Win // stride
-    if oW >= 128:
-        assert oW % 128 == 0
-        return {"bw": 128, "bh": 1, "bnimg": 1}
-    bw = oW
-    assert 128 % bw == 0
-    bh = 128 // bw
-    if bh <= oH:
-        assert oH % bh == 0
-        return {"bw": bw, "bh": bh, "bnimg": 1}
-    assert 128 % (bw * oH) == 0
-    return {"bw": bw, "bh": oH, "bnimg": 128 // (bw * oH)}
 
 
 # ---------------------------------------------------------------------------------------------------------------------------------

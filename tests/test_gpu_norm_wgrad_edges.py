@@ -24,7 +24,7 @@ if ROOT not in sys.path:                # also run as a script: the forced two-p
 
 from kernel_check import CANARY, F32SIN, F32SUM, FWD, NORM, STAT, Canary, compare  # noqa: E402
 from norm_wgrad_plan import (AFFINE_CASES, COLSUM_CASES, CONV_WGRAD_CASES, GN_BATCH_CASES, GN_CASES, GN_OFFSET_SHAPES,  # noqa: E402
-                             GN_OFFSETS, GN_TWO_PASS_CASES, LN_CASES, REPACK_JOBS, SMALL_LINEAR_CASES, WGRAD_CASES, conv_wgrad_plan, gn_plan,
+                             GN_OFFSETS, GN_TWO_PASS_CASES, LN_CASES, REPACK_JOBS, SMALL_LINEAR_CASES, WGRAD_CASES, conv_box, gn_plan,
                              ln_plan, small_linear_dx_plan, wgrad_plan)
 
 pytestmark = pytest.mark.gpu
@@ -378,7 +378,7 @@ def conv_wgrad_ref(x, dy, stride):
 
 @pytest.mark.parametrize("B,H,W,Cin,Cout,stride", CONV_WGRAD_CASES)
 def test_conv3x3_wgrad(B, H, W, Cin, Cout, stride):
-    geo = conv_wgrad_plan(B, H, W, stride)
+    geo = conv_box(B, H, W, stride)
     Ho, Wo = H // stride, W // stride
     x = rnd(B, H, W, Cin, seed=1)
     dy = rnd(B, Ho, Wo, Cout, seed=2)

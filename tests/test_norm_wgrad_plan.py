@@ -1,8 +1,13 @@
 """CPU check that the cases of tests/test_gpu_norm_wgrad_edges.py reach every branch of the host-side planners they restate
 (tests/norm_wgrad_plan.py): each GroupNorm path and cluster size, each LayerNorm instantiation, each weight-gradient tile geometry."""
 from norm_wgrad_plan import (AFFINE_CASES, COLSUM_CASES, CONV_WGRAD_CASES, GN_BATCH_CASES, GN_CASES, GN_OFFSET_SHAPES, GN_TWO_PASS_CASES,
-                             LN_CASES, REPACK_JOBS, SMALL_LINEAR_CASES, WGRAD_CASES, conv_wgrad_plan, gn_plan, ln_plan, repack_paths,
+                             LN_CASES, REPACK_JOBS, SMALL_LINEAR_CASES, WGRAD_CASES, conv_box, gn_plan, ln_plan, repack_paths,
                              small_linear_dx_plan, wgrad_plan)
+
+
+def box_shape(B, H, W, stride):
+    box = conv_box(B, H, W, stride)
+    return box["bw"], box["bh"], box["bnimg"]
 
 
 def test_planners_follow_the_kernels_documented_choices():
@@ -15,7 +20,7 @@ def test_planners_follow_the_kernels_documented_choices():
     assert gn_plan(4096, 320, 0, 32, False, two_pass=True)["path"] == "gn8"
     assert ln_plan(16384, 320) == {"nvpl": 2, "pipe": True, "rpw": 8, "last_rows": 8}
     assert wgrad_plan(16384, 320, 320) == {"sn": 128, "splits": 26, "max_splits": 30, "tiles_per_cta": 5}
-    assert conv_wgrad_plan(1, 128, 128, 1) == {"bw": 128, "bh": 1, "bnimg": 1}
+    assert box_shape(1, 128, 128, 1) == (128, 1, 1)
 
 
 def test_groupnorm_cases_reach_every_path_and_cluster_size():
@@ -71,12 +76,12 @@ def test_wgrad_cases_reach_every_tile_geometry():
     assert {M % 128 for M, _, _ in WGRAD_CASES} >= {1, 127}                       # one-row tails, one row short of a tile
     assert any(p["splits"] == 1 for p in plans) and any(p["splits"] > 1 for p in plans)
     assert any(p["splits"] == p["max_splits"] == 2 * 132 for p in plans)          # the maximum row split: one tile per CTA
-    geos = {(tuple(conv_wgrad_plan(B, H, W, s).values()), s) for B, H, W, _, _, s in CONV_WGRAD_CASES}
+    geos = {(box_shape(B, H, W, s), s) for B, H, W, _, _, s in CONV_WGRAD_CASES}
     bn = {g[0][2] for g in geos}
     assert bn == {1, 2, 8, 32, 128}
     assert {s for g, s in geos if g[1] == 1 and g[2] == 1} == {1, 2}              # 128-wide rows, stride 1 and 2
     assert any(g[1] > 1 and g[2] == 1 for g, _ in geos)                           # several rows per tile
-    assert any(B % conv_wgrad_plan(B, H, W, s)["bnimg"] for B, H, W, _, _, s in CONV_WGRAD_CASES)   # a part-filled image tile
+    assert any(B % conv_box(B, H, W, s)["bnimg"] for B, H, W, _, _, s in CONV_WGRAD_CASES)   # a part-filled image tile
     # stride 2 from 128-, 64- and 16-wide inputs, with a Cin that is not a multiple of 128 (the phase-overlap case) and Cin 128
     s2 = [(W, Cin) for _, _, W, Cin, _, s in CONV_WGRAD_CASES if s == 2]
     assert {W for W, _ in s2} >= {128, 64, 16} and {Cin % 128 for _, Cin in s2} == {0, 64}

@@ -25,8 +25,9 @@ SEQ = {
     "hcp_attn_bwd_bf16": [("attn_bwd_prep", 1, 1), ("attn_bwd_kernel", 1, 3), ("attn_bwd_post_kernel", 1, 1), ("attn_bwd_post_kv", 0, 1)],
     "hcp_groupnorm_fwd_bf16": [("gn", 1, 3)],
     "hcp_groupnorm_bwd_bf16": [("gn", 1, 3)],
-    "hcp_lora_grad_pair": [("lora_grad", 1, 1)],
-    "hcp_lora_grad": [("lora_grad", 1, 1)],
+    # wgrad_tc_kernel<64, true>; launch lists recorded by earlier builds name it lora_grad_tc_kernel
+    "hcp_lora_grad_pair": [("grad_tc_kernel", 1, 1)],
+    "hcp_lora_grad": [("grad_tc_kernel", 1, 1)],
     "hcp_adamw_flat": [("incr_step", 0, 1), ("adamw", 1, 1)],
     "hcp_adamw_flat_dev": [("incr_step", 1, 1), ("adamw_flat_dev", 1, 1)],
 }
