@@ -153,7 +153,7 @@ EXPORTS = [
     "hcp_wgrad_bf16", "hcp_wgrad_conv3x3_bf16", "hcp_colsum_bf16", "hcp_norm_affine_grad_bf16", "hcp_small_linear_bwd_f32", "hcp_silu_f32",
     "hcp_conv_in_wgrad_f32", "hcp_conv_out_wgrad_f32", "hcp_repack_weights", "hcp_adafactor_flat",
     "hcp_attn_fwd_causal_bf16", "hcp_attn_bwd_causal_bf16", "hcp_quick_gelu_fwd_bf16", "hcp_quick_gelu_bwd_bf16", "hcp_embed_gather_bf16",
-    "hcp_sum_bf16_to_f32", "hcp_gelu_fwd_bf16", "hcp_gelu_bwd_bf16",
+    "hcp_sum_bf16_to_f32", "hcp_gelu_fwd_bf16", "hcp_gelu_bwd_bf16", "hcp_eps_loss_grouped_workspace_bytes", "hcp_eps_loss_grouped",
 ]
 
 
@@ -177,6 +177,8 @@ def lib() -> C.CDLL:
             l.hcp_splitk_workspace_bytes.argtypes = [C.c_int64] * 3
             l.hcp_groupnorm_workspace_bytes.restype = C.c_size_t
             l.hcp_groupnorm_workspace_bytes.argtypes = [C.c_int64] * 3
+            l.hcp_eps_loss_grouped_workspace_bytes.restype = C.c_size_t
+            l.hcp_eps_loss_grouped_workspace_bytes.argtypes = [C.c_int64] * 2
             vp, i64, f32, i32 = C.c_void_p, C.c_int64, C.c_float, C.c_int
             l.hcp_gemm_bf16.argtypes = [C.POINTER(GemmArgs), vp]
             l.hcp_conv3x3_bf16.argtypes = [C.POINTER(ConvArgs), vp]
@@ -219,6 +221,8 @@ def lib() -> C.CDLL:
             l.hcp_adamw_flat_dev.argtypes = [vp, vp, vp, vp, i64, vp, f32, vp, f32, vp, vp]
             l.hcp_adafactor_flat.argtypes = [vp, vp, vp, vp, vp, vp, vp, i64, vp, i64, vp, vp, C.c_int32, f32, vp, f32, vp]
             l.hcp_snr_mse_loss.argtypes = [vp, vp, vp, vp, f32, C.c_int32, i64, i64, f32, vp, vp, vp]
+            l.hcp_eps_loss_grouped.argtypes = [vp, vp, vp, vp, vp, vp, vp, C.c_int32, C.c_int32, f32, i64, i64, i64, f32, vp, vp, vp,
+                                               C.c_size_t, vp]
             l.hcp_ema_flat.argtypes = [vp, vp, i64, vp, f32, f32, f32, vp]
             l.hcp_dropout_bf16.argtypes = [vp, i64, vp, i64, vp, i64, i64, i64, i64, f32, vp, C.c_uint32, vp, i64, vp]
             l.hcp_counter_add_u64.argtypes = [vp, C.c_uint64, vp]

@@ -1,6 +1,8 @@
 // SPDX-License-Identifier: Apache-2.0
 // Training-step kernels either side of the UNet call that the plain MSE / AdamW pair of misc.cu does not cover (sm_90a):
 //   * SNR-weighted eps loss (reference hcpdiff/loss/min_snr_loss.py:5-52: MinSNR / SoftMinSNR / KDiffMinSNR / EDM weights)
+//   * the same loss over several data groups of one step with per-sample weights and a per-pixel mask (prior preservation,
+//     att_mask; reference hcpdiff/train_ac.py:467-482, 506-515), reduced in a fixed order
 //   * exponential moving average of the flat trainable buffer (reference hcpdiff/utils/ema.py:18-32)
 //   * nn.Dropout on a patched layer's output (reference hcpdiff/models/lora_base_patch.py:74), counter-based RNG so that the
 //     backward pass regenerates the forward mask instead of storing it, and CUDA-graph replays draw fresh masks
@@ -55,6 +57,96 @@ __global__ void snr_mse_loss_kernel(const float* __restrict__ pred, const float*
         float v = (threadIdx.x < (blockDim.x >> 5)) ? s_part[threadIdx.x] : 0.f;
         v = warp_sum(v);
         if (threadIdx.x == 0) atomicAdd(loss_sum, v / (float)n);
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Grouped, masked eps loss: the reference's get_loss with its per-pixel mask, (criterion(pred, target) * mask).mean()
+// (train_ac.py:506-515), weighted per data group and summed over the groups of one step (train_ac.py:467-482):
+//   group_loss[g] += sum_{b in g} scale_b * sum_{c,p} w(t_b) M[b,p] (pred - target)^2,   scale_b = loss_weight_g / (B_g C HW)
+//   dpred = 2 w M d scale_b grad_scale
+// Grid (chunks, B): block (c, b) covers elements [c * EPS_CHUNK, (c + 1) * EPS_CHUNK) of sample b and writes its partial to
+// ws[b * chunks + c]; eps_loss_reduce_kernel then sums ws per group in index order, so the loss bits do not depend on which
+// block finishes first (CUDA-graph replays are bit-identical).
+// ---------------------------------------------------------------------------------------------
+constexpr int64_t EPS_CHUNK = 4096;             // elements per block: 256 threads x 4 float4
+
+template <bool VEC>
+__global__ void eps_loss_grouped_kernel(const float* __restrict__ pred, const float* __restrict__ target, const int64_t* __restrict__ t,
+                                        const float* __restrict__ acp, const float* __restrict__ mask, const float* __restrict__ scale,
+                                        int mode, float gamma, int64_t per_image, int64_t HW, float grad_scale, float* __restrict__ ws,
+                                        float* __restrict__ dpred) {
+    pdl_trigger();
+    pdl_wait();
+    __shared__ float s_part[8];
+    const int64_t b = blockIdx.y;
+    const float w = mode < 0 ? 1.f : snr_weight(acp[t[b]], gamma, mode);
+    const float sc = scale[b];
+    const float gs = 2.f * w * sc * grad_scale;
+    const float* __restrict__ p_s = pred + b * per_image;
+    const float* __restrict__ q_s = target + b * per_image;
+    float* __restrict__ d_s = dpred ? dpred + b * per_image : nullptr;
+    const float* __restrict__ m_s = mask ? mask + b * HW : nullptr;
+    const int64_t lo = blockIdx.x * EPS_CHUNK;
+    const int64_t hi = min(lo + EPS_CHUNK, per_image);
+    float acc = 0.f;
+    if (VEC) {                                  // per_image % 4 == 0 and 16-byte aligned operands: lo, hi, i are multiples of 4
+        for (int64_t i = lo + 4 * (int64_t)threadIdx.x; i < hi; i += 4 * (int64_t)blockDim.x) {
+            const float4 pv = *reinterpret_cast<const float4*>(p_s + i), qv = *reinterpret_cast<const float4*>(q_s + i);
+            float4 mv = make_float4(1.f, 1.f, 1.f, 1.f);
+            if (m_s) {
+                const int64_t px = i % HW;
+                if ((HW & 3) == 0) mv = *reinterpret_cast<const float4*>(m_s + px);
+                else {                          // the 4 elements may straddle a channel boundary: the pixel index wraps
+                    mv.x = m_s[px];
+                    mv.y = m_s[px + 1 < HW ? px + 1 : px + 1 - HW];
+                    mv.z = m_s[px + 2 < HW ? px + 2 : px + 2 - HW];
+                    mv.w = m_s[px + 3 < HW ? px + 3 : px + 3 - HW];
+                }
+            }
+            const float dx = pv.x - qv.x, dy = pv.y - qv.y, dz = pv.z - qv.z, dw = pv.w - qv.w;
+            const float mx = mv.x * dx, my = mv.y * dy, mz = mv.z * dz, mw = mv.w * dw;
+            acc += mx * dx + my * dy + mz * dz + mw * dw;
+            if (d_s) *reinterpret_cast<float4*>(d_s + i) = make_float4(gs * mx, gs * my, gs * mz, gs * mw);
+        }
+    } else {
+        for (int64_t i = lo + threadIdx.x; i < hi; i += blockDim.x) {
+            const float d = p_s[i] - q_s[i];
+            const float md = (m_s ? m_s[i % HW] : 1.f) * d;
+            acc += md * d;
+            if (d_s) d_s[i] = gs * md;
+        }
+    }
+    acc = warp_sum(acc);
+    if ((threadIdx.x & 31) == 0) s_part[threadIdx.x >> 5] = acc;
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        float v = (threadIdx.x < (blockDim.x >> 5)) ? s_part[threadIdx.x] : 0.f;
+        v = warp_sum(v);
+        if (threadIdx.x == 0) ws[b * gridDim.x + blockIdx.x] = v * w * sc;
+    }
+}
+
+// group_loss[g] += sum of ws[b * chunks + c] over samples b of group g, in a fixed order (one block)
+__global__ void eps_loss_reduce_kernel(const float* __restrict__ ws, const int32_t* __restrict__ sample_group, int64_t B, int64_t chunks,
+                                       int ngroups, float* __restrict__ group_loss) {
+    pdl_trigger();
+    pdl_wait();
+    __shared__ float s_part[8];
+    const int64_t n = B * chunks;
+    for (int g = 0; g < ngroups; ++g) {
+        float acc = 0.f;
+        for (int64_t k = threadIdx.x; k < n; k += blockDim.x)
+            if (sample_group[k / chunks] == g) acc += ws[k];
+        acc = warp_sum(acc);
+        if ((threadIdx.x & 31) == 0) s_part[threadIdx.x >> 5] = acc;
+        __syncthreads();
+        if (threadIdx.x < 32) {
+            float v = (threadIdx.x < (blockDim.x >> 5)) ? s_part[threadIdx.x] : 0.f;
+            v = warp_sum(v);
+            if (threadIdx.x == 0) group_loss[g] += v;
+        }
+        __syncthreads();
     }
 }
 
@@ -185,6 +277,39 @@ extern "C" int hcp_snr_mse_loss(const float* pred, const float* target, const in
     launch_k(snr_mse_loss_kernel, dim3(blocks), dim3(256), 0, (cudaStream_t)st, pred, target, t, alphas_cumprod, gamma, (int)mode, per_image, n,
              grad_scale, loss_sum, dpred);
     LAUNCH_CHECK("snr_mse_loss launch");
+    return HCP_OK;
+}
+
+extern "C" size_t hcp_eps_loss_grouped_workspace_bytes(int64_t B, int64_t per_image) {
+    if (B <= 0 || per_image <= 0) return 0;
+    return (size_t)B * (size_t)((per_image + EPS_CHUNK - 1) / EPS_CHUNK) * sizeof(float);
+}
+
+extern "C" int hcp_eps_loss_grouped(const float* pred, const float* target, const int64_t* t, const float* alphas_cumprod, const float* mask,
+                                    const float* sample_scale, const int32_t* sample_group, int32_t ngroups, int32_t mode, float gamma,
+                                    int64_t B, int64_t C, int64_t HW, float grad_scale, float* group_loss, float* dpred, void* workspace,
+                                    size_t workspace_bytes, hcp_stream_t st) {
+    if (!pred || !target || !sample_scale || !sample_group || !group_loss || !workspace)
+        return set_error(HCP_ERR_INVALID, "eps_loss_grouped: null pointer");
+    if (mode < -1 || mode > 3 || (mode >= 0 && (!t || !alphas_cumprod || !(gamma > 0.f))))
+        return set_error(HCP_ERR_INVALID, "eps_loss_grouped: mode -1 (MSE) or 0..3 (SNR weights with t, alphas_cumprod and gamma > 0)");
+    if (B <= 0 || B > 65535 || C <= 0 || HW <= 0 || ngroups <= 0)
+        return set_error(HCP_ERR_INVALID, "eps_loss_grouped: shape (0 < B <= 65535, C, HW, ngroups > 0)");
+    const int64_t per_image = C * HW;
+    const int64_t chunks = (per_image + EPS_CHUNK - 1) / EPS_CHUNK;
+    if (workspace_bytes < hcp_eps_loss_grouped_workspace_bytes(B, per_image))
+        return set_error(HCP_ERR_INVALID, "eps_loss_grouped: workspace smaller than hcp_eps_loss_grouped_workspace_bytes(B, C * HW)");
+    const bool aligned = ((uintptr_t)pred | (uintptr_t)target | (uintptr_t)(dpred ? dpred : pred) | (uintptr_t)(mask ? mask : pred)) % 16 == 0;
+    const bool vec = aligned && (per_image % 4) == 0 && HW >= 4;
+    const dim3 grid((unsigned)chunks, (unsigned)B);
+    float* ws = (float*)workspace;
+    if (vec) launch_k(eps_loss_grouped_kernel<true>, grid, dim3(256), 0, (cudaStream_t)st, pred, target, t, alphas_cumprod, mask, sample_scale,
+                      (int)mode, gamma, per_image, HW, grad_scale, ws, dpred);
+    else launch_k(eps_loss_grouped_kernel<false>, grid, dim3(256), 0, (cudaStream_t)st, pred, target, t, alphas_cumprod, mask, sample_scale,
+                  (int)mode, gamma, per_image, HW, grad_scale, ws, dpred);
+    LAUNCH_CHECK("eps_loss_grouped launch");
+    launch_k(eps_loss_reduce_kernel, dim3(1), dim3(256), 0, (cudaStream_t)st, (const float*)ws, sample_group, B, chunks, (int)ngroups, group_loss);
+    LAUNCH_CHECK("eps_loss_grouped reduce launch");
     return HCP_OK;
 }
 

@@ -184,15 +184,21 @@ class LoraTrainStep:
     text embedding, and the text encoder runs forward and backward inside the same graph.  `text_encoder_opts`: {'n_repeats',
     'clip_skip', 'clip_final_norm'} of `models.encode_prompt`.  With an SDXL (text_time) UNet the text encoder is a
     `models.SDXLTextEncoder` (SDXLTEUnetWrapper): `step()` takes ids [B, 2 x 77] and `added_cond_kwargs={'time_ids'}`, and
-    `text_embeds` is the encoder's projected pooled row (`models.encode_prompt_sdxl`; n_repeats 1)."""
+    `text_embeds` is the encoder's projected pooled row (`models.encode_prompt_sdxl`; n_repeats 1).
+
+    `loss_weights`: one weight per data group of `step_groups()` (the reference's per-dataset `loss_weight`, e.g. DreamBooth's
+    prior-preservation class set); None weighs every group 1.0."""
 
     def __init__(self, unet: nn.Module, params: Union[Iterable[nn.Parameter], Sequence[dict]], lr: float = 1e-4, betas=(0.9, 0.999),
                  eps: float = 1e-8, weight_decay: float = 1e-2, max_grad_norm: float = 1.0, use_cuda_graph: bool = True,
                  process_group: Optional[dist.ProcessGroup] = None, side_stream: bool = True, grad_accum_steps: int = 1,
                  loss: Union[None, str, dict] = None, ema: Optional[dict] = None, cfg_scale=None, num_train_timesteps: int = 1000,
                  optimizer: str = "adamw", optimizer_kwargs: Optional[dict] = None, text_encoder: Optional[nn.Module] = None,
-                 text_encoder_opts: Optional[dict] = None):
+                 text_encoder_opts: Optional[dict] = None, loss_weights: Optional[Sequence[float]] = None):
         self.unet = unet
+        self.loss_weights = None if loss_weights is None else [float(w) for w in loss_weights]
+        self._group_tables: Dict[tuple, dict] = {}
+        self._graph_kind = None                            # 'step' or 'groups': which public call the CUDA graphs were captured for
         self.te, self.te_opts, self.sdxl = text_encoder, None, False
         if text_encoder is not None:
             if cfg_scale is not None:
@@ -361,22 +367,25 @@ class LoraTrainStep:
                 self.ema.copy_(self.flat.data)
 
     # ---- pieces ------------------------------------------------------------------------------------------------------
-    def _forward_backward(self, latents, noise, t, ehs, added=None):
-        """x_t = add_noise, pred = unet(x_t, t, ehs), loss, backward (gradients ACCUMULATE into the flat buffer)."""
+    def _forward_backward(self, latents, noise, t, ehs, added=None, grouped=None):
+        """x_t = add_noise, pred = unet(x_t, t, ehs), loss, backward (gradients ACCUMULATE into the flat buffer).  `grouped`: the
+        device tables of `step_groups()` (per-group weighted, masked loss into grouped['loss'])."""
         self.loss.zero_()
+        if grouped is not None:
+            grouped["loss"].zero_()
         ops.set_side_stream(self.side_stream)
         overlap = self.buckets is not None and self._micro == self.accum - 1      # DDP no_sync on all but the last micro-step
         if overlap:
             ops.set_grad_ready_callback(self.buckets.on_grad)
         try:
-            self._fb_body(latents, noise, t, ehs, added)
+            self._fb_body(latents, noise, t, ehs, added, grouped)
         finally:
             ops.set_grad_ready_callback(None)
             ops.join_side()
             ops.set_side_stream(False)
         ops.advance_dropout()
 
-    def _fb_body(self, latents, noise, t, ehs, added=None):
+    def _fb_body(self, latents, noise, t, ehs, added=None, grouped=None):
         B = latents.shape[0]
         per_image = latents[0].numel()
         x_t = torch.empty_like(latents)
@@ -397,7 +406,14 @@ class LoraTrainStep:
         self.noise_pred = leaf
         dpred = torch.empty_like(leaf)
         gscale = 1.0 / self.accum                          # accelerator.backward: loss / gradient_accumulation_steps
-        if self.loss_cfg is None:
+        if grouped is not None:                            # sum_g loss_weight_g * (criterion * mask).mean() over the groups' samples
+            mode, gamma = self.loss_cfg if self.loss_cfg is not None else (-1, 1.0)
+            C = leaf.shape[1]
+            ws = grouped["ws"]
+            call("hcp_eps_loss_grouped", leaf.data_ptr(), noise.data_ptr(), t.data_ptr(), self.acp.data_ptr(), _lib.ptr(grouped["mask"]),
+                 grouped["scale"].data_ptr(), grouped["group"].data_ptr(), grouped["loss"].numel(), mode, gamma, B, C, per_image // C,
+                 gscale, grouped["loss"].data_ptr(), dpred.data_ptr(), ws.data_ptr(), ws.numel() * 4, stream_ptr())
+        elif self.loss_cfg is None:
             call("hcp_mse_loss", leaf.data_ptr(), noise.data_ptr(), leaf.numel(), gscale, self.loss.data_ptr(), dpred.data_ptr(), stream_ptr())
         else:
             mode, gamma = self.loss_cfg
@@ -458,8 +474,12 @@ class LoraTrainStep:
                                    ehs.to(dev, non_blocking=True), added)
             self._finish_micro(self._optimizer)
             return self.loss
+        if self._graph_kind == "groups":
+            raise RuntimeError("this LoraTrainStep captured its CUDA graphs for step_groups(); call step_groups() (one group for a "
+                               "single batch) or use a separate instance for step()")
         if self._static is None:
             self._capture(latents, noise, t, ehs, added_cond_kwargs)
+            self._graph_kind = "step"
         s = self._static
         s["latents"].copy_(latents, non_blocking=True)
         s["noise"].copy_(noise, non_blocking=True)
@@ -472,13 +492,133 @@ class LoraTrainStep:
         self._finish_micro(self._graph_opt.replay)
         return self.loss
 
+    def step_groups(self, batches: Sequence[Dict[str, torch.Tensor]]) -> torch.Tensor:
+        """One micro-step over several data groups (the reference's `cfgs.data` datasets, e.g. DreamBooth's instance set next to its
+        prior-preservation class set; hcpdiff/train_ac.py:467-482).  `batches`: one dict per group, {'latents', 'noise', 't', 'ehs'}
+        as `step()` takes them, plus optional 'added_cond_kwargs' and 'mask' (fp32 [B_g, h, w] or [B_g, 1, h, w] at latent
+        resolution, the reference's att_mask weights; absent = ones).  The groups run as ONE UNet pass over their concatenation
+        (every op is per-sample independent), and the loss is sum_g loss_weight_g * mean(criterion * mask) with each group's own
+        mean, so the gradient is the reference's sum over per-group backward passes.  Groups share the latent shape, the text
+        width and the added-cond layout.  Returns the device tensor fp32 [G] of the weighted per-group losses of this micro-step
+        (the reference logs the last one)."""
+        G = len(batches)
+        weights = self.loss_weights if self.loss_weights is not None else [1.0] * G
+        if G == 0 or len(weights) != G:
+            raise ValueError(f"step_groups: {G} batches for {len(weights)} loss_weights")
+        lat, noise, t, ehs, added, mask, sizes = self._concat_groups(batches)
+        dev = self.flat.data.device
+        C, HW = lat.shape[1], lat[0, 0].numel()
+        if not self.use_graph:
+            tables = self._tables(sizes, weights, C, HW)
+            mask_dev = None if mask is None else mask.to(dev, non_blocking=True)
+            added = None if added is None else {k: v.to(dev, non_blocking=True) for k, v in added.items()}
+            self._forward_backward(lat.to(dev, non_blocking=True), noise.to(dev, non_blocking=True), t.to(dev, non_blocking=True),
+                                   ehs.to(dev, non_blocking=True), added, {**tables, "mask": mask_dev})
+            self._finish_micro(self._optimizer)
+            return tables["loss"]
+        if self._graph_kind == "step":
+            raise RuntimeError("this LoraTrainStep captured its CUDA graphs for step(); use a separate instance for step_groups()")
+        if self._static is None:
+            tables = self._tables(sizes, weights, C, HW)
+            self._capture(lat, noise, t, ehs, added, grouped={**tables, "mask": None if mask is None else mask.to(dev).float().clone(),
+                                                              "sizes": sizes})
+            self._graph_kind = "groups"
+        s = self._static
+        grouped = s["grouped"]
+        if sizes != grouped["sizes"]:
+            raise ValueError(f"step_groups: group batch sizes {sizes} differ from the captured {grouped['sizes']}")
+        if mask is not None and grouped["mask"] is None:
+            raise ValueError("step_groups: a mask is given but the CUDA graphs were captured without one (pass a ones mask on the "
+                             "first call to train with masks later)")
+        s["latents"].copy_(lat, non_blocking=True)
+        s["noise"].copy_(noise, non_blocking=True)
+        s["t"].copy_(t, non_blocking=True)
+        s["ehs"].copy_(ehs, non_blocking=True)
+        if s["added"] is not None:
+            for k, v in s["added"].items():
+                v.copy_(added[k], non_blocking=True)
+        if grouped["mask"] is not None:
+            if mask is None:
+                grouped["mask"].fill_(1.0)
+            else:
+                grouped["mask"].copy_(mask, non_blocking=True)
+        self._graph_fb.replay()
+        self._finish_micro(self._graph_opt.replay)
+        return grouped["loss"]
+
+    def _concat_groups(self, batches):
+        """Concatenate the groups' tensors along the batch in the layouts the step expects; refuse groups that cannot share a pass."""
+        allowed = {"latents", "noise", "t", "ehs", "added_cond_kwargs", "mask"}
+        sizes, lats, noises, ts, ehss, addeds, masks = [], [], [], [], [], [], []
+        for g, b in enumerate(batches):
+            unknown = set(b) - allowed
+            if unknown:
+                raise ValueError(f"step_groups: group {g} has unknown keys {sorted(unknown)} (allowed: {sorted(allowed)})")
+            lat, nz, tt, eh = b["latents"], b["noise"], b["t"], b["ehs"]
+            B = lat.shape[0]
+            if lat.dim() != 4 or tuple(nz.shape) != tuple(lat.shape) or tuple(tt.shape) != (B,):
+                raise ValueError(f"step_groups: group {g}: latents [B,C,h,w], noise of the same shape and t [B] (got "
+                                 f"{tuple(lat.shape)}, {tuple(nz.shape)}, {tuple(tt.shape)})")
+            if lats and tuple(lat.shape[1:]) != tuple(lats[0].shape[1:]):
+                raise ValueError(f"step_groups: group {g} latents {tuple(lat.shape[1:])} differ from group 0's "
+                                 f"{tuple(lats[0].shape[1:])}: groups share one latent shape (buckets are not supported)")
+            rows = 2 * B if self.cfg_ctx is not None else B
+            if eh.shape[0] != rows:
+                raise ValueError(f"step_groups: group {g}: ehs has {eh.shape[0]} rows, expected {rows}"
+                                 + (" ([negative | positive] with cfg_scale)" if self.cfg_ctx is not None else ""))
+            if ehss and tuple(eh.shape[1:]) != tuple(ehss[0].shape[1:]):
+                raise ValueError(f"step_groups: group {g} ehs {tuple(eh.shape[1:])} differs from group 0's {tuple(ehss[0].shape[1:])}")
+            ad = b.get("added_cond_kwargs")
+            if addeds and (ad is None) != (addeds[0] is None):
+                raise ValueError(f"step_groups: group {g}: added_cond_kwargs must be given for every group or for none")
+            if ad is not None:
+                if any(v.shape[0] != B for v in ad.values()):
+                    raise ValueError(f"step_groups: group {g}: added_cond_kwargs rows differ from its batch {B}")
+                if addeds and ({k: tuple(v.shape[1:]) for k, v in ad.items()} != {k: tuple(v.shape[1:]) for k, v in addeds[0].items()}):
+                    raise ValueError(f"step_groups: group {g}: added_cond_kwargs layout differs from group 0's")
+            m = b.get("mask")
+            if m is not None:
+                if tuple(m.shape) not in ((B,) + tuple(lat.shape[2:]), (B, 1) + tuple(lat.shape[2:])):
+                    raise ValueError(f"step_groups: group {g}: mask {tuple(m.shape)}, expected [{B}, h, w] or [{B}, 1, h, w] at latent "
+                                     f"resolution {tuple(lat.shape[2:])}")
+                m = m.reshape(B, -1).float()
+            sizes.append(B)
+            lats.append(lat), noises.append(nz), ts.append(tt), ehss.append(eh), addeds.append(ad), masks.append(m)
+        if self.cfg_ctx is not None:                       # [neg_1 .. neg_G | pos_1 .. pos_G], the layout _CfgMixFn expects
+            ehs = torch.cat([e[:B] for e, B in zip(ehss, sizes)] + [e[B:] for e, B in zip(ehss, sizes)], 0)
+        else:
+            ehs = torch.cat(ehss, 0)
+        added = None if addeds[0] is None else {k: torch.cat([a[k] for a in addeds], 0) for k in addeds[0]}
+        mask = None
+        if any(m is not None for m in masks):
+            HW = lats[0][0, 0].numel()
+            mask = torch.cat([m if m is not None else torch.ones((B, HW), dtype=torch.float32, device=lats[g].device)
+                              for g, (m, B) in enumerate(zip(masks, sizes))], 0)
+        return (torch.cat(lats, 0), torch.cat(noises, 0), torch.cat(ts, 0), ehs, added, mask, tuple(sizes))
+
+    def _tables(self, sizes, weights, C, HW):
+        """Device tables of the grouped loss for these group sizes (built once per layout): sample_scale fp32 [B] = w_g / (B_g C HW),
+        sample_group int32 [B], the per-group loss fp32 [G] and the kernel's workspace."""
+        key = (sizes, tuple(weights), C, HW)
+        tab = self._group_tables.get(key)
+        if tab is None:
+            dev = self.flat.data.device
+            scale = [w / (B * C * HW) for w, B in zip(weights, sizes) for _ in range(B)]
+            group = [g for g, B in enumerate(sizes) for _ in range(B)]
+            nbytes = _lib.lib().hcp_eps_loss_grouped_workspace_bytes(sum(sizes), C * HW)
+            tab = {"scale": torch.tensor(scale, dtype=torch.float32, device=dev), "group": torch.tensor(group, dtype=torch.int32, device=dev),
+                   "loss": torch.zeros(len(sizes), dtype=torch.float32, device=dev),
+                   "ws": torch.zeros((nbytes + 3) // 4, dtype=torch.float32, device=dev)}
+            self._group_tables[key] = tab
+        return tab
+
     def step_resident(self) -> torch.Tensor:
         """Replay on the inputs already resident in the static device buffers (kernel-only timing in bench.py)."""
         if self._static is None:
             raise RuntimeError("call step() once before step_resident()")
         self._graph_fb.replay()
         self._finish_micro(self._graph_opt.replay)
-        return self.loss
+        return self.loss if self._graph_kind != "groups" else self._static["grouped"]["loss"]
 
     def ema_state(self) -> Dict[nn.Parameter, torch.Tensor]:
         """{parameter: EMA tensor view} (what ModelEMA.state_dict() holds for the trainable parameters)."""
@@ -499,13 +639,14 @@ class LoraTrainStep:
         ops.dropout_state_restore(saved[3])
         self.flat.grad.zero_()
 
-    def _capture(self, latents, noise, t, ehs, added=None):
+    def _capture(self, latents, noise, t, ehs, added=None, grouped=None):
         dev = self.flat.data.device
         self._static = {
             "latents": latents.to(dev).float().contiguous().clone(), "noise": noise.to(dev).float().contiguous().clone(),
             "t": t.to(dev).long().contiguous().clone(),
             "ehs": (ehs.to(dev).long() if self.te is not None else ehs.to(dev).float()).contiguous().clone(),
             "added": None if added is None else {k: v.to(dev).float().contiguous().clone() for k, v in added.items()},
+            "grouped": grouped,
         }
         s = self._static
         # warm-up on a side stream (builds the packed weights, tensor maps, autograd metadata) -- parameters, optimizer state and
@@ -517,7 +658,7 @@ class LoraTrainStep:
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
             for _ in range(2):
-                self._forward_backward(s["latents"], s["noise"], s["t"], s["ehs"], s["added"])
+                self._forward_backward(s["latents"], s["noise"], s["t"], s["ehs"], s["added"], s["grouped"])
                 self._optimizer()
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
@@ -525,7 +666,7 @@ class LoraTrainStep:
         before = _lib.launch_count
         self._graph_fb = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self._graph_fb):
-            self._forward_backward(s["latents"], s["noise"], s["t"], s["ehs"], s["added"])
+            self._forward_backward(s["latents"], s["noise"], s["t"], s["ehs"], s["added"], s["grouped"])
         self._graph_opt = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self._graph_opt):
             self._optimizer()

@@ -25,6 +25,15 @@ Colossal-AI trainers.  Inputs are the synthetic latents / text embeddings of SUR
 in a .pt file (`data.path`: {'latents': [N,4,h,w], 'encoder_hidden_states': [N,L,768]}, plus 'text_embeds' / 'time_ids' for an
 SDXL ('text_time') UNet, whose synthetic time ids are (H, W, 0, 0, H, W) in pixels).
 
+Data groups (the reference's dict of datasets, cfgs/train/dataset/base_dataset.yaml and regularization_dataset.yaml, e.g.
+DreamBooth's `dataset1` next to its prior-preservation `dataset_class`): `data` with a top-level `batch_size` is the flat form
+above; otherwise every mapping under `data` is a group with its own `batch_size`, `loss_weight` (default 1.0) and `path` or
+synthetic `num_samples` / `tokens`.  A group's .pt file may also hold 'mask' fp32 [N, h, w], the per-pixel loss weights at latent
+resolution (the reference's `att_mask` after its grey-to-weight mapping and resize; absent = ones).  Every step runs all groups as
+one micro-step (`LoraTrainStep.step_groups`: gradient sum_g loss_weight_g * loss_g, reference train_ac.py:467-482), `scale_lr`
+counts the sum of the groups' batch sizes, the img/s log counts every group's images and the logged loss is the last group's
+weighted loss, as the reference logs it.  Groups share one latent shape (no aspect-ratio buckets).
+
 Launch data-parallel with torchrun (one process per GPU); gradients are all-reduced over NCCL, every replica starts from rank
 0's parameters (DDP's construction-time broadcast), the learning rate is scaled by batch x world x accumulation when
 `train.scale_lr` is set (reference train_ac.py:192-197).
@@ -78,6 +87,31 @@ def optimizer_from_cfg(opt_cfg):
             kw["eps"] = tuple(kw["eps"])
         return "adafactor", adafactor.check_options(kw)
     raise NotImplementedError(f"train.optimizer._target_={target!r}: torch.optim.AdamW or transformers.optimization.Adafactor")
+
+
+def data_groups(data_cfg):
+    """`data` -> None for the flat form (a top-level `batch_size`, or no dataset mappings: one batch of `batch_size`, default 4), else
+    [(name, cfg, batch_size, loss_weight)] for the reference's dict of datasets (cfgs/train/dataset/base_dataset.yaml,
+    regularization_dataset.yaml): every mapping under `data` is a group with its own `batch_size`, `loss_weight` (default 1.0) and
+    `path` or synthetic `num_samples` / `tokens`."""
+    data_cfg = data_cfg or {}
+    if "batch_size" in data_cfg:
+        return None
+    groups = [(name, g, int(g.get("batch_size", 1)), float(g.get("loss_weight", 1.0))) for name, g in data_cfg.items() if isinstance(g, dict)]
+    if not groups:
+        return None
+    for name, _, bs, _ in groups:
+        if bs <= 0:
+            raise ValueError(f"data.{name}.batch_size must be positive")
+    return groups
+
+
+def images_per_step(data_cfg) -> int:
+    """Images of one micro-step over every data group: what `scale_lr` multiplies by (reference train_ac.py:192-197)."""
+    groups = data_groups(data_cfg)
+    if groups is None:
+        return int((data_cfg or {}).get("batch_size", 4))
+    return sum(bs for _, _, bs, _ in groups)
 
 
 class _LrOnly(torch.optim.Optimizer):
@@ -158,7 +192,8 @@ class Trainer:
             self.unet.enable_gradient_checkpointing()
 
         tr = cfgs.train
-        bs = int(cfgs.data.get("batch_size", 4))
+        self.groups = data_groups(cfgs.data)
+        bs = images_per_step(cfgs.data)
         accum = int(tr.get("gradient_accumulation_steps", 1))
         lr_scale = bs * self.world * accum if tr.get("scale_lr", False) else 1
         opt_cfg = tr.get("optimizer") or {}
@@ -194,7 +229,8 @@ class Trainer:
                                      max_grad_norm=float(tr.get("max_grad_norm", 1.0)), use_cuda_graph=bool(tr.get("cuda_graph", True)),
                                      grad_accum_steps=accum, loss=loss_from_cfg(tr.get("loss")), ema=ema,
                                      cfg_scale=None if cfg_scale in (None, "1.0", 1.0) else str(cfg_scale),
-                                     optimizer=opt_name, optimizer_kwargs=af_opts, text_encoder=self.te, text_encoder_opts=te_opts)
+                                     optimizer=opt_name, optimizer_kwargs=af_opts, text_encoder=self.te, text_encoder_opts=te_opts,
+                                     loss_weights=None if self.groups is None else [w for _, _, _, w in self.groups])
         self.step_fn.sync_params(src=0)
         self.sched_step = make_scheduler(tr.get("scheduler"), self.step_fn)
         self.bs, self.accum = bs, accum
@@ -241,23 +277,39 @@ class Trainer:
         g = torch.Generator().manual_seed(1234 + self.rank)
         cfg = self.unet.config
         self.text_time = getattr(cfg, "addition_embed_type", None) == "text_time"
-        self.text_embeds = self.time_ids = None
+        if self.groups is None:
+            src = self._load_source(d, seed)
+            self.latents, self.ehs, self.ehs_neg = src["latents"], src["ehs"], src["ehs_neg"]
+            self.time_ids, self.text_embeds = src["time_ids"], src["text_embeds"]
+        else:                                                    # one source per data group, each with its own synthetic seed
+            self.sources = [self._load_source(gc, seed + 1000 * i) for i, (_, gc, _, _) in enumerate(self.groups)]
+        self.gen = g
+
+    def _load_source(self, d, seed: int):
+        """One dataset: the tensors of `d.path`, or synthetic latents / text of `d.num_samples` / `d.tokens` drawn from `seed`."""
+        cfg = self.unet.config
+        src = {"text_embeds": None, "time_ids": None, "mask": None}
         if d.get("path"):
-            blob = torch.load(d.path, map_location="cpu")
-            self.latents = blob["latents"].float()
-            self.ehs = blob["input_ids"].long() if self.te is not None else blob["encoder_hidden_states"].float()
-            self.ehs_neg = blob.get("negative_hidden_states")
+            blob = torch.load(d["path"], map_location="cpu")
+            src["latents"] = blob["latents"].float()
+            src["ehs"] = blob["input_ids"].long() if self.te is not None else blob["encoder_hidden_states"].float()
+            src["ehs_neg"] = blob.get("negative_hidden_states")
             if self.text_time:
-                self.time_ids = blob["time_ids"].float()
+                src["time_ids"] = blob["time_ids"].float()
                 if self.te is None:                              # with a text encoder, text_embeds is its pooled projection
-                    self.text_embeds = blob["text_embeds"].float()
+                    src["text_embeds"] = blob["text_embeds"].float()
+            if blob.get("mask") is not None:                     # att_mask weights at latent resolution [N, h, w]
+                src["mask"] = blob["mask"].float()
+                if tuple(src["mask"].shape) != (src["latents"].shape[0],) + tuple(src["latents"].shape[2:]):
+                    raise ValueError(f"{d['path']}: 'mask' {tuple(src['mask'].shape)} must be [N, h, w] of the latents "
+                                     f"{tuple(src['latents'].shape)}")
         else:
             n = int(d.get("num_samples", 64))
             s = int(self.unet.config.sample_size)
             gd = torch.Generator().manual_seed(seed)             # the synthetic "dataset" is the same on every rank; the sampling differs
-            self.latents = torch.randn((n, self.unet.config.in_channels, s, s), generator=gd)
-            self.ehs = torch.randn((n, int(d.get("tokens", 77)), self.unet.config.cross_attention_dim), generator=gd)
-            self.ehs_neg = torch.randn((n, int(d.get("tokens", 77)), self.unet.config.cross_attention_dim), generator=gd)
+            src["latents"] = torch.randn((n, self.unet.config.in_channels, s, s), generator=gd)
+            src["ehs"] = torch.randn((n, int(d.get("tokens", 77)), self.unet.config.cross_attention_dim), generator=gd)
+            src["ehs_neg"] = torch.randn((n, int(d.get("tokens", 77)), self.unet.config.cross_attention_dim), generator=gd)
             if self.te is not None:                              # prompts of 77-token chunks: BOS, random tokens, EOS padding
                 R = self.step_fn.te_opts["n_repeats"]
                 ids = torch.full((n * R, 77), 49407, dtype=torch.int64)
@@ -266,19 +318,19 @@ class Trainer:
                 words = torch.randint(0, 49406, (n * R, 75), generator=gd)
                 keep = torch.arange(75)[None] < lens[:, None]
                 ids[:, 1:76] = torch.where(keep, words, ids[:, 1:76])
-                self.ehs = ids.reshape(n, 77 * R)
+                src["ehs"] = ids.reshape(n, 77 * R)
                 if self.step_fn.sdxl:                            # the same words for bigG, whose tokenizer pads with id 0 after EOS
                     ids_g = ids.clone()
                     ids_g[:, 1:] = torch.where(torch.arange(1, 77)[None] <= lens[:, None] + 1, ids[:, 1:], 0)
-                    self.ehs = torch.cat([ids, ids_g], 1)
+                    src["ehs"] = torch.cat([ids, ids_g], 1)
             if self.text_time:                                   # pooled text embedding ~ N(0,1); (H, W, 0, 0, H, W) in pixels
                 n_ids = 6
                 if self.te is None:
-                    self.text_embeds = torch.randn((n, cfg.projection_class_embeddings_input_dim - n_ids * cfg.addition_time_embed_dim),
-                                                   generator=gd)
+                    src["text_embeds"] = torch.randn((n, cfg.projection_class_embeddings_input_dim - n_ids * cfg.addition_time_embed_dim),
+                                                     generator=gd)
                 px = float(s * 8)
-                self.time_ids = torch.tensor([[px, px, 0.0, 0.0, px, px]]).repeat(n, 1)
-        self.gen = g
+                src["time_ids"] = torch.tensor([[px, px, 0.0, 0.0, px, px]]).repeat(n, 1)
+        return src
 
     def next_batch(self):
         idx = torch.randint(0, self.latents.shape[0], (self.bs,), generator=self.gen)
@@ -296,6 +348,27 @@ class Trainer:
             batch.append(added)
         return batch
 
+    def next_group_batches(self):
+        """One batch per data group, as `LoraTrainStep.step_groups` takes them."""
+        out = []
+        for (_, _, bs, _), src in zip(self.groups, self.sources):
+            idx = torch.randint(0, src["latents"].shape[0], (bs,), generator=self.gen)
+            lat, ehs = src["latents"][idx], src["ehs"][idx]
+            if self.cfg_doubled:
+                neg = src["ehs_neg"][idx] if src["ehs_neg"] is not None else torch.zeros_like(ehs)
+                ehs = torch.cat([neg, ehs], 0)
+            noise = torch.randn(lat.shape, generator=self.gen)
+            t = torch.randint(0, 1000, (bs,), generator=self.gen, dtype=torch.int64)
+            b = {"latents": lat, "noise": noise, "t": t, "ehs": ehs}
+            if self.text_time:
+                b["added_cond_kwargs"] = {"time_ids": src["time_ids"][idx]}
+                if src["text_embeds"] is not None:
+                    b["added_cond_kwargs"]["text_embeds"] = src["text_embeds"][idx]
+            if src["mask"] is not None:
+                b["mask"] = src["mask"][idx]
+            out.append(b)
+        return out
+
     def save(self, step: int):
         base_trained = any(p.requires_grad for n, p in self.unet.named_parameters() if "lora_block_" not in n)
         path = self.ckpt.save_model_with_lora(self.unet if base_trained else None, self.lora, "unet", step,
@@ -311,10 +384,13 @@ class Trainer:
         t0, seen = time.time(), 0
         for step in range(self.start_step + 1, steps + 1):
             for _ in range(self.accum):
-                loss = self.step_fn.step(*self.next_batch())
+                if self.groups is None:
+                    loss = self.step_fn.step(*self.next_batch())
+                else:                                            # the reference logs the last group's weighted loss
+                    loss = self.step_fn.step_groups(self.next_group_batches())[-1]
             if self.sched_step is not None:
                 self.sched_step()
-            seen += self.bs * self.world * self.accum
+            seen += self.bs * self.world * self.accum            # self.bs: every group's images of one micro-step
             if step % log_step == 0 or step == steps:
                 val = float(loss.cpu())
                 if self.rank == 0:

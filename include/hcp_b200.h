@@ -402,6 +402,19 @@ int hcp_adafactor_flat(float* p, const float* g, float* state, float* exp_avg, f
 int hcp_snr_mse_loss(const float* pred, const float* target, const int64_t* t, const float* alphas_cumprod, float gamma, int32_t mode,
                      int64_t per_image, int64_t n, float grad_scale, float* loss_sum /* += */, float* dpred /* may be NULL */,
                      hcp_stream_t stream);
+/* The eps loss over the data groups of one step (reference train_ac.py:467-482, get_loss :506-515 with its per-pixel mask):
+ *   group_loss[g] += sum_{b: sample_group[b] == g} sample_scale[b] * sum_{c,p} w(t_b) mask[b,p] (pred - target)^2
+ *   dpred = 2 w(t_b) mask[b,p] (pred - target) sample_scale[b] grad_scale
+ * pred / target / dpred fp32 [B, C, HW]; mask fp32 [B, HW] broadcast over channels (NULL = ones); sample_scale fp32 [B] =
+ * loss_weight_g / (B_g C HW) (mean over all elements, not over the mask); sample_group int32 [B] in [0, ngroups); mode -1 plain
+ * MSE (t / alphas_cumprod unused, may be NULL), 0..3 the weights of hcp_snr_mse_loss.  All tables are in device memory (CUDA-graph
+ * capturable).  workspace: hcp_eps_loss_grouped_workspace_bytes(B, C * HW) bytes of block partials, summed per group in a fixed
+ * order by a second launch, so repeated calls give bit-identical losses. */
+size_t hcp_eps_loss_grouped_workspace_bytes(int64_t B, int64_t per_image);
+int hcp_eps_loss_grouped(const float* pred, const float* target, const int64_t* t, const float* alphas_cumprod, const float* mask,
+                         const float* sample_scale, const int32_t* sample_group, int32_t ngroups, int32_t mode, float gamma, int64_t B,
+                         int64_t C, int64_t HW, float grad_scale, float* group_loss /* fp32 [ngroups], += */, float* dpred /* may be NULL */,
+                         void* workspace, size_t workspace_bytes, hcp_stream_t stream);
 /* ModelEMA.update on a flat fp32 buffer (reference hcpdiff/utils/ema.py:18-27): decay = clip(1 - (1 + step/inv_gamma)^-power, 0,
  * decay_max), ema = lerp(ema, p, 1 - decay); `step_device` is the optimizer's device-side step counter (already incremented). */
 int hcp_ema_flat(float* ema, const float* p, int64_t n, const int* step_device, float decay_max, float inv_gamma, float power,
