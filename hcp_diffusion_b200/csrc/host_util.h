@@ -45,6 +45,12 @@ struct ConvTap {
 };
 ConvTap conv_tap(int kh, int kw, int stride, int64_t C);
 
+// true when every pointer is 16-byte aligned (NULL counts as aligned): the elementwise kernels load and store uint4 / float4
+template <typename... P>
+inline bool aligned16(const P*... p) {
+    return ((((uintptr_t)p) | ... | (uintptr_t)0) & 15) == 0;
+}
+
 // Launch with programmatic stream serialization (PDL): the kernel may start while its predecessor on the stream drains; every
 // kernel of the library calls pdl_wait() (common.cuh) before touching global memory.  HCP_PDL=0 turns the attribute off.
 bool pdl_enabled();

@@ -169,20 +169,22 @@ __global__ void skinny_linear_kernel(const float* __restrict__ x, const __nv_bfl
 }
 
 // ---------------------------------------------------------------------------------------------
-// fp32 -> bf16 cast (weights once, encoder_hidden_states per step)
+// fp32 -> bf16 cast (weights once, encoder_hidden_states per step); four elements per thread, 16-byte loads when VEC (x 16-byte
+// and y 8-byte aligned), element by element otherwise (a user tensor or a slice of one may start anywhere)
 // ---------------------------------------------------------------------------------------------
+template <bool VEC>
 __global__ void cast_f32_bf16_kernel(const float* __restrict__ x, int64_t n, __nv_bfloat16* __restrict__ y) {
     pdl_trigger();
     pdl_wait();
     const int64_t i = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) * 4;
-    if (i + 3 < n) {
+    if (VEC && i + 3 < n) {
         const float4 v = *reinterpret_cast<const float4*>(x + i);
         uint2 o;
         o.x = pack_bf16x2(v.x, v.y);
         o.y = pack_bf16x2(v.z, v.w);
         *reinterpret_cast<uint2*>(y + i) = o;
     } else {
-        for (int64_t j = i; j < n; ++j) y[j] = __float2bfloat16(x[j]);
+        for (int64_t j = i; j < n && j < i + 4; ++j) y[j] = __float2bfloat16(x[j]);
     }
 }
 
@@ -560,9 +562,14 @@ extern "C" int hcp_skinny_linear(const float* x, const void* w_bf16, const float
 
 extern "C" int hcp_cast_f32_to_bf16(const float* x, int64_t n, void* y, hcp_stream_t st) {
     if (!x || !y) return set_error(HCP_ERR_INVALID, "cast: null pointer");
+    if (n < 0) return set_error(HCP_ERR_INVALID, "cast: negative size");
     if (n == 0) return HCP_OK;
     const int64_t threads = (n + 3) / 4;
-    launch_k(cast_f32_bf16_kernel, dim3((unsigned)((threads + 255) / 256)), dim3(256), 0, (cudaStream_t)st, x, n, (__nv_bfloat16*)y);
+    const dim3 grid((unsigned)((threads + 255) / 256));
+    if ((((uintptr_t)x & 15) | ((uintptr_t)y & 7)) == 0)
+        launch_k(cast_f32_bf16_kernel<true>, grid, dim3(256), 0, (cudaStream_t)st, x, n, (__nv_bfloat16*)y);
+    else
+        launch_k(cast_f32_bf16_kernel<false>, grid, dim3(256), 0, (cudaStream_t)st, x, n, (__nv_bfloat16*)y);
     LAUNCH_CHECK("cast launch");
     return HCP_OK;
 }
@@ -605,6 +612,8 @@ extern "C" int hcp_lora_pack_conv(const hcp_lora_conv_job* jobs_device, int64_t 
 extern "C" int hcp_mse_loss(const float* pred, const float* target, int64_t n, float grad_scale, float* loss_sum, float* dpred,
                             hcp_stream_t st) {
     if (!pred || !target || !loss_sum) return set_error(HCP_ERR_INVALID, "mse_loss: null pointer");
+    if (n < 0) return set_error(HCP_ERR_INVALID, "mse_loss: negative size");
+    if (n == 0) return HCP_OK;
     int blocks = (int)((n + 255) / 256);
     if (blocks > 592) blocks = 592;
     launch_k(mse_loss_kernel, dim3(blocks), dim3(256), 0, (cudaStream_t)st, pred, target, n, grad_scale, loss_sum, dpred);
@@ -615,7 +624,9 @@ extern "C" int hcp_mse_loss(const float* pred, const float* target, int64_t n, f
 extern "C" int hcp_add_noise(const float* x0, const float* noise, const int64_t* t, const float* alphas_cumprod, int64_t B,
                              int64_t per_image, float* xt, hcp_stream_t st) {
     if (!x0 || !noise || !t || !alphas_cumprod || !xt) return set_error(HCP_ERR_INVALID, "add_noise: null pointer");
+    if (B < 0 || per_image < 0) return set_error(HCP_ERR_INVALID, "add_noise: negative size");
     const int64_t n = B * per_image;
+    if (n == 0) return HCP_OK;
     launch_k(add_noise_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, (cudaStream_t)st, x0, noise, t, alphas_cumprod, per_image, n, xt);
     LAUNCH_CHECK("add_noise launch");
     return HCP_OK;
@@ -623,6 +634,8 @@ extern "C" int hcp_add_noise(const float* x0, const float* noise, const int64_t*
 
 extern "C" int hcp_sumsq(const float* g, int64_t n, float* out, hcp_stream_t st) {
     if (!g || !out) return set_error(HCP_ERR_INVALID, "sumsq: null pointer");
+    if (n < 0) return set_error(HCP_ERR_INVALID, "sumsq: negative size");
+    if (n == 0) return HCP_OK;
     int blocks = (int)((n + 255) / 256);
     if (blocks > 592) blocks = 592;
     launch_k(sumsq_kernel, dim3(blocks), dim3(256), 0, (cudaStream_t)st, g, n, out);
@@ -634,6 +647,8 @@ extern "C" int hcp_adamw_flat(float* p, const float* g, float* m, float* v, int6
                               float eps, float weight_decay, float grad_scale, const float* sumsq_device, float max_norm,
                               int* step_device, hcp_stream_t st) {
     if (!p || !g || !m || !v || !lr_device || !step_device) return set_error(HCP_ERR_INVALID, "adamw: null pointer");
+    if (n < 0) return set_error(HCP_ERR_INVALID, "adamw: negative size");
+    if (n == 0) return HCP_OK;
     launch_k(incr_step_kernel, dim3(1), dim3(1), 0, (cudaStream_t)st, step_device);
     launch_k(adamw_flat_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, (cudaStream_t)st, p, g, m, v, n, lr_device, beta1, beta2, eps, weight_decay,
                                                                                grad_scale, sumsq_device, max_norm, step_device);
@@ -644,11 +659,13 @@ extern "C" int hcp_adamw_flat(float* p, const float* g, float* m, float* v, int6
 extern "C" int hcp_adamw_flat_dev(float* p, const float* g, float* m, float* v, int64_t n, const float* hyper_device, float grad_scale,
                                   const float* sumsq_device, float max_norm, int* step_device, hcp_stream_t st) {
     if (!p || !g || !m || !v || !hyper_device || !step_device) return set_error(HCP_ERR_INVALID, "adamw_dev: null pointer");
-    launch_k(incr_step_kernel, dim3(1), dim3(1), 0, (cudaStream_t)st, step_device);
+    if (n < 0) return set_error(HCP_ERR_INVALID, "adamw_dev: negative size");
     if (((uintptr_t)p | (uintptr_t)g | (uintptr_t)m | (uintptr_t)v) & 15) return set_error(HCP_ERR_INVALID, "adamw_dev: buffers must be 16-byte aligned");
+    if (n == 0) return HCP_OK;
     int64_t blocks = ((n >> 2) + 255) / 256;
     if (blocks > num_sms() * 16) blocks = num_sms() * 16;
     if (blocks < 1) blocks = 1;
+    launch_k(incr_step_kernel, dim3(1), dim3(1), 0, (cudaStream_t)st, step_device);
     launch_k(adamw_flat_dev_kernel, dim3((unsigned)blocks), dim3(256), 0, (cudaStream_t)st, p, g, m, v, n, hyper_device, grad_scale,
              sumsq_device, max_norm, step_device);
     LAUNCH_CHECK("adamw_dev launch");

@@ -18,9 +18,12 @@ __device__ __forceinline__ float silu_grad(float z) {
     const float s = 1.f / (1.f + __expf(-z));
     return s * (1.f + z * (1.f - s));
 }
-__device__ __forceinline__ float gelu_f(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752f)); }
+// Phi(x) = erfc(-x / sqrt 2) / 2: 1 + erf(x / sqrt 2) cancels below x ~ -3 (fp32 erf rounds to -1 from x ~ -5.9 on), erfc keeps
+// the lower tail's relative accuracy.  erfcf takes more registers than erff: the GEGLU / GELU kernels cap them at 40 (six
+// 256-thread blocks per SM, no spills) so that these HBM-bound kernels keep their occupancy
+__device__ __forceinline__ float gelu_f(float x) { return 0.5f * x * erfcf(x * -0.70710678118654752f); }
 __device__ __forceinline__ float gelu_grad(float x) {
-    const float cdf = 0.5f * (1.f + erff(x * 0.70710678118654752f));
+    const float cdf = 0.5f * erfcf(x * -0.70710678118654752f);
     const float pdf = 0.3989422804014327f * __expf(-0.5f * x * x);
     return cdf + x * pdf;
 }
@@ -885,7 +888,7 @@ static void launch_layernorm(const __nv_bfloat16* x, const __nv_bfloat16* dy, co
 // =============================================================================================
 // GEGLU: u = [a | g] (each F wide);  h = a * gelu(g)
 // =============================================================================================
-__global__ void geglu_fwd_kernel(const __nv_bfloat16* __restrict__ u, int64_t M, int F, __nv_bfloat16* __restrict__ h) {
+__global__ void __launch_bounds__(256, 6) geglu_fwd_kernel(const __nv_bfloat16* __restrict__ u, int64_t M, int F, __nv_bfloat16* __restrict__ h) {
     pdl_trigger();
     pdl_wait();
     const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;   // one thread per 8 outputs
@@ -904,7 +907,7 @@ __global__ void geglu_fwd_kernel(const __nv_bfloat16* __restrict__ u, int64_t M,
     }
     *reinterpret_cast<uint4*>(h + m * F + c) = make_uint4(o[0], o[1], o[2], o[3]);
 }
-__global__ void geglu_bwd_kernel(const __nv_bfloat16* __restrict__ u, const __nv_bfloat16* __restrict__ dh, int64_t M, int F,
+__global__ void __launch_bounds__(256, 6) geglu_bwd_kernel(const __nv_bfloat16* __restrict__ u, const __nv_bfloat16* __restrict__ dh, int64_t M, int F,
                                  __nv_bfloat16* __restrict__ du) {
     pdl_trigger();
     pdl_wait();
@@ -970,7 +973,7 @@ __global__ void quick_gelu_bwd_kernel(const __nv_bfloat16* __restrict__ x, const
 // exact GELU (OpenCLIP-bigG MLP, transformers hidden_act='gelu'): y = 0.5 x (1 + erf(x / sqrt 2));
 // dx = dy * (Phi(x) + x phi(x))  -- gelu_f / gelu_grad, the same functions GEGLU uses
 // =============================================================================================
-__global__ void gelu_fwd_kernel(const __nv_bfloat16* __restrict__ x, int64_t n8, __nv_bfloat16* __restrict__ y) {
+__global__ void __launch_bounds__(256, 6) gelu_fwd_kernel(const __nv_bfloat16* __restrict__ x, int64_t n8, __nv_bfloat16* __restrict__ y) {
     pdl_trigger();
     pdl_wait();
     const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;   // one thread per 8 elements
@@ -985,7 +988,7 @@ __global__ void gelu_fwd_kernel(const __nv_bfloat16* __restrict__ x, int64_t n8,
     }
     reinterpret_cast<uint4*>(y)[i] = make_uint4(o[0], o[1], o[2], o[3]);
 }
-__global__ void gelu_bwd_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ dy, int64_t n8,
+__global__ void __launch_bounds__(256, 6) gelu_bwd_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ dy, int64_t n8,
                                 __nv_bfloat16* __restrict__ dx) {
     pdl_trigger();
     pdl_wait();
@@ -1227,62 +1230,73 @@ extern "C" int hcp_layernorm_bwd_bf16(const void* x, const void* dy, const void*
 }
 
 extern "C" int hcp_geglu_fwd_bf16(const void* u, int64_t M, int64_t F, void* h, hcp_stream_t stream_) {
-    if (!u || !h || F % 8 != 0) return set_error(HCP_ERR_INVALID, "geglu_fwd");
+    if (!u || !h || M < 0 || F < 0 || F % 8 != 0) return set_error(HCP_ERR_INVALID, "geglu_fwd");
     const int64_t n = M * (F / 8);
+    if (n == 0) return HCP_OK;
+    if (!aligned16(u, h)) return set_error(HCP_ERR_INVALID, "geglu_fwd: buffers must be 16-byte aligned");
     launch_k(geglu_fwd_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, (cudaStream_t)stream_, (const __nv_bfloat16*)u, M, (int)F, (__nv_bfloat16*)h);
     LAUNCH_CHECK("geglu_fwd launch");
     return HCP_OK;
 }
 extern "C" int hcp_geglu_bwd_bf16(const void* u, const void* dh, int64_t M, int64_t F, void* du, hcp_stream_t stream_) {
-    if (!u || !dh || !du || F % 8 != 0) return set_error(HCP_ERR_INVALID, "geglu_bwd");
+    if (!u || !dh || !du || M < 0 || F < 0 || F % 8 != 0) return set_error(HCP_ERR_INVALID, "geglu_bwd");
     const int64_t n = M * (F / 8);
+    if (n == 0) return HCP_OK;
+    if (!aligned16(u, dh, du)) return set_error(HCP_ERR_INVALID, "geglu_bwd: buffers must be 16-byte aligned");
     launch_k(geglu_bwd_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, (cudaStream_t)stream_, (const __nv_bfloat16*)u, (const __nv_bfloat16*)dh, M,
                                                                                    (int)F, (__nv_bfloat16*)du);
     LAUNCH_CHECK("geglu_bwd launch");
     return HCP_OK;
 }
 extern "C" int hcp_quick_gelu_fwd_bf16(const void* x, int64_t M, int64_t F, void* y, hcp_stream_t stream_) {
-    if (!x || !y || M < 0 || F % 8 != 0) return set_error(HCP_ERR_INVALID, "quick_gelu_fwd");
+    if (!x || !y || M < 0 || F < 0 || F % 8 != 0) return set_error(HCP_ERR_INVALID, "quick_gelu_fwd");
     const int64_t n8 = M * (F / 8);
     if (n8 == 0) return HCP_OK;
+    if (!aligned16(x, y)) return set_error(HCP_ERR_INVALID, "quick_gelu_fwd: buffers must be 16-byte aligned");
     launch_k(quick_gelu_fwd_kernel, dim3((unsigned)((n8 + 255) / 256)), dim3(256), 0, (cudaStream_t)stream_, (const __nv_bfloat16*)x, n8,
              (__nv_bfloat16*)y);
     LAUNCH_CHECK("quick_gelu_fwd launch");
     return HCP_OK;
 }
 extern "C" int hcp_quick_gelu_bwd_bf16(const void* x, const void* dy, int64_t M, int64_t F, void* dx, hcp_stream_t stream_) {
-    if (!x || !dy || !dx || M < 0 || F % 8 != 0) return set_error(HCP_ERR_INVALID, "quick_gelu_bwd");
+    if (!x || !dy || !dx || M < 0 || F < 0 || F % 8 != 0) return set_error(HCP_ERR_INVALID, "quick_gelu_bwd");
     const int64_t n8 = M * (F / 8);
     if (n8 == 0) return HCP_OK;
+    if (!aligned16(x, dy, dx)) return set_error(HCP_ERR_INVALID, "quick_gelu_bwd: buffers must be 16-byte aligned");
     launch_k(quick_gelu_bwd_kernel, dim3((unsigned)((n8 + 255) / 256)), dim3(256), 0, (cudaStream_t)stream_, (const __nv_bfloat16*)x,
              (const __nv_bfloat16*)dy, n8, (__nv_bfloat16*)dx);
     LAUNCH_CHECK("quick_gelu_bwd launch");
     return HCP_OK;
 }
 extern "C" int hcp_gelu_fwd_bf16(const void* x, int64_t M, int64_t F, void* y, hcp_stream_t stream_) {
-    if (!x || !y || M < 0 || F % 8 != 0) return set_error(HCP_ERR_INVALID, "gelu_fwd");
+    if (!x || !y || M < 0 || F < 0 || F % 8 != 0) return set_error(HCP_ERR_INVALID, "gelu_fwd");
     const int64_t n8 = M * (F / 8);
     if (n8 == 0) return HCP_OK;
+    if (!aligned16(x, y)) return set_error(HCP_ERR_INVALID, "gelu_fwd: buffers must be 16-byte aligned");
     launch_k(gelu_fwd_kernel, dim3((unsigned)((n8 + 255) / 256)), dim3(256), 0, (cudaStream_t)stream_, (const __nv_bfloat16*)x, n8,
              (__nv_bfloat16*)y);
     LAUNCH_CHECK("gelu_fwd launch");
     return HCP_OK;
 }
 extern "C" int hcp_gelu_bwd_bf16(const void* x, const void* dy, int64_t M, int64_t F, void* dx, hcp_stream_t stream_) {
-    if (!x || !dy || !dx || M < 0 || F % 8 != 0) return set_error(HCP_ERR_INVALID, "gelu_bwd");
+    if (!x || !dy || !dx || M < 0 || F < 0 || F % 8 != 0) return set_error(HCP_ERR_INVALID, "gelu_bwd");
     const int64_t n8 = M * (F / 8);
     if (n8 == 0) return HCP_OK;
+    if (!aligned16(x, dy, dx)) return set_error(HCP_ERR_INVALID, "gelu_bwd: buffers must be 16-byte aligned");
     launch_k(gelu_bwd_kernel, dim3((unsigned)((n8 + 255) / 256)), dim3(256), 0, (cudaStream_t)stream_, (const __nv_bfloat16*)x,
              (const __nv_bfloat16*)dy, n8, (__nv_bfloat16*)dx);
     LAUNCH_CHECK("gelu_bwd launch");
     return HCP_OK;
 }
 extern "C" int hcp_sum_bf16_to_f32(const void* const* srcs, int64_t nsrc, int64_t n, float* out, hcp_stream_t stream_) {
-    if (!srcs || !out || nsrc <= 0 || n % 8 != 0) return set_error(HCP_ERR_INVALID, "sum_bf16_to_f32: need sources and n % 8 == 0");
+    if (!srcs || !out || nsrc <= 0 || n < 0 || n % 8 != 0) return set_error(HCP_ERR_INVALID, "sum_bf16_to_f32: need sources and n % 8 == 0");
     for (int64_t k = 0; k < nsrc; ++k)
         if (!srcs[k]) return set_error(HCP_ERR_INVALID, "sum_bf16_to_f32: null source");
     const int64_t n8 = n / 8;
     if (n8 == 0) return HCP_OK;
+    if (!aligned16(out)) return set_error(HCP_ERR_INVALID, "sum_bf16_to_f32: buffers must be 16-byte aligned");
+    for (int64_t k = 0; k < nsrc; ++k)
+        if (!aligned16(srcs[k])) return set_error(HCP_ERR_INVALID, "sum_bf16_to_f32: buffers must be 16-byte aligned");
     for (int64_t k0 = 0; k0 < nsrc; k0 += kSumSrcs) {
         SumSrcs s;
         memset(&s, 0, sizeof(s));
@@ -1306,24 +1320,30 @@ extern "C" int hcp_embed_gather_bf16(const int64_t* ids, const int64_t* pos_ids,
     return HCP_OK;
 }
 extern "C" int hcp_upsample2x_fwd_bf16(const void* x, int64_t B, int64_t H, int64_t W, int64_t C, void* y, hcp_stream_t stream_) {
-    if (!x || !y || C % 8 != 0) return set_error(HCP_ERR_INVALID, "upsample2x_fwd");
+    if (!x || !y || B < 0 || H < 0 || W < 0 || C < 0 || C % 8 != 0) return set_error(HCP_ERR_INVALID, "upsample2x_fwd");
     const int64_t n = B * 4 * H * W * (C / 8);
+    if (n == 0) return HCP_OK;
+    if (!aligned16(x, y)) return set_error(HCP_ERR_INVALID, "upsample2x_fwd: buffers must be 16-byte aligned");
     launch_k(upsample2x_fwd_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, (cudaStream_t)stream_, (const __nv_bfloat16*)x, (int)B, (int)H, (int)W,
                                                                                         (int)C, (__nv_bfloat16*)y);
     LAUNCH_CHECK("upsample2x_fwd launch");
     return HCP_OK;
 }
 extern "C" int hcp_upsample2x_bwd_bf16(const void* dy, int64_t B, int64_t H, int64_t W, int64_t C, void* dx, hcp_stream_t stream_) {
-    if (!dy || !dx || C % 8 != 0) return set_error(HCP_ERR_INVALID, "upsample2x_bwd");
+    if (!dy || !dx || B < 0 || H < 0 || W < 0 || C < 0 || C % 8 != 0) return set_error(HCP_ERR_INVALID, "upsample2x_bwd");
     const int64_t n = B * H * W * (C / 8);
+    if (n == 0) return HCP_OK;
+    if (!aligned16(dy, dx)) return set_error(HCP_ERR_INVALID, "upsample2x_bwd: buffers must be 16-byte aligned");
     launch_k(upsample2x_bwd_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, (cudaStream_t)stream_, (const __nv_bfloat16*)dy, (int)B, (int)H, (int)W,
                                                                                         (int)C, (__nv_bfloat16*)dx);
     LAUNCH_CHECK("upsample2x_bwd launch");
     return HCP_OK;
 }
 extern "C" int hcp_add_bf16(const void* a, const void* b, int64_t n, void* out, hcp_stream_t stream_) {
-    if (!a || !b || !out || n % 8 != 0) return set_error(HCP_ERR_INVALID, "add_bf16");
+    if (!a || !b || !out || n < 0 || n % 8 != 0) return set_error(HCP_ERR_INVALID, "add_bf16");
     const int64_t n8 = n / 8;
+    if (n8 == 0) return HCP_OK;
+    if (!aligned16(a, b, out)) return set_error(HCP_ERR_INVALID, "add_bf16: buffers must be 16-byte aligned");
     launch_k(add_bf16_kernel, dim3((unsigned)((n8 + 255) / 256)), dim3(256), 0, (cudaStream_t)stream_, (const __nv_bfloat16*)a, (const __nv_bfloat16*)b, n8,
                                                                                    (__nv_bfloat16*)out);
     LAUNCH_CHECK("add_bf16 launch");

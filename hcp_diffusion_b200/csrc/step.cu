@@ -328,6 +328,8 @@ extern "C" int hcp_dropout_bf16(const void* x, int64_t ldx, const void* residual
     if (rows <= 0 || ncols <= 0 || (ncols % 8) || (ldx % 8) || (ldo % 8) || (residual && (ldr % 8)) || !(p >= 0.f && p < 1.f) ||
         (rowbias && (rows_per_group <= 0 || (rowbias_ld % 4))))
         return set_error(HCP_ERR_INVALID, "dropout: shape (columns and pitches in multiples of 8, 0 <= p < 1)");
+    if (!aligned16(x, residual, rowbias, out))
+        return set_error(HCP_ERR_INVALID, "dropout: buffers must be 16-byte aligned");
     const int64_t n = rows * (ncols / 8);
     launch_k(dropout_bf16_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, (cudaStream_t)st, (const __nv_bfloat16*)x, ldx,
              (const __nv_bfloat16*)residual, ldr, rowbias, rowbias_ld, rows_per_group, rows, (int)ncols, p, (const unsigned long long*)state_device, site, (__nv_bfloat16*)out, ldo);

@@ -13,7 +13,11 @@
  *     memory, never synchronises and only enqueues work on the `stream` argument (a cudaStream_t).
  *   - activations are bf16, row-major "NHWC": a [B,H,W,C] feature map is the same memory as the [B*H*W, C]
  *     token matrix the transformer blocks use.  Accumulation is fp32.  `ld*` are row pitches in ELEMENTS.
- *   - all device pointers must be 16-byte aligned, all row pitches multiples of 8 elements.
+ *   - all device pointers must be 16-byte aligned, all row pitches multiples of 8 elements.  The elementwise bf16 kernels (GEGLU,
+ *     GELU, quick-GELU, upsample, add, the bf16 sum, dropout) and hcp_adamw_flat_dev refuse a pointer off 16-byte alignment with
+ *     HCP_ERR_INVALID before any launch; hcp_cast_f32_to_bf16 takes an element-wise path for it instead.
+ *   - the elementwise and training-step kernels refuse a negative size with HCP_ERR_INVALID; an empty one (n, M or B == 0) returns
+ *     HCP_OK and launches nothing.  A refused call launches nothing and changes no device state (step counters included).
  */
 #ifndef HCP_B200_H_
 #define HCP_B200_H_
@@ -220,7 +224,7 @@ int hcp_quick_gelu_bwd_bf16(const void* x, const void* dy, int64_t M, int64_t F,
 
 /* exact GELU (transformers GELUActivation, hidden_act='gelu': the MLP of SDXL's second text encoder, OpenCLIP ViT-bigG/14): x, y, dy,
  * dx bf16 [M,F], F % 8 == 0;  y = 0.5 x (1 + erf(x / sqrt 2));  dx = dy * (Phi(x) + x phi(x)) from the saved pre-activation x.
- * fp32 arithmetic. */
+ * fp32 arithmetic, Phi(x) = erfc(-x / sqrt 2) / 2 (accurate in the lower tail, where 1 + erf cancels). */
 int hcp_gelu_fwd_bf16(const void* x, int64_t M, int64_t F, void* y, hcp_stream_t stream);
 int hcp_gelu_bwd_bf16(const void* x, const void* dy, int64_t M, int64_t F, void* dx, hcp_stream_t stream);
 
@@ -263,6 +267,7 @@ int hcp_conv_out_dgrad_f32(const float* dy_nchw, const float* w, int64_t B, int6
  * sinusoidal embedding (diffusers Timesteps: [cos | sin], freq = exp(-ln(1e4) * j / (K/2))).  W is bf16. */
 int hcp_skinny_linear(const float* x, const void* w_bf16, const float* bias, int64_t M, int64_t K, int64_t N, int in_mode,
                       int out_silu, float* y, hcp_stream_t stream);
+/* y bf16 [n] = x fp32 [n] rounded to nearest even; any alignment (16-byte x and 8-byte y take the vector path) */
 int hcp_cast_f32_to_bf16(const float* x, int64_t n, void* y, hcp_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
@@ -361,7 +366,9 @@ int hcp_adamw_flat(float* p, const float* g, float* m, float* v, int64_t n, cons
                    float eps, float weight_decay, float grad_scale, const float* sumsq_device, float max_norm,
                    int* step_device, hcp_stream_t stream);
 /* The same step with the hyper-parameters in device memory: hyper_device = {lr, beta1, beta2, eps, weight_decay} (fp32 [5]); an LR
- * scheduler (OneCycleLR cycles lr AND beta1) rewrites them between CUDA-graph replays. */
+ * scheduler (OneCycleLR cycles lr AND beta1) rewrites them between CUDA-graph replays.  p, g, m, v 16-byte aligned (a segment of a
+ * flat buffer starts at a multiple of 4 elements).  Both AdamW calls advance *step_device once per call with n > 0; n == 0 is a
+ * no-op and leaves it. */
 int hcp_adamw_flat_dev(float* p, const float* g, float* m, float* v, int64_t n, const float* hyper_device, float grad_scale,
                        const float* sumsq_device, float max_norm, int* step_device, hcp_stream_t stream);
 
