@@ -1,5 +1,6 @@
 // SPDX-License-Identifier: Apache-2.0
-// Adafactor (transformers.optimization.Adafactor.step) over the flat fp32 parameter buffer of the training step (sm_90a).
+// Adafactor (transformers.optimization.Adafactor.step) over the flat fp32 parameter buffer of the training step (sm_90a), and
+// Lion (lion_pytorch.Lion.step, one elementwise kernel at the end of this file).
 //
 // Every trainable tensor keeps its module shape: a tensor with two or more dims is factored over its LAST TWO dims, viewed as
 // [P, R, C] with the leading dims a batch (a Conv2d weight [O, I, 3, 3] is P = O*I slabs of 3 x 3); a 1-D tensor keeps an
@@ -284,6 +285,42 @@ __global__ void adafactor_incr_kernel(int* steps, int ngroups) {
     if ((int)threadIdx.x < ngroups) steps[threadIdx.x] += 1;
 }
 
+// Lion (lion_pytorch.Lion.step; Chen et al. 2023, Program 1) over one segment of the flat buffer, hyper = {lr, beta1, beta2, eps
+// (unused), weight_decay} as adamw_flat_dev_kernel reads it.  Per element, in this order and in fp32:
+//   p = p (1 - lr wd);  c = b1 m + (1 - b1) g;  p = p - lr sign(c)  (sign(0) = 0);  m = b2 m + (1 - b2) g
+// One moment, no bias correction: the step counter is only advanced (by block 0), for hcp_ema_flat.  Four elements per thread
+// and iteration (16-byte accesses: 20 B of traffic per element), the n % 4 tail in block 0.
+__global__ void __launch_bounds__(256) lion_flat_dev_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
+                                                            int64_t n, const float* __restrict__ hyper, float gscale,
+                                                            const float* __restrict__ sumsq, float max_norm, int* __restrict__ step_ptr) {
+    pdl_trigger();
+    pdl_wait();
+    if (blockIdx.x == 0 && threadIdx.x == 0) *step_ptr += 1;
+    const float gs = af_grad_scale(gscale, sumsq, max_norm);
+    const float lr = hyper[0], beta1 = hyper[1], beta2 = hyper[2], wd = hyper[4];
+    const float decay = __fsub_rn(1.f, __fmul_rn(lr, wd));      // 1 - lr * wd rounded twice, as lion-pytorch's fp32 tensors see it
+    auto upd = [&](float& w, float grad, float& mi) {
+        grad *= gs;
+        w *= decay;
+        const float c = beta1 * mi + (1.f - beta1) * grad;
+        w -= lr * (float)((c > 0.f) - (c < 0.f));
+        mi = beta2 * mi + (1.f - beta2) * grad;
+    };
+    const int64_t n4 = n >> 2, stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n4; i += stride) {
+        float4 w4 = reinterpret_cast<float4*>(p)[i], m4 = reinterpret_cast<float4*>(m)[i];
+        const float4 g4 = reinterpret_cast<const float4*>(g)[i];
+        upd(w4.x, g4.x, m4.x); upd(w4.y, g4.y, m4.y); upd(w4.z, g4.z, m4.z); upd(w4.w, g4.w, m4.w);
+        reinterpret_cast<float4*>(p)[i] = w4; reinterpret_cast<float4*>(m)[i] = m4;
+    }
+    if (blockIdx.x == 0 && threadIdx.x < (n & 3)) {
+        const int64_t i = (n4 << 2) + threadIdx.x;
+        float w = p[i], mi = m[i];
+        upd(w, g[i], mi);
+        p[i] = w; m[i] = mi;
+    }
+}
+
 }  // namespace hcp
 
 using namespace hcp;
@@ -309,5 +346,20 @@ extern "C" int hcp_adafactor_flat(float* p, const float* g, float* state, float*
     launch_k(adafactor_apply_kernel, dim3((unsigned)nitems), dim3(AF_T), 0, s, p, g, (const float*)state, exp_avg, (const float*)work,
              tensors_device, items_device, (int)nitems, hyper_device, (const int*)steps_device, grad_scale, sumsq_device, max_norm);
     LAUNCH_CHECK("adafactor launch");
+    return HCP_OK;
+}
+
+extern "C" int hcp_lion_flat_dev(float* p, const float* g, float* m, int64_t n, const float* hyper_device, float grad_scale,
+                                 const float* sumsq_device, float max_norm, int* step_device, hcp_stream_t st) {
+    if (!p || !g || !m || !hyper_device || !step_device) return set_error(HCP_ERR_INVALID, "lion_dev: null pointer");
+    if (n < 0) return set_error(HCP_ERR_INVALID, "lion_dev: negative size");
+    if (((uintptr_t)p | (uintptr_t)g | (uintptr_t)m) & 15) return set_error(HCP_ERR_INVALID, "lion_dev: buffers must be 16-byte aligned");
+    if (n == 0) return HCP_OK;
+    int64_t blocks = ((n >> 2) + 255) / 256;
+    if (blocks > num_sms() * 16) blocks = num_sms() * 16;
+    if (blocks < 1) blocks = 1;
+    launch_k(lion_flat_dev_kernel, dim3((unsigned)blocks), dim3(256), 0, (cudaStream_t)st, p, g, m, n, hyper_device, grad_scale,
+             sumsq_device, max_norm, step_device);
+    LAUNCH_CHECK("lion_dev launch");
     return HCP_OK;
 }

@@ -163,7 +163,8 @@ class _CfgMixFn(torch.autograd.Function):
 
 
 class LoraTrainStep:
-    """One optimisation step of LoRA (or full) training on a `UNet2DConditionModel`: eps-prediction loss, grad-norm clip, AdamW.
+    """One optimisation step of LoRA (or full) training on a `UNet2DConditionModel`: eps-prediction loss, grad-norm clip, AdamW
+    (or Adafactor, or Lion).
 
     `params`: parameters, or optimizer-style groups [{'params': [...], 'lr': ..., 'weight_decay': ...}] (one per `lora_unet:` /
     `unet:` config item, reference cfg_net_tools.py:96-127).  `grad_accum_steps`: micro-batches per optimizer step
@@ -172,10 +173,11 @@ class LoraTrainStep:
     `train.cfg_scale` string / (lo, hi, fn) for DreamArtist training: the UNet then runs on the doubled batch
     [latents | latents] against a text embedding of 2B rows [negative | positive].
 
-    `optimizer`: 'adamw' (torch.optim.AdamW with `lr`, `betas`, `eps`, `weight_decay`) or 'adafactor'
-    (transformers.optimization.Adafactor; `optimizer_kwargs` takes its constructor keys with its defaults -- `lr`, `eps`,
-    `clip_threshold`, `decay_rate`, `beta1`, `weight_decay`, `scale_parameter`, `relative_step`, `warmup_init` -- and a group's own
-    'lr' / 'weight_decay' win over them).  Adafactor keeps factored second moments per tensor of the module's shape (state sized by
+    `optimizer`: 'adamw' (torch.optim.AdamW with `lr`, `betas`, `eps`, `weight_decay`; betas / weight_decay default to
+    (0.9, 0.999) / 1e-2), 'lion' (lion_pytorch.Lion with `lr`, `betas`, `weight_decay`, defaults (0.9, 0.99) / 0.0: one flat
+    momentum buffer, half of AdamW's state) or 'adafactor' (transformers.optimization.Adafactor; `optimizer_kwargs` takes its
+    constructor keys with its defaults -- `lr`, `eps`, `clip_threshold`, `decay_rate`, `beta1`, `weight_decay`, `scale_parameter`,
+    `relative_step`, `warmup_init` -- and a group's own 'lr' / 'weight_decay' win over them).  Adafactor keeps factored second moments per tensor of the module's shape (state sized by
     adafactor.state_numel), plus one flat first-moment buffer only when `beta1` is set.
 
     `text_encoder`: a `models.CLIPTextModel` whose LoRA adapters train together with the UNet's (the reference's `lora_text_encoder`,
@@ -189,8 +191,8 @@ class LoraTrainStep:
     `loss_weights`: one weight per data group of `step_groups()` (the reference's per-dataset `loss_weight`, e.g. DreamBooth's
     prior-preservation class set); None weighs every group 1.0."""
 
-    def __init__(self, unet: nn.Module, params: Union[Iterable[nn.Parameter], Sequence[dict]], lr: float = 1e-4, betas=(0.9, 0.999),
-                 eps: float = 1e-8, weight_decay: float = 1e-2, max_grad_norm: float = 1.0, use_cuda_graph: bool = True,
+    def __init__(self, unet: nn.Module, params: Union[Iterable[nn.Parameter], Sequence[dict]], lr: float = 1e-4, betas=None,
+                 eps: float = 1e-8, weight_decay: Optional[float] = None, max_grad_norm: float = 1.0, use_cuda_graph: bool = True,
                  process_group: Optional[dist.ProcessGroup] = None, side_stream: bool = True, grad_accum_steps: int = 1,
                  loss: Union[None, str, dict] = None, ema: Optional[dict] = None, cfg_scale=None, num_train_timesteps: int = 1000,
                  optimizer: str = "adamw", optimizer_kwargs: Optional[dict] = None, text_encoder: Optional[nn.Module] = None,
@@ -218,9 +220,12 @@ class LoraTrainStep:
                     "SDXL with n_repeats > 1 (tokenizer_repeats) is not supported: the reference pools bigG's text_embeds at the "
                     "largest id of the raw tokenizer output before it is cut into 77-token chunks, which pre-chunked ids cannot "
                     "express (the reference's SDXL config uses tokenizer_repeats: 1)")
-        if optimizer not in ("adamw", "adafactor"):
-            raise ValueError(f"optimizer {optimizer!r}: one of 'adamw', 'adafactor'")
+        if optimizer not in ("adamw", "adafactor", "lion"):
+            raise ValueError(f"optimizer {optimizer!r}: one of 'adamw', 'adafactor', 'lion'")
         self.optimizer = optimizer
+        default_betas, default_wd = ((0.9, 0.99), 0.0) if optimizer == "lion" else ((0.9, 0.999), 1e-2)
+        betas = default_betas if betas is None else tuple(betas)
+        weight_decay = default_wd if weight_decay is None else weight_decay
         af_opts = None
         if optimizer == "adafactor":
             af_opts = adafactor.check_options(optimizer_kwargs)
@@ -228,7 +233,7 @@ class LoraTrainStep:
             if af_opts["lr"] is not None:
                 lr = af_opts["lr"]
         elif optimizer_kwargs:
-            raise ValueError("optimizer_kwargs are the Adafactor options; AdamW takes lr / betas / eps / weight_decay")
+            raise ValueError("optimizer_kwargs are the Adafactor options; AdamW and Lion take lr / betas / weight_decay (AdamW also eps)")
         params = list(params)
         if params and isinstance(params[0], dict):
             groups = [{"params": list(g["params"]), "lr": float(g.get("lr", lr)), "weight_decay": float(g.get("weight_decay", weight_decay))}
@@ -252,7 +257,7 @@ class LoraTrainStep:
             self._init_adafactor(groups, af_opts)
         else:
             self.m = torch.zeros_like(self.flat.data)
-            self.v = torch.zeros_like(self.flat.data)
+            self.v = torch.zeros_like(self.flat.data) if optimizer == "adamw" else None
         # parameter groups = contiguous segments of the flat buffer, each with a device-side lr and step counter
         self.segments, i0 = [], 0
         for g in groups:
@@ -332,12 +337,12 @@ class LoraTrainStep:
         """Bytes of optimizer state (moments; not the parameters, gradients or scratch)."""
         if self.optimizer == "adafactor":
             return 4 * (self.af_state.numel() + (0 if self.af_exp_avg is None else self.af_exp_avg.numel()))
-        return 4 * (self.m.numel() + self.v.numel())
+        return 4 * sum(b.numel() for b in (self.m, self.v) if b is not None)
 
     def _opt_buffers(self) -> List[torch.Tensor]:
         if self.optimizer == "adafactor":
             return [self.af_state, self.af_steps] + ([] if self.af_exp_avg is None else [self.af_exp_avg])
-        return [self.m, self.v] + [s["step"] for s in self.segments]
+        return [b for b in (self.m, self.v) if b is not None] + [s["step"] for s in self.segments]
 
     def set_lr(self, lr: float, group: Optional[int] = None):
         """Set the lr of one group, or scale every group's configured lr by lr / base lr of group 0 (what an LR scheduler does)."""
@@ -349,13 +354,14 @@ class LoraTrainStep:
             s["lr"].fill_(s["base_lr"] * ratio)
 
     def set_hyper(self, group: int, lr: Optional[float] = None, beta1: Optional[float] = None):
-        """What an LR scheduler writes per step (OneCycleLR cycles the lr and, for Adam, beta1): device-side, graph-replay safe."""
+        """What an LR scheduler writes per step (OneCycleLR cycles the lr and, for AdamW and Lion, beta1): device-side, graph-replay
+        safe."""
         h = self.segments[group]["hyper"]
         if lr is not None:
             h[0:1].fill_(lr)
         if beta1 is not None:
-            if self.optimizer != "adamw":
-                raise ValueError("beta1 is scheduled for AdamW only")
+            if self.optimizer == "adafactor":
+                raise ValueError("beta1 is scheduled for AdamW and Lion only")
             h[1:2].fill_(beta1)
 
     def sync_params(self, src: int = 0):
@@ -431,11 +437,14 @@ class LoraTrainStep:
                  _lib.ptr(self.af_exp_avg), self.af_work.data_ptr(), self.af_tensors.data_ptr(), self.af_items.data_ptr(), lay.items.size,
                  _lib.ptr(self.af_factor_items), lay.factor_items.size, self.af_hyper.data_ptr(), self.af_steps.data_ptr(),
                  len(self.segments), 1.0 / self.world, self.gsq.data_ptr(), float(self.max_norm or 0.0), stream_ptr())
-        for s in (self.segments if self.optimizer == "adamw" else ()):
+        for s in (self.segments if self.optimizer != "adafactor" else ()):
             lo, cnt = s["lo"], s["hi"] - s["lo"]
-            call("hcp_adamw_flat_dev", self.flat.data.data_ptr() + 4 * lo, self.flat.grad.data_ptr() + 4 * lo, self.m.data_ptr() + 4 * lo,
-                 self.v.data_ptr() + 4 * lo, cnt, s["hyper"].data_ptr(), 1.0 / self.world, self.gsq.data_ptr(), float(self.max_norm or 0.0),
-                 s["step"].data_ptr(), stream_ptr())
+            p, g, m = (b.data_ptr() + 4 * lo for b in (self.flat.data, self.flat.grad, self.m))
+            tail = (1.0 / self.world, self.gsq.data_ptr(), float(self.max_norm or 0.0), s["step"].data_ptr(), stream_ptr())
+            if self.optimizer == "lion":
+                call("hcp_lion_flat_dev", p, g, m, cnt, s["hyper"].data_ptr(), *tail)
+            else:
+                call("hcp_adamw_flat_dev", p, g, m, self.v.data_ptr() + 4 * lo, cnt, s["hyper"].data_ptr(), *tail)
         if self.ema is not None:
             call("hcp_ema_flat", self.ema.data_ptr(), self.flat.data.data_ptr(), n, self.step_count.data_ptr(), *self.ema_cfg, stream_ptr())
         self.flat.grad.zero_()                             # optimizer.zero_grad() (reference train_ac.py:494)

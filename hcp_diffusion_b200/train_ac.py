@@ -5,8 +5,10 @@ the hot path: build the UNet (cfg `model.unet`, the reference's injection seam t
 training) and `lora_unet:` lists through `make_hcpdiff` (train_ac.py:324-359), then run `train.train_steps` optimizer steps with
 the H100 engine and save `ckpts/unet-<step>.safetensors` every `train.save_step` in the reference checkpoint format
 (train_ac.py:523-544).  Honoured `train.*` keys: `gradient_accumulation_steps`, `max_grad_norm`, `scale_lr`, `optimizer.{lr,
-weight_decay, betas, eps}` for `torch.optim.AdamW` (the default `_target_`) or the constructor keys of
-`transformers.optimization.Adafactor` (reference cfgs/train/examples/FT_sdxl.yaml), `scheduler.{name, num_warmup_steps, num_training_steps, scheduler_kwargs}` (one_cycle / constant /
+weight_decay, betas, eps}` for `torch.optim.AdamW` (the default `_target_`), the constructor keys of
+`transformers.optimization.Adafactor` (reference cfgs/train/examples/FT_sdxl.yaml) or of `lion_pytorch.Lion` (`lr, betas,
+weight_decay`, reference cfgs/train/examples/Lion_optimizer.yaml; `use_triton` is accepted and changes nothing, since it only picks
+lion-pytorch's Triton kernel for the same arithmetic), `scheduler.{name, num_warmup_steps, num_training_steps, scheduler_kwargs}` (one_cycle / constant /
 constant_with_warmup), `loss.criterion` (`torch.nn.MSELoss` or `hcpdiff.loss.MinSNRLoss`-family `_target_` + `gamma`), `cfg_scale`
 (DreamArtist), `resume.{ckpt_path.unet, start_step}`; `model.ema` (`decay_max`, `inv_gamma`, `power`).
 
@@ -14,8 +16,8 @@ Text encoder (SD1.x CLIP): `lora_text_encoder` items train LoRA on it next to th
 `model.text_encoder` (instantiable, default CLIP-L) with weights from `model.text_encoder_init`, `model.clip_skip`,
 `model.clip_final_norm`, `model.tokenizer_repeats`; `ckpts/text_encoder-<step>` is saved next to `unet-<step>` and
 `resume.ckpt_path.TE` is loaded.  A `text_encoder:` full fine-tune list, a non-null `tokenizer_pt.train` and DreamArtist++ items in
-`lora_text_encoder` raise NotImplementedError.  The ids are given (no tokenizer): `data.path` holds 'input_ids' [N, 77 R], or
-synthetic prompts are BOS 49406, random tokens, EOS 49407 padding.  With an SDXL ('text_time') UNet the default text encoder is
+`lora_text_encoder` raise NotImplementedError (so `train.optimizer_pt`, the prompt-tuning optimizer, is never read).  The ids
+are given (no tokenizer): `data.path` holds 'input_ids' [N, 77 R], or synthetic prompts are BOS 49406, random tokens, EOS 49407 padding.  With an SDXL ('text_time') UNet the default text encoder is
 SDXL's pair (`models.SDXLTextEncoder`, CLIP-L + OpenCLIP-bigG, reference cfgs/train/examples/lora_sdxl.yaml): ids are [N, 2 x 77]
 (clip_B's chunk, then bigG's; synthetic bigG chunks carry the same words and are padded with id 0 after EOS, as SDXL's second
 tokenizer pads), `text_embeds` comes from the encoder and the data holds only 'time_ids'.
@@ -73,20 +75,37 @@ def loss_from_cfg(loss_cfg):
     raise NotImplementedError(f"train.loss.criterion {target!r} is not supported on the H100 hot path")
 
 
+# lion_pytorch.Lion.__init__ keywords and defaults (decoupled_weight_decay exists in newer releases)
+LION_DEFAULTS = {"lr": 1e-4, "betas": (0.9, 0.99), "weight_decay": 0.0, "use_triton": False, "decoupled_weight_decay": False}
+
+
 def optimizer_from_cfg(opt_cfg):
-    """`train.optimizer` -> (engine optimizer, Adafactor options or None).  No `_target_` or torch.optim.AdamW: AdamW from `lr /
+    """`train.optimizer` -> (engine optimizer, options or None).  No `_target_` or torch.optim.AdamW: AdamW from `lr /
     weight_decay / betas / eps`; transformers.optimization.Adafactor: its constructor keys with transformers' defaults (a manual
-    `lr` with `relative_step: True` is refused, as transformers refuses it)."""
+    `lr` with `relative_step: True` is refused, as transformers refuses it); lion_pytorch.Lion: {'lr', 'betas', 'weight_decay'}
+    with Lion's defaults (an unknown key is a TypeError, as Lion's constructor raises; `decoupled_weight_decay: True` is refused)."""
     target = str((opt_cfg or {}).get("_target_", "torch.optim.AdamW"))
     name = target.rsplit(".", 1)[-1]
     if name == "AdamW" and target.startswith("torch."):
         return "adamw", None
+    kw = {k: v for k, v in (opt_cfg or {}).items() if k not in ("_target_", "_partial_")}
     if name == "Adafactor" and target.startswith("transformers."):
-        kw = {k: v for k, v in opt_cfg.items() if k not in ("_target_", "_partial_")}
         if "eps" in kw:
             kw["eps"] = tuple(kw["eps"])
         return "adafactor", adafactor.check_options(kw)
-    raise NotImplementedError(f"train.optimizer._target_={target!r}: torch.optim.AdamW or transformers.optimization.Adafactor")
+    if name == "Lion" and target.startswith("lion_pytorch."):
+        unknown = sorted(set(kw) - set(LION_DEFAULTS))
+        if unknown:
+            raise TypeError(f"Lion.__init__() got unexpected keyword arguments {unknown}")
+        opts = {**LION_DEFAULTS, **kw}
+        if opts["decoupled_weight_decay"]:
+            raise NotImplementedError("lion_pytorch.Lion with decoupled_weight_decay: True is not supported")
+        betas = tuple(float(b) for b in opts["betas"])
+        if len(betas) != 2:
+            raise ValueError(f"Lion betas {opts['betas']!r}: two values (beta1, beta2)")
+        return "lion", {"lr": float(opts["lr"]), "betas": betas, "weight_decay": float(opts["weight_decay"])}
+    raise NotImplementedError(f"train.optimizer._target_={target!r}: torch.optim.AdamW, transformers.optimization.Adafactor or "
+                              "lion_pytorch.Lion")
 
 
 def data_groups(data_cfg):
@@ -126,15 +145,16 @@ class _LrOnly(torch.optim.Optimizer):
 
 def make_scheduler(cfg, step_fn: LoraTrainStep):
     """Reference get_scheduler_with_name (hcpdiff/utils/net_utils.py:22-82) driven on a stand-in optimizer with the engine's groups:
-    the real torch schedulers produce the numbers, `step()` copies lr (and OneCycleLR's cycled beta1) to the device."""
+    the real torch schedulers produce the numbers, `step()` copies lr (and OneCycleLR's cycled beta1) to the device.  AdamW and
+    Lion have `betas` (OneCycleLR cycles beta1 on both), so an AdamW stand-in with the engine's betas serves for either."""
     if not cfg or not cfg.get("name"):
         return None
     name = cfg["name"]
     warm, total = int(cfg.get("num_warmup_steps", 0)), int(cfg.get("num_training_steps", 1))
     kwargs = dict(cfg.get("scheduler_kwargs") or {})
     dummy = [torch.nn.Parameter(torch.zeros(1)) for _ in step_fn.segments]
-    adamw = step_fn.optimizer == "adamw"
-    if adamw:
+    has_betas = step_fn.optimizer != "adafactor"
+    if has_betas:
         opt = torch.optim.AdamW([{"params": [d], "lr": s["base_lr"]} for d, s in zip(dummy, step_fn.segments)], betas=tuple(step_fn.betas))
     else:                                       # Adafactor has no betas: OneCycleLR's cycle_momentum fails as it does in torch
         opt = _LrOnly([{"params": [d], "lr": s["base_lr"]} for d, s in zip(dummy, step_fn.segments)])
@@ -150,7 +170,7 @@ def make_scheduler(cfg, step_fn: LoraTrainStep):
 
     def push():
         for i, g in enumerate(opt.param_groups):
-            step_fn.set_hyper(i, lr=float(g["lr"]), beta1=float(g["betas"][0]) if adamw else None)
+            step_fn.set_hyper(i, lr=float(g["lr"]), beta1=float(g["betas"][0]) if has_betas else None)
 
     def step():
         opt.step()              # keeps torch's "optimizer.step() before lr_scheduler.step()" contract on the stand-in
@@ -197,7 +217,11 @@ class Trainer:
         accum = int(tr.get("gradient_accumulation_steps", 1))
         lr_scale = bs * self.world * accum if tr.get("scale_lr", False) else 1
         opt_cfg = tr.get("optimizer") or {}
-        opt_name, af_opts = optimizer_from_cfg(opt_cfg)
+        opt_name, opt_opts = optimizer_from_cfg(opt_cfg)
+        if opt_name == "lion":
+            betas, weight_decay = opt_opts["betas"], opt_opts["weight_decay"]
+        else:
+            betas, weight_decay = tuple(opt_cfg.get("betas", (0.9, 0.999))), float(opt_cfg.get("weight_decay", 1e-2))
         groups, self.lora = make_hcpdiff(self.unet, cfgs.get("unet"), cfgs.get("lora_unet"), default_lr=float(opt_cfg.get("lr", 1e-4)))
         groups = [{"params": g["params"], "lr": float(g["lr"]) * lr_scale} for g in groups if len(g["params"])]
         self.te, self.te_lora, te_opts = self._build_text_encoder(cfgs)
@@ -224,12 +248,11 @@ class Trainer:
         if ema_cfg:
             ema = {k: ema_cfg[k] for k in ("decay_max", "inv_gamma", "power") if k in ema_cfg}
         cfg_scale = tr.get("cfg_scale")
-        self.step_fn = LoraTrainStep(self.unet, groups, weight_decay=float(opt_cfg.get("weight_decay", 1e-2)),
-                                     betas=tuple(opt_cfg.get("betas", (0.9, 0.999))), eps=float(opt_cfg.get("eps", 1e-8)),
+        self.step_fn = LoraTrainStep(self.unet, groups, weight_decay=weight_decay, betas=betas, eps=float(opt_cfg.get("eps", 1e-8)),
                                      max_grad_norm=float(tr.get("max_grad_norm", 1.0)), use_cuda_graph=bool(tr.get("cuda_graph", True)),
                                      grad_accum_steps=accum, loss=loss_from_cfg(tr.get("loss")), ema=ema,
                                      cfg_scale=None if cfg_scale in (None, "1.0", 1.0) else str(cfg_scale),
-                                     optimizer=opt_name, optimizer_kwargs=af_opts, text_encoder=self.te, text_encoder_opts=te_opts,
+                                     optimizer=opt_name, optimizer_kwargs=opt_opts if opt_name == "adafactor" else None, text_encoder=self.te, text_encoder_opts=te_opts,
                                      loss_weights=None if self.groups is None else [w for _, _, _, w in self.groups])
         self.step_fn.sync_params(src=0)
         self.sched_step = make_scheduler(tr.get("scheduler"), self.step_fn)

@@ -371,6 +371,12 @@ int hcp_adamw_flat(float* p, const float* g, float* m, float* v, int64_t n, cons
  * no-op and leaves it. */
 int hcp_adamw_flat_dev(float* p, const float* g, float* m, float* v, int64_t n, const float* hyper_device, float grad_scale,
                        const float* sumsq_device, float max_norm, int* step_device, hcp_stream_t stream);
+/* Lion (lion_pytorch.Lion.step) with the contract of hcp_adamw_flat_dev: the same hyper row (eps unused), gradient g * grad_scale
+ * clipped with sumsq_device, *step_device advanced once per call with n > 0 (Lion itself has no bias correction; hcp_ema_flat
+ * reads it), 16-byte aligned p / g / m, n == 0 a no-op, no host synchronisation.  Per element, in fp32:
+ *   p = p (1 - lr wd);  c = beta1 m + (1 - beta1) g;  p = p - lr sign(c) (sign(0) = 0);  m = beta2 m + (1 - beta2) g.  One launch. */
+int hcp_lion_flat_dev(float* p, const float* g, float* m, int64_t n, const float* hyper_device, float grad_scale,
+                      const float* sumsq_device, float max_norm, int* step_device, hcp_stream_t stream);
 
 /* Adafactor (transformers.optimization.Adafactor.step) over the flat buffer, per tensor of the module's shape.  A tensor with two or
  * more dims is factored over its last two: view [P, R, C], exp_avg_sq_row [P, R] at state+row, exp_avg_sq_col [P, C] at state+col.

@@ -1,13 +1,14 @@
 """BASELINE config 4 on one H100: SDXL-base UNet (2.57 B parameters, random init), LoRA rank 16 on every attn / ff Linear and on the
 resnet / sampler convolutions (locon), batch 2, 1024x1024 (128x128 latent), 77 tokens x 2048.  Prints one JSON line with the step
 time.  Not the benchmark contract (bench.py measures config 2); a reference point for the SDXL rows of DESIGN.md.
-`--full-ft` trains every parameter of the UNet instead (reference cfgs/train/examples/FT_sdxl.yaml), with `--optimizer adamw` or
-`adafactor` (relative_step False, lr 1e-6, weight_decay 1e-3 as there); the line then also gives the optimizer's own time per step.
+`--full-ft` trains every parameter of the UNet instead (reference cfgs/train/examples/FT_sdxl.yaml), with `--optimizer adamw`,
+`adafactor` (relative_step False, lr 1e-6, weight_decay 1e-3 as there) or `lion` (lr 1e-6, weight_decay 1e-2 as the reference's
+Lion_optimizer.yaml); the line then also gives the optimizer's own time per step.
 `--lora-te` times, in the same run, the step above and then the same step with SDXL's two text encoders (CLIP-L + OpenCLIP-bigG,
 full size, random init) in front, LoRA rank 4 on their self_attn + mlp layers (reference cfgs/train/examples/lora_sdxl.yaml's
 lora_text_encoder item, clip_skip 1, no final norm): the line gives both step times, the card and its power limit.
 
-  python tools/bench_sdxl.py [--batch 2] [--steps 5] [--no-locon] [--full-ft --optimizer adafactor] [--lora-te]
+  python tools/bench_sdxl.py [--batch 2] [--steps 5] [--no-locon] [--full-ft --optimizer adafactor|lion] [--lora-te]
 """
 import argparse
 import json
@@ -30,7 +31,7 @@ ap.add_argument("--latent", type=int, default=128)
 ap.add_argument("--rank", type=int, default=16)
 ap.add_argument("--no-locon", action="store_true")
 ap.add_argument("--full-ft", action="store_true")
-ap.add_argument("--optimizer", choices=("adamw", "adafactor"), default="adamw")
+ap.add_argument("--optimizer", choices=("adamw", "adafactor", "lion"), default="adamw")
 ap.add_argument("--lora-te", action="store_true")
 args = ap.parse_args()
 if args.lora_te and (args.full_ft or args.optimizer != "adamw"):
@@ -86,6 +87,8 @@ else:
 params = [p for g in groups for p in g["params"]]
 if args.optimizer == "adafactor":
     step = LoraTrainStep(unet, groups, optimizer="adafactor", optimizer_kwargs={"relative_step": False, "weight_decay": 1e-3})
+elif args.optimizer == "lion":
+    step = LoraTrainStep(unet, groups if args.full_ft else params, optimizer="lion", weight_decay=1e-2)
 else:
     step = LoraTrainStep(unet, groups if args.full_ft else params)
 B, S = args.batch, args.latent

@@ -30,6 +30,7 @@ SEQ = {
     "hcp_lora_grad": [("grad_tc_kernel", 1, 1)],
     "hcp_adamw_flat": [("incr_step", 0, 1), ("adamw", 1, 1)],
     "hcp_adamw_flat_dev": [("incr_step", 1, 1), ("adamw_flat_dev", 1, 1)],
+    "hcp_lion_flat_dev": [("lion_flat_dev", 1, 1)],
 }
 
 
