@@ -154,7 +154,9 @@ EXPORTS = [
     "hcp_conv_in_wgrad_f32", "hcp_conv_out_wgrad_f32", "hcp_repack_weights", "hcp_adafactor_flat",
     "hcp_attn_fwd_causal_bf16", "hcp_attn_bwd_causal_bf16", "hcp_quick_gelu_fwd_bf16", "hcp_quick_gelu_bwd_bf16", "hcp_embed_gather_bf16",
     "hcp_sum_bf16_to_f32", "hcp_gelu_fwd_bf16", "hcp_gelu_bwd_bf16", "hcp_eps_loss_grouped_workspace_bytes", "hcp_eps_loss_grouped",
+    "hcp_pyramid_plan", "hcp_pyramid_workspace_bytes", "hcp_pyramid_noise", "hcp_add_noise_scaled",
 ]
+PYRAMID_MAX_LEVEL, PYRAMID_MAX_GROUPS, PYRAMID_PLAN_INTS = 16, 64, 32       # HCP_PYRAMID_* of include/hcp_b200.h
 
 
 def lib() -> C.CDLL:
@@ -237,6 +239,12 @@ def lib() -> C.CDLL:
             l.hcp_conv_out_wgrad_f32.argtypes = [vp, vp, i64, i64, i64, i64, i64, vp, vp, vp]
             l.hcp_repack_weights.argtypes = [vp, i64, vp]
             l.hcp_cfg_mix_f32.argtypes = [vp, vp, vp, i64, i64, f32, f32, C.c_int32, C.c_int32, vp, vp]
+            f64 = C.c_double
+            l.hcp_pyramid_plan.argtypes = [vp, C.c_int32, C.c_int32, f64, i64, i64, vp, vp]
+            l.hcp_pyramid_workspace_bytes.restype = C.c_size_t
+            l.hcp_pyramid_workspace_bytes.argtypes = [i64, i64, i64, i64, C.c_int32, f64]
+            l.hcp_pyramid_noise.argtypes = [vp, vp, vp, C.c_int32, vp, C.c_int32, f64, f64, i64, i64, i64, i64, vp, vp, vp, C.c_size_t, vp]
+            l.hcp_add_noise_scaled.argtypes = [vp, vp, vp, vp, vp, vp, C.c_int32, i64, i64, vp, vp]
             _lib = l
     return _lib
 

@@ -27,6 +27,7 @@ from torch import nn
 from . import _lib, adafactor, ops
 from ._lib import call, stream_ptr
 from .models.clip import SDXLTextEncoder, encode_prompt, encode_prompt_sdxl
+from .noise import resolve as resolve_noise_schedule
 
 SNR_LOSS_MODES = {"min_snr": 0, "soft_min_snr": 1, "kdiff_min_snr": 2, "edm": 3,
                   "MinSNRLoss": 0, "SoftMinSNRLoss": 1, "KDiffMinSNRLoss": 2, "EDMLoss": 3}
@@ -189,14 +190,22 @@ class LoraTrainStep:
     `text_embeds` is the encoder's projected pooled row (`models.encode_prompt_sdxl`; n_repeats 1).
 
     `loss_weights`: one weight per data group of `step_groups()` (the reference's per-dataset `loss_weight`, e.g. DreamBooth's
-    prior-preservation class set); None weighs every group 1.0."""
+    prior-preservation class set); None weighs every group 1.0.
+
+    `noise_scheduler`: None (SD1.x's scaled_linear DDPM table over `num_train_timesteps`, default 1000), the reference's
+    `model.noise_scheduler` config or a resolved `noise.NoiseSchedule`.  Its alphas_cumprod table serves add_noise, the Min-SNR
+    weights and the grouped loss, and its T the CFG rate (a different `num_train_timesteps` is an error).  With a
+    PyramidNoiseScheduler the base N(0,1) noise the caller passes becomes pyramid noise on the device, per data group and
+    micro-step (`ops.PyramidNoise`; seed it with `set_noise_seed`), and the loss target is the un-normalised pyramid sum, as in the
+    reference."""
 
     def __init__(self, unet: nn.Module, params: Union[Iterable[nn.Parameter], Sequence[dict]], lr: float = 1e-4, betas=None,
                  eps: float = 1e-8, weight_decay: Optional[float] = None, max_grad_norm: float = 1.0, use_cuda_graph: bool = True,
                  process_group: Optional[dist.ProcessGroup] = None, side_stream: bool = True, grad_accum_steps: int = 1,
-                 loss: Union[None, str, dict] = None, ema: Optional[dict] = None, cfg_scale=None, num_train_timesteps: int = 1000,
+                 loss: Union[None, str, dict] = None, ema: Optional[dict] = None, cfg_scale=None,
                  optimizer: str = "adamw", optimizer_kwargs: Optional[dict] = None, text_encoder: Optional[nn.Module] = None,
-                 text_encoder_opts: Optional[dict] = None, loss_weights: Optional[Sequence[float]] = None):
+                 text_encoder_opts: Optional[dict] = None, loss_weights: Optional[Sequence[float]] = None,
+                 noise_scheduler=None, num_train_timesteps: Optional[int] = None):
         self.unet = unet
         self.loss_weights = None if loss_weights is None else [float(w) for w in loss_weights]
         self._group_tables: Dict[tuple, dict] = {}
@@ -286,6 +295,13 @@ class LoraTrainStep:
             if kind not in SNR_LOSS_MODES:
                 raise ValueError(f"unknown loss {kind!r}: one of mse, {sorted(SNR_LOSS_MODES)}")
             self.loss_cfg = (SNR_LOSS_MODES[kind], float(loss.get("gamma", 1.0)))
+        self.noise_sched = None if noise_scheduler is None else resolve_noise_schedule(noise_scheduler, loss)
+        if self.noise_sched is not None:
+            T = self.noise_sched.num_train_timesteps
+            if num_train_timesteps is not None and int(num_train_timesteps) != T:
+                raise ValueError(f"num_train_timesteps={num_train_timesteps} disagrees with the noise scheduler's {T}")
+            num_train_timesteps = T
+        num_train_timesteps = 1000 if num_train_timesteps is None else int(num_train_timesteps)
         self.cfg_ctx = None
         if cfg_scale is not None:
             lo, hi, fn = get_cfg_range(cfg_scale) if isinstance(cfg_scale, str) else cfg_scale
@@ -297,7 +313,12 @@ class LoraTrainStep:
         if ema is not None:
             self.ema_cfg = (float(ema.get("decay_max", 0.9997)), float(ema.get("inv_gamma", 1.0)), float(ema.get("power", 2 / 3)))
             self.ema = self.flat.data.clone()
-        self.acp = ddpm_alphas_cumprod(num_train_timesteps).to(dev)
+        if self.noise_sched is None:
+            self.acp = ddpm_alphas_cumprod(num_train_timesteps).to(dev)
+        else:
+            self.acp = self.noise_sched.alphas_cumprod.to(dev)
+        pyr = None if self.noise_sched is None else self.noise_sched.pyramid
+        self.pyramid = None if pyr is None else ops.PyramidNoise(pyr["level"], pyr["discount"], pyr["step_size"], dev)
         self.loss = torch.zeros(1, dtype=torch.float32, device=dev)
         self.noise_pred: Optional[torch.Tensor] = None     # the UNet output of the last micro-step (kept alive across graph replays)
         self.gsq = torch.zeros(1, dtype=torch.float32, device=dev)
@@ -390,13 +411,23 @@ class LoraTrainStep:
             ops.join_side()
             ops.set_side_stream(False)
         ops.advance_dropout()
+        if self.pyramid is not None:
+            self.pyramid.advance()
+
+    def set_noise_seed(self, seed: int) -> None:
+        """Seed of the pyramid noise draws (one per data-parallel rank, as the dropout seed); no-op without a pyramid."""
+        if self.pyramid is not None:
+            self.pyramid.set_seed(seed)
 
     def _fb_body(self, latents, noise, t, ehs, added=None, grouped=None):
         B = latents.shape[0]
         per_image = latents[0].numel()
-        x_t = torch.empty_like(latents)
-        call("hcp_add_noise", latents.data_ptr(), noise.data_ptr(), t.data_ptr(), self.acp.data_ptr(), B, per_image, x_t.data_ptr(),
-             stream_ptr())
+        if self.pyramid is not None:                       # PyramidNoiseScheduler.add_noise per group; the loss target is its sum
+            x_t, noise = self.pyramid.add_noise(latents, noise, t, self.acp, (B,) if grouped is None else grouped["sizes"])
+        else:
+            x_t = torch.empty_like(latents)
+            call("hcp_add_noise", latents.data_ptr(), noise.data_ptr(), t.data_ptr(), self.acp.data_ptr(), B, per_image, x_t.data_ptr(),
+                 stream_ptr())
         x_in, t_in = x_t, t
         if self.cfg_ctx is not None:                       # DreamArtistPTContext.pre: 'b c h w -> (pn b) c h w', timesteps.repeat(2)
             x_in, t_in = torch.cat([x_t, x_t], 0), torch.cat([t, t], 0)
@@ -522,7 +553,7 @@ class LoraTrainStep:
             mask_dev = None if mask is None else mask.to(dev, non_blocking=True)
             added = None if added is None else {k: v.to(dev, non_blocking=True) for k, v in added.items()}
             self._forward_backward(lat.to(dev, non_blocking=True), noise.to(dev, non_blocking=True), t.to(dev, non_blocking=True),
-                                   ehs.to(dev, non_blocking=True), added, {**tables, "mask": mask_dev})
+                                   ehs.to(dev, non_blocking=True), added, {**tables, "mask": mask_dev, "sizes": sizes})
             self._finish_micro(self._optimizer)
             return tables["loss"]
         if self._graph_kind == "step":
@@ -637,7 +668,8 @@ class LoraTrainStep:
 
     def _snapshot(self):
         return (self.flat.data.clone(), [b.clone() for b in self._opt_buffers()],
-                None if self.ema is None else self.ema.clone(), ops.dropout_state_snapshot())
+                None if self.ema is None else self.ema.clone(), ops.dropout_state_snapshot(),
+                None if self.pyramid is None else self.pyramid.state.clone())
 
     def _restore(self, saved):
         self.flat.data.copy_(saved[0])
@@ -646,6 +678,8 @@ class LoraTrainStep:
         if self.ema is not None:
             self.ema.copy_(saved[2])
         ops.dropout_state_restore(saved[3])
+        if self.pyramid is not None:
+            self.pyramid.state.copy_(saved[4])
         self.flat.grad.zero_()
 
     def _capture(self, latents, noise, t, ehs, added=None, grouped=None):

@@ -119,6 +119,66 @@ def dropout_state_restore(saved) -> None:
         _Drop.state.copy_(saved)
 
 
+class PyramidNoise:
+    """PyramidNoiseScheduler.add_noise (reference hcpdiff/noise/pyramid_noise.py:17-32) on the device, once per data group:
+    hcp_pyramid_plan -> hcp_pyramid_noise -> hcp_add_noise_scaled.  Owns the {seed, draw} Philox state (separate from dropout's:
+    the dropout streams stay as they are), the plan, 1/std and the workspaces; everything is graph-capturable once the buffers
+    of a layout exist.  `add_noise` returns (x_t, target): target is the un-normalised pyramid sum, which the reference uses as the
+    loss target because its `noise +=` runs in place on make_noise's tensor while only x_t sees `noise / noise.std()`."""
+
+    def __init__(self, level: int, discount: float, step_size: float, device, seed: Optional[int] = None):
+        self.level, self.discount, self.step_size = int(level), float(discount), float(step_size)
+        self.device = torch.device(device)
+        self.state = torch.zeros(2, dtype=torch.int64, device=self.device)
+        self.set_seed(torch.initial_seed() if seed is None else seed)
+        self._bufs = {}
+
+    def set_seed(self, seed: int) -> None:
+        self.state.copy_(torch.tensor([int(seed) & 0x7FFFFFFFFFFFFFFF, 0], dtype=torch.int64))
+
+    def advance(self) -> None:
+        """End of a micro-step: the next one draws new ratios and grids."""
+        call("hcp_counter_add_u64", self.state.data_ptr() + 8, 1, stream_ptr())
+
+    def buffers(self, sizes: Sequence[int], C: int, H: int, W: int) -> dict:
+        """Device tables of one layout (group batch sizes, latent shape), built once: group_start int32 [G+1], plan, inv_std, workspace."""
+        key = (tuple(sizes), C, H, W)
+        buf = self._bufs.get(key)
+        if buf is None:
+            starts = [0]
+            for b in sizes:
+                starts.append(starts[-1] + int(b))
+            nbytes = _lib.lib().hcp_pyramid_workspace_bytes(starts[-1], C, H, W, self.level, self.step_size)
+            buf = {"group_start": torch.tensor(starts, dtype=torch.int32, device=self.device),
+                   "plan": torch.zeros((len(sizes), _lib.PYRAMID_PLAN_INTS), dtype=torch.int32, device=self.device),
+                   "inv_std": torch.zeros(len(sizes), dtype=torch.float32, device=self.device),
+                   "ws": torch.zeros((nbytes + 15) // 16 * 4, dtype=torch.float32, device=self.device)}
+            self._bufs[key] = buf
+        return buf
+
+    def plan(self, buf: dict, H: int, W: int) -> None:
+        call("hcp_pyramid_plan", self.state.data_ptr(), buf["plan"].shape[0], self.level, self.step_size, H, W, buf["plan"].data_ptr(),
+             stream_ptr())
+
+    def pyramid(self, noise: torch.Tensor, buf: dict, target: torch.Tensor) -> None:
+        B, C, H, W = noise.shape
+        call("hcp_pyramid_noise", noise.data_ptr(), buf["plan"].data_ptr(), buf["group_start"].data_ptr(), buf["plan"].shape[0],
+             self.state.data_ptr(), self.level, self.discount, self.step_size, B, C, H, W, target.data_ptr(), buf["inv_std"].data_ptr(),
+             buf["ws"].data_ptr(), buf["ws"].numel() * 4, stream_ptr())
+
+    def add_noise(self, latents: torch.Tensor, noise: torch.Tensor, t: torch.Tensor, acp: torch.Tensor, sizes: Sequence[int]):
+        """(x_t, target) for fp32 NCHW latents / base N(0,1) noise whose batch is the groups of `sizes` in order."""
+        B, C, H, W = latents.shape
+        buf = self.buffers(sizes, C, H, W)
+        target = torch.empty_like(noise)
+        x_t = torch.empty_like(latents)
+        self.plan(buf, H, W)
+        self.pyramid(noise, buf, target)
+        call("hcp_add_noise_scaled", latents.data_ptr(), target.data_ptr(), t.data_ptr(), acp.data_ptr(), buf["inv_std"].data_ptr(),
+             buf["group_start"].data_ptr(), len(sizes), B, C * H * W, x_t.data_ptr(), stream_ptr())
+        return x_t, target
+
+
 class DropoutFn(torch.autograd.Function):
     """out[:, c0:c0+n] = dropout_p(y[:, c0:c0+n]) for every (c0, n, p) range (p = 0: copy), + residual + per-image row bias.
     y bf16 [..., N]; the ranges must tile [0, N)."""

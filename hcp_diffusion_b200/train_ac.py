@@ -10,7 +10,9 @@ weight_decay, betas, eps}` for `torch.optim.AdamW` (the default `_target_`), the
 weight_decay`, reference cfgs/train/examples/Lion_optimizer.yaml; `use_triton` is accepted and changes nothing, since it only picks
 lion-pytorch's Triton kernel for the same arithmetic), `scheduler.{name, num_warmup_steps, num_training_steps, scheduler_kwargs}` (one_cycle / constant /
 constant_with_warmup), `loss.criterion` (`torch.nn.MSELoss` or `hcpdiff.loss.MinSNRLoss`-family `_target_` + `gamma`), `cfg_scale`
-(DreamArtist), `resume.{ckpt_path.unet, start_step}`; `model.ema` (`decay_max`, `inv_gamma`, `power`).
+(DreamArtist), `resume.{ckpt_path.unet, start_step}`; `model.ema` (`decay_max`, `inv_gamma`, `power`); `model.noise_scheduler`
+(`noise.resolve`: DDPMScheduler / .from_pretrained, ZeroTerminalScheduler, PyramidNoiseScheduler; `t` is drawn from [0, its
+num_train_timesteps), and null keeps SD1.x's DDPM table).
 
 Text encoder (SD1.x CLIP): `lora_text_encoder` items train LoRA on it next to the UNet (reference train_ac.py:61,335):
 `model.text_encoder` (instantiable, default CLIP-L) with weights from `model.text_encoder_init`, `model.clip_skip`,
@@ -53,6 +55,7 @@ import torch.distributed as dist
 from . import adafactor
 from .ckpt_manager import CkptManagerPKL, CkptManagerSafe, auto_manager
 from .engine import LoraTrainStep
+from .noise import resolve as resolve_noise_schedule
 from .utils.cfg_net_tools import load_lora_state, make_hcpdiff
 from .utils.config import instantiate, load_config_with_cli
 
@@ -248,12 +251,16 @@ class Trainer:
         if ema_cfg:
             ema = {k: ema_cfg[k] for k in ("decay_max", "inv_gamma", "power") if k in ema_cfg}
         cfg_scale = tr.get("cfg_scale")
+        loss = loss_from_cfg(tr.get("loss"))
+        self.noise_sched = resolve_noise_schedule(cfgs.model.get("noise_scheduler"), loss)
+        self.T = self.noise_sched.num_train_timesteps
         self.step_fn = LoraTrainStep(self.unet, groups, weight_decay=weight_decay, betas=betas, eps=float(opt_cfg.get("eps", 1e-8)),
                                      max_grad_norm=float(tr.get("max_grad_norm", 1.0)), use_cuda_graph=bool(tr.get("cuda_graph", True)),
-                                     grad_accum_steps=accum, loss=loss_from_cfg(tr.get("loss")), ema=ema,
+                                     grad_accum_steps=accum, loss=loss, ema=ema,
                                      cfg_scale=None if cfg_scale in (None, "1.0", 1.0) else str(cfg_scale),
                                      optimizer=opt_name, optimizer_kwargs=opt_opts if opt_name == "adafactor" else None, text_encoder=self.te, text_encoder_opts=te_opts,
-                                     loss_weights=None if self.groups is None else [w for _, _, _, w in self.groups])
+                                     loss_weights=None if self.groups is None else [w for _, _, _, w in self.groups],
+                                     noise_scheduler=None if cfgs.model.get("noise_scheduler") is None else self.noise_sched)
         self.step_fn.sync_params(src=0)
         self.sched_step = make_scheduler(tr.get("scheduler"), self.step_fn)
         self.bs, self.accum = bs, accum
@@ -264,6 +271,7 @@ class Trainer:
             self.ckpt.set_save_dir(os.path.join(self.exp_dir, "ckpts"))
         from . import ops
         ops.set_dropout_seed(seed + 7919 * (self.rank + 1))
+        self.step_fn.set_noise_seed(seed + 104729 * (self.rank + 1))
         self._load_data(seed)
 
     def _build_text_encoder(self, cfgs):
@@ -362,7 +370,7 @@ class Trainer:
             neg = self.ehs_neg[idx] if self.ehs_neg is not None else torch.zeros_like(ehs)
             ehs = torch.cat([neg, ehs], 0)
         noise = torch.randn(lat.shape, generator=self.gen)
-        t = torch.randint(0, 1000, (self.bs,), generator=self.gen, dtype=torch.int64)
+        t = torch.randint(0, self.T, (self.bs,), generator=self.gen, dtype=torch.int64)
         batch = [x.pin_memory() for x in (lat, noise, t, ehs)]
         if self.text_time:
             added = {"time_ids": self.time_ids[idx].pin_memory()}
@@ -381,7 +389,7 @@ class Trainer:
                 neg = src["ehs_neg"][idx] if src["ehs_neg"] is not None else torch.zeros_like(ehs)
                 ehs = torch.cat([neg, ehs], 0)
             noise = torch.randn(lat.shape, generator=self.gen)
-            t = torch.randint(0, 1000, (bs,), generator=self.gen, dtype=torch.int64)
+            t = torch.randint(0, self.T, (bs,), generator=self.gen, dtype=torch.int64)
             b = {"latents": lat, "noise": noise, "t": t, "ehs": ehs}
             if self.text_time:
                 b["added_cond_kwargs"] = {"time_ids": src["time_ids"][idx]}

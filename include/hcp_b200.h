@@ -449,6 +449,37 @@ int hcp_counter_add_u64(uint64_t* counter_device, uint64_t inc, hcp_stream_t str
 int hcp_cfg_mix_f32(const float* eps2, const float* dout, const int64_t* t, int64_t B, int64_t per_image, float scale_lo,
                     float scale_hi, int32_t mode, int32_t num_train_timesteps, float* out, hcp_stream_t stream);
 
+/* Pyramid (multi-resolution) noise: PyramidNoiseScheduler(base, level, discount, step_size, 'bilinear').add_noise (reference
+ * hcpdiff/noise/pyramid_noise.py:17-32), called once per data group and micro-step by Trainer.make_noise (hcpdiff/train_ac.py:437-447).
+ * Three calls, all CUDA-graph capturable (no host synchronisation, no allocation); bad pointers and sizes are refused before any
+ * launch.  Random numbers come from Philox4x32-10 on state_device = {seed, draw} (uint64 [2], its own state, not the dropout one):
+ * the caller advances `draw` once per micro-step with hcp_counter_add_u64, and the data group g is the Philox site.
+ *
+ * Plan: plan int32 [ngroups, HCP_PYRAMID_PLAN_INTS], row g = {n, 0, hn_1, wn_1, .., hn_n, wn_n, 0 ..}: for i = 1 .. level-1,
+ * r_i = 2 U + step_size (U a 53-bit double), hn_i, wn_i = max(1, int(H / r_i^i)), max(1, int(W / r_i^i)) in float64, stopping after
+ * the first level with hn_i == 1 or wn_i == 1 (pyramid_noise.py:26-31).  A caller may write its own plan instead; the sum clamps
+ * n to the level count and each size to [1, the size at r = step_size], the largest grid the workspace holds. */
+#define HCP_PYRAMID_MAX_LEVEL 16
+#define HCP_PYRAMID_MAX_GROUPS 64
+#define HCP_PYRAMID_PLAN_INTS 32
+int hcp_pyramid_plan(const uint64_t* state_device, int32_t ngroups, int32_t level /* 1 .. HCP_PYRAMID_MAX_LEVEL */,
+                     double step_size /* >= 1 */, int64_t H, int64_t W, int32_t* plan, hcp_stream_t stream);
+/* Sum: target = noise + sum_i bilinear(N(0,1) [b_g, C, hn_i, wn_i] -> [H, W]) * fp32(discount^i), per element in fp32 in level
+ * order (F.interpolate, align_corners=False), and inv_std[g] = 1 / std(target over group g), unbiased, from fp64 partials summed in
+ * a fixed order (replays are bit-identical).  target is the reference's loss target: its `noise +=` runs in place on make_noise's
+ * tensor, and only the x_t input sees the normalised noise.  target may alias noise.  group_start int32 [ngroups + 1] (device):
+ * group g is batch rows [group_start[g], group_start[g+1]), 0 = group_start[0] < .. < group_start[ngroups] = B.  Grid values of
+ * level i: counter (q, i, g, draw_lo), key (seed_lo, seed_hi ^ draw_hi), Box-Muller in float64 on words (0, 1) and (2, 3) for
+ * elements 4q .. 4q+3 of the group's grid.  Each level grid is generated once into the workspace.  B == 0 is a no-op. */
+size_t hcp_pyramid_workspace_bytes(int64_t B, int64_t C, int64_t H, int64_t W, int32_t level, double step_size);
+int hcp_pyramid_noise(const float* noise, const int32_t* plan, const int32_t* group_start, int32_t ngroups, const uint64_t* state_device,
+                      int32_t level, double discount, double step_size, int64_t B, int64_t C, int64_t H, int64_t W, float* target,
+                      float* inv_std /* fp32 [ngroups] */, void* workspace, size_t workspace_bytes, hcp_stream_t stream);
+/* x_t = sqrt(acp[t]) x0 + sqrt(1 - acp[t]) (noise * inv_std[g(b)])  (the base scheduler's DDPMScheduler.add_noise on the normalised
+ * pyramid noise, pyramid_noise.py:32), g(b) from group_start as above.  hcp_add_noise is the same with inv_std = 1. */
+int hcp_add_noise_scaled(const float* x0, const float* noise, const int64_t* t, const float* alphas_cumprod, const float* inv_std,
+                         const int32_t* group_start, int32_t ngroups, int64_t B, int64_t per_image, float* xt, hcp_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Full fine-tune (reference `unet:` config items, hcpdiff/utils/cfg_net_tools.py:96-106; cfgs/train/examples/DreamBooth.yaml:6-10):
  * gradients of the base model's own parameters and the per-step repack of the trained fp32 masters.  Every gradient is ACCUMULATED
