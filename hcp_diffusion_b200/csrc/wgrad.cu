@@ -668,12 +668,30 @@ static int lg_table(LGTable& t, const hcp_lora_grad_block* blocks, int32_t nbloc
     return HCP_OK;
 }
 
+// X-column ranges and destination pitches of a linear launch's blocks.  The kernel reduces only X columns [n_begin, n_end), so a
+// block reaching outside them would silently lose those columns; a pitch below the row length would make destination rows overlap.
+static int lg_check_ranges(const hcp_lora_grad_block* blocks, int32_t nblocks, int64_t n_begin, int64_t n_end) {
+    for (int i = 0; i < nblocks; ++i) {
+        const hcp_lora_grad_block& k = blocks[i];
+        if (k.n_lo >= k.n_hi || k.n_lo < n_begin || k.n_hi > n_end)
+            return set_error(HCP_ERR_INVALID, "lora_grad: block columns [n_lo, n_hi) must be a non-empty part of [n_begin, n_end)");
+        if (k.dst_ld < (k.transpose_out ? (int64_t)k.rank : k.n_hi - k.n_lo))
+            return set_error(HCP_ERR_INVALID, "lora_grad: block dst_ld below its row length (rank, or n_hi - n_lo without transpose)");
+    }
+    return HCP_OK;
+}
+
 static int lg_fill(WgradParams& p, int z, const void* S, int64_t lds, const void* X, int64_t ldx, int64_t M, int64_t n_begin,
                    int64_t n_end, const hcp_lora_grad_block* blocks, int32_t nblocks, int target_ctas) {
     if (!S || !X || !blocks || nblocks < 1 || nblocks > LG_MAX_BLOCKS) return set_error(HCP_ERR_INVALID, "lora_grad: 1..8 blocks per problem");
-    if (n_end <= n_begin || (ldx % 8) != 0 || (n_begin % 8) != 0 || lds < 64 || (lds % 8) != 0) return set_error(HCP_ERR_INVALID, "lora_grad: shape");
+    if (n_begin < 0 || n_end <= n_begin || (ldx % 8) != 0 || (n_begin % 8) != 0 || lds < 64 || (lds % 8) != 0)
+        return set_error(HCP_ERR_INVALID, "lora_grad: shape");
+    // the X tensor map is ldx columns wide: columns past it would read as zeros
+    if (n_end > ldx) return set_error(HCP_ERR_INVALID, "lora_grad: n_end > ldx");
+    int rc = lg_check_ranges(blocks, nblocks, n_begin, n_end);
+    if (rc) return rc;
     WgProblem& q = p.prob[z];
-    int rc = make_tmap_2d(&q.tmX, X, (uint64_t)ldx, (uint64_t)M, (uint64_t)ldx, 64, 128);
+    rc = make_tmap_2d(&q.tmX, X, (uint64_t)ldx, (uint64_t)M, (uint64_t)ldx, 64, 128);
     if (rc) return rc;
     rc = make_tmap_2d(&q.tmS, S, 64, (uint64_t)M, (uint64_t)lds, 64, 128);     // the 64 columns of S this launch reduces
     if (rc) return rc;

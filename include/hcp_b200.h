@@ -331,7 +331,11 @@ int hcp_lora_pack_conv(const hcp_lora_conv_job* jobs_device, int64_t njobs, hcp_
  *     D[n, j] = scale_b * sum_m X[m, n] * S[m, c0_b + j],   j < rank_b      (S bf16 [M,64] with row pitch lds >= 64: one 64-column
  *     slab of the group's T / U buffer -- wider groups call once per slab with S advanced by 64 columns; X bf16 [M,ldx])
  * is ACCUMULATED (fp32 atomics) into  dst_b[j*dst_ld + (n-n_lo)]  (transpose_out = 0: dW_down[r,in], S = dY.(alpha B), X = x)
- *                               or   dst_b[(n-n_lo)*dst_ld + j]  (transpose_out = 1: dW_up[out,r],  S = x.A^T, X = dY). */
+ *                               or   dst_b[(n-n_lo)*dst_ld + j]  (transpose_out = 1: dW_up[out,r],  S = x.A^T, X = dY).
+ * hcp_lora_grad and hcp_lora_grad_pair refuse, before any launch:
+ *   - 0 <= n_begin < n_end <= ldx not holding (X columns past ldx would read as zeros);
+ *   - a block with n_lo >= n_hi or [n_lo, n_hi) not inside [n_begin, n_end) (the columns outside would be dropped);
+ *   - a block with dst_ld < rank (transpose_out = 1) or dst_ld < n_hi - n_lo (transpose_out = 0): rows would overlap. */
 typedef struct hcp_lora_grad_block {
     int64_t n_lo, n_hi;
     int32_t c0, rank;
