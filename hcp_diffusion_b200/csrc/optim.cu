@@ -1,6 +1,7 @@
 // SPDX-License-Identifier: Apache-2.0
 // Adafactor (transformers.optimization.Adafactor.step) over the flat fp32 parameter buffer of the training step (sm_90a), and
-// Lion (lion_pytorch.Lion.step, one elementwise kernel at the end of this file).
+// Lion (lion_pytorch.Lion.step, one elementwise kernel) and AdamW8bit (bitsandbytes.optim.AdamW8bit, blockwise 8-bit moments), both
+// near the end of this file.
 //
 // Every trainable tensor keeps its module shape: a tensor with two or more dims is factored over its LAST TWO dims, viewed as
 // [P, R, C] with the leading dims a batch (a Conv2d weight [O, I, 3, 3] is P = O*I slabs of 3 x 3); a 1-D tensor keeps an
@@ -321,6 +322,175 @@ __global__ void __launch_bounds__(256) lion_flat_dev_kernel(float* __restrict__ 
     }
 }
 
+// AdamW8bit (bitsandbytes.optim.AdamW8bit: Optimizer2State, optim_bits 8, block_wise; kOptimizerStatic8bit2StateBlockwise and
+// kOptimizer32bit2State) over the tensors of a host-built table, hyper = fp32 [ngroups, 5] rows {lr, beta1, beta2, eps,
+// weight_decay} as adamw_flat_dev_kernel reads them, steps int32 [ngroups] already advanced by adafactor_incr_kernel.
+//
+// A work item is a run of whole 256-element blocks of one tensor; CTAs walk the items grid-stride, four blocks at a time, one
+// quarter (64 threads, two warps) per block and four consecutive elements per thread.  Per element, in fp32 with every product
+// and sum rounded on its own (no contraction, so the moments, scales and codes are reproducible from fp32 on any machine):
+//   g' = g * gscale_clip;   s1 = map1[c1] * absmax1;  s2 = map2[c2] * absmax2                       (8-bit; 32-bit: s1 = m, s2 = v)
+//   s1 = s1 b1 + (1 - b1) g';  s2 = s2 b2 + ((1 - b2) g') g'
+//   p = p + (-lr sqrt(1 - b2^t) / (1 - b1^t)) s1 / (sqrt(s2) + eps sqrt(1 - b2^t));  if wd > 0: p = p (1 - lr wd)
+// 8-bit only: a non-finite g sets s1 = s2 = 0 and leaves p; the block's new scale is max |s| over its elements (a warp max, then
+// the two warps of the quarter -- an exact, order-free reduction inside the CTA), and each s / scale (0 for an all-zero block) is
+// re-encoded with bitsandbytes' binary search and midpoint rule (an exact midpoint goes to the last probed entry); a first-moment
+// code whose value has the other sign bit than s1 moves one step toward s1's sign.  The maps live in shared memory at index
+// k + k / 32, which spreads the search's probes (entries 32 apart) over different banks.
+constexpr int A8_T = 256;
+constexpr int A8_BLOCK = 256;
+
+__host__ __device__ constexpr int a8_idx(int k) { return k + (k >> 5); }
+
+__device__ __forceinline__ float a8_grad_scale(float gscale, const float* __restrict__ sumsq, float max_norm) {
+    float clip = 1.f;
+    if (sumsq && max_norm > 0.f) {                     // clip_grad_norm_ as af_grad_scale, each operation rounded on its own
+        const float norm = __fmul_rn(sqrtf(*sumsq), gscale);
+        clip = fminf(1.f, __fdiv_rn(max_norm, __fadd_rn(norm, 1e-6f)));
+    }
+    return __fmul_rn(gscale, clip);
+}
+
+template <bool SIGNED>
+__device__ __forceinline__ int a8_quantize(const float* __restrict__ s_map, float x) {
+    int pivot = 127, upper_pivot = 255, lower_pivot = 0;
+    float lower = SIGNED ? -1.f : 0.f, upper = 1.f;
+    float val = s_map[a8_idx(pivot)];
+#pragma unroll
+    for (int i = 64; i > 0; i >>= 1) {
+        if (x > val) { lower_pivot = pivot; lower = val; pivot += i; }
+        else { upper_pivot = pivot; upper = val; pivot -= i; }
+        val = s_map[a8_idx(pivot)];
+    }
+    if (x > val) return x > __fmul_rn(__fadd_rn(upper, val), 0.5f) ? upper_pivot : pivot;
+    return x < __fmul_rn(__fadd_rn(lower, val), 0.5f) ? lower_pivot : pivot;
+}
+
+__global__ void __launch_bounds__(A8_T, 4) adamw8bit_kernel(float* __restrict__ p, const float* __restrict__ g, uint8_t* __restrict__ code1,
+                                                         uint8_t* __restrict__ code2, float* __restrict__ absmax1, float* __restrict__ absmax2,
+                                                         float* __restrict__ m32, float* __restrict__ v32, const float* __restrict__ maps,
+                                                         const hcp_adamw8bit_tensor* __restrict__ tensors,
+                                                         const hcp_adamw8bit_item* __restrict__ items, int nitems,
+                                                         const float* __restrict__ hyper, const int* __restrict__ steps, float gscale,
+                                                         const float* __restrict__ sumsq, float max_norm) {
+    pdl_trigger();
+    pdl_wait();
+    __shared__ float s_map1[a8_idx(256)], s_map2[a8_idx(256)];
+    __shared__ float s_max[2][A8_T / 32][2];           // [parity][warp][moment]
+    for (int k = threadIdx.x; k < 256; k += A8_T) {
+        s_map1[a8_idx(k)] = maps[k];
+        s_map2[a8_idx(k)] = maps[256 + k];
+    }
+    __syncthreads();
+    const float gs = a8_grad_scale(gscale, sumsq, max_norm);
+    const int q = threadIdx.x >> 6, lane64 = threadIdx.x & 63, warp = threadIdx.x >> 5;
+    int parity = 0;
+    for (int ii = blockIdx.x; ii < nitems; ii += gridDim.x) {
+        const hcp_adamw8bit_item it = items[ii];
+        const hcp_adamw8bit_tensor T = tensors[it.tensor];
+        const float* hy = hyper + 5 * T.group;
+        const float lr = hy[0], b1 = hy[1], b2 = hy[2], eps = hy[3], wd = hy[4];
+        const float t = (float)steps[T.group];
+        const float corr1 = 1.f - powf(b1, t), corr2 = sqrtf(1.f - powf(b2, t));
+        const float step_size = __fdiv_rn(__fmul_rn(-lr, corr2), corr1);
+        const float eps_c = __fmul_rn(eps, corr2);
+        const float omb1 = 1.f - b1, omb2 = 1.f - b2, decay = __fsub_rn(1.f, __fmul_rn(lr, wd));
+        const bool q8 = T.mode == 1;
+        float* pt = p + T.offset;
+        const float* gt = g + T.offset;
+        for (int b0 = it.block0; b0 < it.block1; b0 += 4) {
+            const int64_t b = b0 + q;
+            const bool active = b < it.block1;
+            const int64_t e0 = b * A8_BLOCK + lane64 * 4;
+            const int nv = active ? (int)max((int64_t)0, min((int64_t)4, T.numel - e0)) : 0;
+            float w[4] = {0.f, 0.f, 0.f, 0.f}, gr[4] = {0.f, 0.f, 0.f, 0.f}, s1[4] = {0.f, 0.f, 0.f, 0.f}, s2[4] = {0.f, 0.f, 0.f, 0.f};
+            uint8_t c1[4] = {0, 0, 0, 0}, c2[4] = {0, 0, 0, 0};
+            if (nv == 4) {
+                const float4 w4 = *reinterpret_cast<const float4*>(pt + e0), g4 = *reinterpret_cast<const float4*>(gt + e0);
+                w[0] = w4.x; w[1] = w4.y; w[2] = w4.z; w[3] = w4.w;
+                gr[0] = g4.x; gr[1] = g4.y; gr[2] = g4.z; gr[3] = g4.w;
+                if (q8) {
+                    const uchar4 a = *reinterpret_cast<const uchar4*>(code1 + T.state + e0), c = *reinterpret_cast<const uchar4*>(code2 + T.state + e0);
+                    c1[0] = a.x; c1[1] = a.y; c1[2] = a.z; c1[3] = a.w;
+                    c2[0] = c.x; c2[1] = c.y; c2[2] = c.z; c2[3] = c.w;
+                } else {
+                    const float4 m4 = *reinterpret_cast<const float4*>(m32 + T.state + e0), v4 = *reinterpret_cast<const float4*>(v32 + T.state + e0);
+                    s1[0] = m4.x; s1[1] = m4.y; s1[2] = m4.z; s1[3] = m4.w;
+                    s2[0] = v4.x; s2[1] = v4.y; s2[2] = v4.z; s2[3] = v4.w;
+                }
+            } else {
+                for (int j = 0; j < nv; ++j) {
+                    w[j] = pt[e0 + j];
+                    gr[j] = gt[e0 + j];
+                    if (q8) { c1[j] = code1[T.state + e0 + j]; c2[j] = code2[T.state + e0 + j]; }
+                    else { s1[j] = m32[T.state + e0 + j]; s2[j] = v32[T.state + e0 + j]; }
+                }
+            }
+            float am1 = 0.f, am2 = 0.f;
+            if (q8 && active) { am1 = absmax1[T.absmax + b]; am2 = absmax2[T.absmax + b]; }
+            float mx1 = 0.f, mx2 = 0.f;
+            bool fin[4];
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                fin[j] = !q8 || isfinite(gr[j]);
+                if (j >= nv) continue;
+                if (fin[j]) {
+                    const float gv = __fmul_rn(gr[j], gs);
+                    float a = s1[j], c = s2[j];
+                    if (q8) { a = __fmul_rn(s_map1[a8_idx(c1[j])], am1); c = __fmul_rn(s_map2[a8_idx(c2[j])], am2); }
+                    s2[j] = __fadd_rn(__fmul_rn(c, b2), __fmul_rn(__fmul_rn(omb2, gv), gv));
+                    s1[j] = __fadd_rn(__fmul_rn(a, b1), __fmul_rn(omb1, gv));
+                    float wj = __fadd_rn(w[j], __fmul_rn(step_size, __fdiv_rn(s1[j], __fadd_rn(sqrtf(s2[j]), eps_c))));
+                    if (wd > 0.f) wj = __fmul_rn(wj, decay);
+                    w[j] = wj;
+                } else {
+                    s1[j] = 0.f;
+                    s2[j] = 0.f;
+                }
+                mx1 = fmaxf(mx1, fabsf(s1[j]));
+                mx2 = fmaxf(mx2, fabsf(s2[j]));
+            }
+            if (q8) {                                      // uniform across the CTA: every item of one CTA step is one tensor's
+#pragma unroll
+                for (int o = 16; o > 0; o >>= 1) {
+                    mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, o));
+                    mx2 = fmaxf(mx2, __shfl_xor_sync(0xffffffffu, mx2, o));
+                }
+                if ((threadIdx.x & 31) == 0) { s_max[parity][warp][0] = mx1; s_max[parity][warp][1] = mx2; }
+                __syncthreads();
+                mx1 = fmaxf(s_max[parity][2 * q][0], s_max[parity][2 * q + 1][0]);
+                mx2 = fmaxf(s_max[parity][2 * q][1], s_max[parity][2 * q + 1][1]);
+                parity ^= 1;                               // the next write goes to the other half: one barrier per step
+                if (active && lane64 == 0) { absmax1[T.absmax + b] = mx1; absmax2[T.absmax + b] = mx2; }
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const float x1 = mx1 > 0.f ? __fdiv_rn(s1[j], mx1) : 0.f, x2 = mx2 > 0.f ? __fdiv_rn(s2[j], mx2) : 0.f;
+                    int k1 = a8_quantize<true>(s_map1, x1);
+                    if (signbit(s_map1[a8_idx(k1)]) != signbit(s1[j])) k1 = (k1 + (s1[j] > 0.f ? 1 : -1)) & 255;
+                    c1[j] = (uint8_t)k1;
+                    c2[j] = (uint8_t)a8_quantize<false>(s_map2, x2);
+                }
+            }
+            if (nv == 4) {
+                *reinterpret_cast<float4*>(pt + e0) = make_float4(w[0], w[1], w[2], w[3]);
+                if (q8) {
+                    *reinterpret_cast<uchar4*>(code1 + T.state + e0) = make_uchar4(c1[0], c1[1], c1[2], c1[3]);
+                    *reinterpret_cast<uchar4*>(code2 + T.state + e0) = make_uchar4(c2[0], c2[1], c2[2], c2[3]);
+                } else {
+                    *reinterpret_cast<float4*>(m32 + T.state + e0) = make_float4(s1[0], s1[1], s1[2], s1[3]);
+                    *reinterpret_cast<float4*>(v32 + T.state + e0) = make_float4(s2[0], s2[1], s2[2], s2[3]);
+                }
+            } else {
+                for (int j = 0; j < nv; ++j) {
+                    pt[e0 + j] = w[j];
+                    if (q8) { code1[T.state + e0 + j] = c1[j]; code2[T.state + e0 + j] = c2[j]; }
+                    else { m32[T.state + e0 + j] = s1[j]; v32[T.state + e0 + j] = s2[j]; }
+                }
+            }
+        }
+    }
+}
+
 }  // namespace hcp
 
 using namespace hcp;
@@ -361,5 +531,77 @@ extern "C" int hcp_lion_flat_dev(float* p, const float* g, float* m, int64_t n, 
     launch_k(lion_flat_dev_kernel, dim3((unsigned)blocks), dim3(256), 0, (cudaStream_t)st, p, g, m, n, hyper_device, grad_scale,
              sumsq_device, max_norm, step_device);
     LAUNCH_CHECK("lion_dev launch");
+    return HCP_OK;
+}
+
+// Host-side check of the tables the kernel will read (their device copies are the caller's): every tensor inside p / g and its
+// state inside the buffers, aligned for 16-byte (p, g, m, v) and 4-byte (codes) accesses, tensors and states in increasing,
+// non-overlapping order, and the items tiling each tensor's blocks once, in table order.
+static int adamw8bit_check_tables(const hcp_adamw8bit_tensor* T, int32_t ntensors, const hcp_adamw8bit_item* I, int64_t nitems, int64_t n,
+                                  int64_t code_bytes, int64_t nblocks, int64_t small_numel, int32_t ngroups) {
+    int64_t p_end = 0, code_end = 0, blk_end = 0, small_end = 0;
+    for (int32_t i = 0; i < ntensors; ++i) {
+        const hcp_adamw8bit_tensor& t = T[i];
+        if (t.numel <= 0 || t.offset < p_end || (t.offset & 3) || t.numel > n - t.offset)
+            return set_error(HCP_ERR_INVALID, "adamw8bit: tensor outside p / g, overlapping, or off 16-byte alignment");
+        if (t.group < 0 || t.group >= ngroups) return set_error(HCP_ERR_INVALID, "adamw8bit: tensor group out of range");
+        const int64_t nb = (t.numel + A8_BLOCK - 1) / A8_BLOCK;
+        if (t.mode == 1) {
+            if (t.state < code_end || (t.state & 3) || t.numel > code_bytes - t.state || t.absmax < blk_end || nb > nblocks - t.absmax)
+                return set_error(HCP_ERR_INVALID, "adamw8bit: 8-bit state outside the code / absmax buffers, overlapping or misaligned");
+            code_end = t.state + t.numel;
+            blk_end = t.absmax + nb;
+        } else if (t.mode == 0) {
+            if (t.state < small_end || (t.state & 3) || t.numel > small_numel - t.state)
+                return set_error(HCP_ERR_INVALID, "adamw8bit: 32-bit state outside state32, overlapping or misaligned");
+            small_end = t.state + t.numel;
+        } else {
+            return set_error(HCP_ERR_INVALID, "adamw8bit: tensor mode must be 0 (32-bit) or 1 (8-bit)");
+        }
+        p_end = t.offset + t.numel;
+    }
+    int32_t cur = 0;
+    int64_t next = 0;                                  // the next block of tensor `cur` an item must start at
+    for (int64_t k = 0; k < nitems; ++k) {
+        const hcp_adamw8bit_item& it = I[k];
+        if (it.tensor == cur + 1 && cur + 1 < ntensors && next == (T[cur].numel + A8_BLOCK - 1) / A8_BLOCK) { cur += 1; next = 0; }
+        if (it.tensor != cur || it.block0 != next || it.block1 <= it.block0 ||
+            it.block1 > (T[cur].numel + A8_BLOCK - 1) / A8_BLOCK)
+            return set_error(HCP_ERR_INVALID, "adamw8bit: items must tile every tensor's blocks once, in table order");
+        next = it.block1;
+    }
+    if (cur != ntensors - 1 || next != (T[cur].numel + A8_BLOCK - 1) / A8_BLOCK)
+        return set_error(HCP_ERR_INVALID, "adamw8bit: items leave blocks uncovered");
+    return HCP_OK;
+}
+
+extern "C" int hcp_adamw8bit_flat(float* p, const float* g, uint8_t* codes, float* absmax, float* state32, const float* maps_device,
+                                  const hcp_adamw8bit_tensor* tensors_host, const hcp_adamw8bit_tensor* tensors_device, int32_t ntensors,
+                                  const hcp_adamw8bit_item* items_host, const hcp_adamw8bit_item* items_device, int64_t nitems, int64_t n,
+                                  int64_t code_bytes, int64_t nblocks, int64_t small_numel, const float* hyper_device, int* steps_device,
+                                  int32_t ngroups, float grad_scale, const float* sumsq_device, float max_norm, hcp_stream_t st) {
+    if (ntensors < 0 || nitems < 0 || n < 0 || code_bytes < 0 || nblocks < 0 || small_numel < 0)
+        return set_error(HCP_ERR_INVALID, "adamw8bit: negative size");
+    if (ntensors == 0) return HCP_OK;
+    if (!p || !g || !maps_device || !tensors_host || !tensors_device || !items_host || !items_device || !hyper_device || !steps_device ||
+        ((code_bytes || nblocks) && (!codes || !absmax)) || (small_numel && !state32))
+        return set_error(HCP_ERR_INVALID, "adamw8bit: null pointer");
+    if (((uintptr_t)p | (uintptr_t)g | (uintptr_t)state32) & 15 || ((uintptr_t)codes & 15) || ((uintptr_t)absmax & 3) || (code_bytes & 15) ||
+        (small_numel & 3))
+        return set_error(HCP_ERR_INVALID, "adamw8bit: p / g / state32 / codes must be 16-byte aligned, code_bytes a multiple of 16 and "
+                                          "small_numel of 4");
+    if (ngroups <= 0 || ngroups > A8_T) return set_error(HCP_ERR_INVALID, "adamw8bit: group count");
+    if (nitems == 0 || nitems >= (1ll << 31) || nblocks >= (1ll << 40))
+        return set_error(HCP_ERR_INVALID, "adamw8bit: item count");
+    const int rc = adamw8bit_check_tables(tensors_host, ntensors, items_host, nitems, n, code_bytes, nblocks, small_numel, ngroups);
+    if (rc != HCP_OK) return rc;
+    const cudaStream_t s = (cudaStream_t)st;
+    int64_t blocks = nitems;                           // persistent: 64 registers per thread keep 4 CTAs of 256 on an SM
+    if (blocks > num_sms() * 4) blocks = num_sms() * 4;
+    launch_k(adafactor_incr_kernel, dim3(1), dim3(AF_T), 0, s, steps_device, (int)ngroups);
+    launch_k(adamw8bit_kernel, dim3((unsigned)blocks), dim3(A8_T), 0, s, p, g, codes, codes + code_bytes, absmax, absmax + nblocks,
+             state32, state32 + small_numel, maps_device, tensors_device, items_device, (int)nitems, hyper_device,
+             (const int*)steps_device, grad_scale, sumsq_device, max_norm);
+    LAUNCH_CHECK("adamw8bit launch");
     return HCP_OK;
 }

@@ -24,7 +24,7 @@ import torch
 import torch.distributed as dist
 from torch import nn
 
-from . import _lib, adafactor, ops
+from . import _lib, adafactor, adamw8bit, ops
 from ._lib import call, stream_ptr
 from .models.clip import SDXLTextEncoder, encode_prompt, encode_prompt_sdxl
 from .noise import resolve as resolve_noise_schedule
@@ -165,7 +165,7 @@ class _CfgMixFn(torch.autograd.Function):
 
 class LoraTrainStep:
     """One optimisation step of LoRA (or full) training on a `UNet2DConditionModel`: eps-prediction loss, grad-norm clip, AdamW
-    (or Adafactor, or Lion).
+    (or Adafactor, Lion or AdamW8bit).
 
     `params`: parameters, or optimizer-style groups [{'params': [...], 'lr': ..., 'weight_decay': ...}] (one per `lora_unet:` /
     `unet:` config item, reference cfg_net_tools.py:96-127).  `grad_accum_steps`: micro-batches per optimizer step
@@ -179,7 +179,11 @@ class LoraTrainStep:
     momentum buffer, half of AdamW's state) or 'adafactor' (transformers.optimization.Adafactor; `optimizer_kwargs` takes its
     constructor keys with its defaults -- `lr`, `eps`, `clip_threshold`, `decay_rate`, `beta1`, `weight_decay`, `scale_parameter`,
     `relative_step`, `warmup_init` -- and a group's own 'lr' / 'weight_decay' win over them).  Adafactor keeps factored second moments per tensor of the module's shape (state sized by
-    adafactor.state_numel), plus one flat first-moment buffer only when `beta1` is set.
+    adafactor.state_numel), plus one flat first-moment buffer only when `beta1` is set.  'adamw8bit' is bitsandbytes.optim.AdamW8bit
+    (`lr`, `betas`, `eps`, `weight_decay` with AdamW's defaults; `optimizer_kwargs` takes its constructor keys -- those four win
+    over the arguments when given, and `min_8bit_size`, default 4096 -- and refuses the options adamw8bit.check_options refuses):
+    tensors of at least min_8bit_size elements keep both moments as 8-bit codes with one fp32 scale per 256-element block (about
+    2 B per parameter), smaller ones fp32 moments; weight decay is applied after the step, as bitsandbytes applies it.
 
     `text_encoder`: a `models.CLIPTextModel` whose LoRA adapters train together with the UNet's (the reference's `lora_text_encoder`,
     `TEUnetWrapper`); its adapter parameters must be among `params` (their own groups), so they share the flat buffer: one all-reduce,
@@ -229,14 +233,21 @@ class LoraTrainStep:
                     "SDXL with n_repeats > 1 (tokenizer_repeats) is not supported: the reference pools bigG's text_embeds at the "
                     "largest id of the raw tokenizer output before it is cut into 77-token chunks, which pre-chunked ids cannot "
                     "express (the reference's SDXL config uses tokenizer_repeats: 1)")
-        if optimizer not in ("adamw", "adafactor", "lion"):
-            raise ValueError(f"optimizer {optimizer!r}: one of 'adamw', 'adafactor', 'lion'")
+        if optimizer not in ("adamw", "adafactor", "lion", "adamw8bit"):
+            raise ValueError(f"optimizer {optimizer!r}: one of 'adamw', 'adafactor', 'lion', 'adamw8bit'")
         self.optimizer = optimizer
         default_betas, default_wd = ((0.9, 0.99), 0.0) if optimizer == "lion" else ((0.9, 0.999), 1e-2)
         betas = default_betas if betas is None else tuple(betas)
         weight_decay = default_wd if weight_decay is None else weight_decay
-        af_opts = None
-        if optimizer == "adafactor":
+        af_opts = a8_opts = None
+        if optimizer == "adamw8bit":
+            given = dict(optimizer_kwargs or {})
+            a8_opts = adamw8bit.check_options(given)
+            lr = a8_opts["lr"] if "lr" in given else lr
+            betas = a8_opts["betas"] if "betas" in given else betas
+            eps = a8_opts["eps"] if "eps" in given else eps
+            weight_decay = a8_opts["weight_decay"] if "weight_decay" in given else weight_decay
+        elif optimizer == "adafactor":
             af_opts = adafactor.check_options(optimizer_kwargs)
             weight_decay = af_opts["weight_decay"]
             if af_opts["lr"] is not None:
@@ -264,6 +275,8 @@ class LoraTrainStep:
         self.m = self.v = None
         if af_opts is not None:
             self._init_adafactor(groups, af_opts)
+        elif a8_opts is not None:
+            self._init_adamw8bit(groups, a8_opts, betas, eps)
         else:
             self.m = torch.zeros_like(self.flat.data)
             self.v = torch.zeros_like(self.flat.data) if optimizer == "adamw" else None
@@ -277,6 +290,9 @@ class LoraTrainStep:
             if af_opts is not None:                        # rows of the [groups, 8] table the Adafactor kernels read
                 gi = len(self.segments)
                 hyper, step = self.af_hyper[gi], self.af_steps[gi:gi + 1]
+            elif a8_opts is not None:                      # rows of the [groups, 5] table the AdamW8bit kernel reads
+                gi = len(self.segments)
+                hyper, step = self.a8_hyper[gi], self.a8_steps[gi:gi + 1]
             else:
                 hyper = torch.tensor([g["lr"], betas[0], betas[1], eps, g["weight_decay"]], dtype=torch.float32, device=dev)
                 step = torch.zeros(1, dtype=torch.int32, device=dev)
@@ -353,14 +369,32 @@ class LoraTrainStep:
         self.af_tensors, self.af_items = to_dev(lay.tensors), to_dev(lay.items)
         self.af_factor_items = to_dev(lay.factor_items) if lay.factor_items.size else None
 
+    def _init_adamw8bit(self, groups, opts, betas, eps):
+        dev = self.flat.data.device
+        groups = [g for g in groups if g["params"]]          # the segments: a group emptied by de-duplication has none
+        group_of = [gi for gi, g in enumerate(groups) for _ in g["params"]]
+        self.a8_layout = lay = adamw8bit.Layout([p.numel() for p in self.flat.params], self.flat.offsets, group_of, opts["min_8bit_size"])
+        self.a8_hyper = torch.tensor([[g["lr"], betas[0], betas[1], eps, g["weight_decay"]] for g in groups], dtype=torch.float32, device=dev)
+        self.a8_steps = torch.zeros(len(groups), dtype=torch.int32, device=dev)
+        self.a8_codes = torch.zeros(2 * lay.code_bytes, dtype=torch.uint8, device=dev)
+        self.a8_absmax = torch.zeros(2 * lay.nblocks, dtype=torch.float32, device=dev)
+        self.a8_state32 = torch.zeros(2 * lay.small_numel, dtype=torch.float32, device=dev)
+        self.a8_maps = adamw8bit.maps().to(dev)
+        to_dev = lambda a: torch.from_numpy(a.view(np.uint8).copy()).to(dev)      # noqa: E731  (packed C structs)
+        self.a8_tensors, self.a8_items = to_dev(lay.tensors), to_dev(lay.items)
+
     @property
     def optimizer_state_bytes(self) -> int:
         """Bytes of optimizer state (moments; not the parameters, gradients or scratch)."""
+        if self.optimizer == "adamw8bit":
+            return sum(b.numel() * b.element_size() for b in (self.a8_codes, self.a8_absmax, self.a8_state32))
         if self.optimizer == "adafactor":
             return 4 * (self.af_state.numel() + (0 if self.af_exp_avg is None else self.af_exp_avg.numel()))
         return 4 * sum(b.numel() for b in (self.m, self.v) if b is not None)
 
     def _opt_buffers(self) -> List[torch.Tensor]:
+        if self.optimizer == "adamw8bit":
+            return [self.a8_codes, self.a8_absmax, self.a8_state32, self.a8_steps]
         if self.optimizer == "adafactor":
             return [self.af_state, self.af_steps] + ([] if self.af_exp_avg is None else [self.af_exp_avg])
         return [b for b in (self.m, self.v) if b is not None] + [s["step"] for s in self.segments]
@@ -375,14 +409,14 @@ class LoraTrainStep:
             s["lr"].fill_(s["base_lr"] * ratio)
 
     def set_hyper(self, group: int, lr: Optional[float] = None, beta1: Optional[float] = None):
-        """What an LR scheduler writes per step (OneCycleLR cycles the lr and, for AdamW and Lion, beta1): device-side, graph-replay
-        safe."""
+        """What an LR scheduler writes per step (OneCycleLR cycles the lr and, for AdamW, AdamW8bit and Lion, beta1): device-side,
+        graph-replay safe."""
         h = self.segments[group]["hyper"]
         if lr is not None:
             h[0:1].fill_(lr)
         if beta1 is not None:
             if self.optimizer == "adafactor":
-                raise ValueError("beta1 is scheduled for AdamW and Lion only")
+                raise ValueError("beta1 is scheduled for AdamW, AdamW8bit and Lion only")
             h[1:2].fill_(beta1)
 
     def sync_params(self, src: int = 0):
@@ -468,7 +502,15 @@ class LoraTrainStep:
                  _lib.ptr(self.af_exp_avg), self.af_work.data_ptr(), self.af_tensors.data_ptr(), self.af_items.data_ptr(), lay.items.size,
                  _lib.ptr(self.af_factor_items), lay.factor_items.size, self.af_hyper.data_ptr(), self.af_steps.data_ptr(),
                  len(self.segments), 1.0 / self.world, self.gsq.data_ptr(), float(self.max_norm or 0.0), stream_ptr())
-        for s in (self.segments if self.optimizer != "adafactor" else ()):
+        elif self.optimizer == "adamw8bit":
+            lay = self.a8_layout
+            nz = lambda t: t.data_ptr() if t.numel() else None      # noqa: E731  (a buffer no tensor uses is passed as NULL)
+            call("hcp_adamw8bit_flat", self.flat.data.data_ptr(), self.flat.grad.data_ptr(), nz(self.a8_codes), nz(self.a8_absmax),
+                 nz(self.a8_state32), self.a8_maps.data_ptr(), lay.tensors.ctypes.data, self.a8_tensors.data_ptr(), len(lay.tensors), lay.items.ctypes.data,
+                 self.a8_items.data_ptr(), lay.items.size, n, lay.code_bytes, lay.nblocks, lay.small_numel, self.a8_hyper.data_ptr(),
+                 self.a8_steps.data_ptr(), len(self.segments), 1.0 / self.world, self.gsq.data_ptr(), float(self.max_norm or 0.0),
+                 stream_ptr())
+        for s in (self.segments if self.optimizer in ("adamw", "lion") else ()):
             lo, cnt = s["lo"], s["hi"] - s["lo"]
             p, g, m = (b.data_ptr() + 4 * lo for b in (self.flat.data, self.flat.grad, self.m))
             tail = (1.0 / self.world, self.gsq.data_ptr(), float(self.max_norm or 0.0), s["step"].data_ptr(), stream_ptr())

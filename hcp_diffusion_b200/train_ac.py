@@ -8,7 +8,8 @@ the H100 engine and save `ckpts/unet-<step>.safetensors` every `train.save_step`
 weight_decay, betas, eps}` for `torch.optim.AdamW` (the default `_target_`), the constructor keys of
 `transformers.optimization.Adafactor` (reference cfgs/train/examples/FT_sdxl.yaml) or of `lion_pytorch.Lion` (`lr, betas,
 weight_decay`, reference cfgs/train/examples/Lion_optimizer.yaml; `use_triton` is accepted and changes nothing, since it only picks
-lion-pytorch's Triton kernel for the same arithmetic), `scheduler.{name, num_warmup_steps, num_training_steps, scheduler_kwargs}` (one_cycle / constant /
+lion-pytorch's Triton kernel for the same arithmetic) or of `bitsandbytes.optim.AdamW8bit` (`lr, betas, eps, weight_decay,
+min_8bit_size`; percentile clipping, non-blockwise or paged state, AMSGrad and `args` are refused), `scheduler.{name, num_warmup_steps, num_training_steps, scheduler_kwargs}` (one_cycle / constant /
 constant_with_warmup), `loss.criterion` (`torch.nn.MSELoss` or `hcpdiff.loss.MinSNRLoss`-family `_target_` + `gamma`), `cfg_scale`
 (DreamArtist), `resume.{ckpt_path.unet, start_step}`; `model.ema` (`decay_max`, `inv_gamma`, `power`); `model.noise_scheduler`
 (`noise.resolve`: DDPMScheduler / .from_pretrained, ZeroTerminalScheduler, PyramidNoiseScheduler; `t` is drawn from [0, its
@@ -52,7 +53,7 @@ import time
 import torch
 import torch.distributed as dist
 
-from . import adafactor
+from . import adafactor, adamw8bit
 from .ckpt_manager import CkptManagerPKL, CkptManagerSafe, auto_manager
 from .engine import LoraTrainStep
 from .noise import resolve as resolve_noise_schedule
@@ -86,7 +87,9 @@ def optimizer_from_cfg(opt_cfg):
     """`train.optimizer` -> (engine optimizer, options or None).  No `_target_` or torch.optim.AdamW: AdamW from `lr /
     weight_decay / betas / eps`; transformers.optimization.Adafactor: its constructor keys with transformers' defaults (a manual
     `lr` with `relative_step: True` is refused, as transformers refuses it); lion_pytorch.Lion: {'lr', 'betas', 'weight_decay'}
-    with Lion's defaults (an unknown key is a TypeError, as Lion's constructor raises; `decoupled_weight_decay: True` is refused)."""
+    with Lion's defaults (an unknown key is a TypeError, as Lion's constructor raises; `decoupled_weight_decay: True` is refused);
+    bitsandbytes.optim.AdamW8bit: adamw8bit.check_options (its constructor keys and defaults; the other bitsandbytes optimizers
+    are refused)."""
     target = str((opt_cfg or {}).get("_target_", "torch.optim.AdamW"))
     name = target.rsplit(".", 1)[-1]
     if name == "AdamW" and target.startswith("torch."):
@@ -107,8 +110,13 @@ def optimizer_from_cfg(opt_cfg):
         if len(betas) != 2:
             raise ValueError(f"Lion betas {opts['betas']!r}: two values (beta1, beta2)")
         return "lion", {"lr": float(opts["lr"]), "betas": betas, "weight_decay": float(opts["weight_decay"])}
-    raise NotImplementedError(f"train.optimizer._target_={target!r}: torch.optim.AdamW, transformers.optimization.Adafactor or "
-                              "lion_pytorch.Lion")
+    if target.startswith("bitsandbytes."):
+        if name != "AdamW8bit":
+            raise NotImplementedError(f"train.optimizer._target_={target!r}: of bitsandbytes' optimizers only "
+                                      "bitsandbytes.optim.AdamW8bit is supported")
+        return "adamw8bit", adamw8bit.check_options(kw)
+    raise NotImplementedError(f"train.optimizer._target_={target!r}: torch.optim.AdamW, transformers.optimization.Adafactor, "
+                              "lion_pytorch.Lion or bitsandbytes.optim.AdamW8bit")
 
 
 def data_groups(data_cfg):
@@ -221,8 +229,10 @@ class Trainer:
         lr_scale = bs * self.world * accum if tr.get("scale_lr", False) else 1
         opt_cfg = tr.get("optimizer") or {}
         opt_name, opt_opts = optimizer_from_cfg(opt_cfg)
-        if opt_name == "lion":
+        eps = float(opt_cfg.get("eps", 1e-8))
+        if opt_name in ("lion", "adamw8bit"):
             betas, weight_decay = opt_opts["betas"], opt_opts["weight_decay"]
+            eps = opt_opts.get("eps", eps)          # Lion has none: the engine's default, unread by its kernel
         else:
             betas, weight_decay = tuple(opt_cfg.get("betas", (0.9, 0.999))), float(opt_cfg.get("weight_decay", 1e-2))
         groups, self.lora = make_hcpdiff(self.unet, cfgs.get("unet"), cfgs.get("lora_unet"), default_lr=float(opt_cfg.get("lr", 1e-4)))
@@ -254,11 +264,12 @@ class Trainer:
         loss = loss_from_cfg(tr.get("loss"))
         self.noise_sched = resolve_noise_schedule(cfgs.model.get("noise_scheduler"), loss)
         self.T = self.noise_sched.num_train_timesteps
-        self.step_fn = LoraTrainStep(self.unet, groups, weight_decay=weight_decay, betas=betas, eps=float(opt_cfg.get("eps", 1e-8)),
+        opt_kwargs = {"adafactor": opt_opts, "adamw8bit": {"min_8bit_size": (opt_opts or {}).get("min_8bit_size")}}.get(opt_name)
+        self.step_fn = LoraTrainStep(self.unet, groups, weight_decay=weight_decay, betas=betas, eps=eps,
                                      max_grad_norm=float(tr.get("max_grad_norm", 1.0)), use_cuda_graph=bool(tr.get("cuda_graph", True)),
                                      grad_accum_steps=accum, loss=loss, ema=ema,
                                      cfg_scale=None if cfg_scale in (None, "1.0", 1.0) else str(cfg_scale),
-                                     optimizer=opt_name, optimizer_kwargs=opt_opts if opt_name == "adafactor" else None, text_encoder=self.te, text_encoder_opts=te_opts,
+                                     optimizer=opt_name, optimizer_kwargs=opt_kwargs, text_encoder=self.te, text_encoder_opts=te_opts,
                                      loss_weights=None if self.groups is None else [w for _, _, _, w in self.groups],
                                      noise_scheduler=None if cfgs.model.get("noise_scheduler") is None else self.noise_sched)
         self.step_fn.sync_params(src=0)

@@ -382,6 +382,40 @@ int hcp_adamw_flat_dev(float* p, const float* g, float* m, float* v, int64_t n, 
 int hcp_lion_flat_dev(float* p, const float* g, float* m, int64_t n, const float* hyper_device, float grad_scale,
                       const float* sumsq_device, float max_norm, int* step_device, hcp_stream_t stream);
 
+/* AdamW8bit (bitsandbytes.optim.AdamW8bit: blockwise 8-bit Adam moments) over the tensors of a table.  A tensor in mode 1 keeps
+ * its first and second moments as uint8 codes, code1 at codes + state and code2 at codes + code_bytes + state (numel each), with one
+ * fp32 scale per 256-element block counted from the tensor's first element: absmax1 at absmax + absmax_row, absmax2 at absmax +
+ * nblocks + absmax_row.  Codes decode through maps_device (fp32 [2, 256]: bitsandbytes' signed dynamic map for the first moment,
+ * the unsigned one for the second).  A tensor in mode 0 keeps fp32 m at state32 + state and v at state32 + small_numel + state. */
+typedef struct {
+    int64_t offset;     /* first element in p and g (a multiple of 4) */
+    int64_t numel;
+    int64_t state;      /* mode 1: first code (a multiple of 4); mode 0: first element of m / v (a multiple of 4) */
+    int64_t absmax;     /* mode 1: first block scale; mode 0: unused */
+    int32_t mode;       /* 1: 8-bit blockwise, 0: 32-bit */
+    int32_t group;
+} hcp_adamw8bit_tensor;
+/* Blocks [block0, block1) of one tensor, walked by one CTA.  The items tile every tensor's blocks once, in table order. */
+typedef struct {
+    int32_t tensor, block0, block1, pad;
+} hcp_adamw8bit_item;
+/* The contract of hcp_adamw_flat_dev per group: hyper_device fp32 [ngroups, 5] = {lr, beta1, beta2, eps, weight_decay} rows,
+ * steps_device int32 [ngroups] each advanced once per call (the bias corrections read it; hcp_ema_flat reads group 0's), the gradient
+ * g * grad_scale clipped to max_norm with the device-side sumsq.  Per element, in fp32 (each operation rounded on its own):
+ *   s1 = b1 s1 + (1 - b1) g;  s2 = b2 s2 + (1 - b2) g^2;  p += -lr sqrt(1 - b2^t) / (1 - b1^t) s1 / (sqrt(s2) + eps sqrt(1 - b2^t));
+ *   then, when weight_decay > 0, p *= 1 - lr weight_decay (after the step, as bitsandbytes).
+ * Mode 1: a non-finite g sets both moments to 0 and leaves p; each block's new scale is max |s| over the block after the update,
+ * and s / scale (0 when the scale is 0) is re-encoded with bitsandbytes' search and midpoint rule; a first-moment code of the other
+ * sign than s1 moves one step toward it.  Mode 0 (bitsandbytes' 32-bit path) has no non-finite guard.  tensors_host / items_host
+ * are checked before any launch (inside the buffers, aligned, increasing, the items tiling each tensor once); tensors_device /
+ * items_device are their device copies, which the kernel reads.  p, g, state32 and codes 16-byte aligned, code_bytes a multiple of
+ * 16, small_numel of 4.  An empty table is a no-op.  Two launches; no host synchronisation (CUDA-graph capturable). */
+int hcp_adamw8bit_flat(float* p, const float* g, uint8_t* codes, float* absmax, float* state32, const float* maps_device,
+                       const hcp_adamw8bit_tensor* tensors_host, const hcp_adamw8bit_tensor* tensors_device, int32_t ntensors,
+                       const hcp_adamw8bit_item* items_host, const hcp_adamw8bit_item* items_device, int64_t nitems, int64_t n,
+                       int64_t code_bytes, int64_t nblocks, int64_t small_numel, const float* hyper_device, int* steps_device,
+                       int32_t ngroups, float grad_scale, const float* sumsq_device, float max_norm, hcp_stream_t stream);
+
 /* Adafactor (transformers.optimization.Adafactor.step) over the flat buffer, per tensor of the module's shape.  A tensor with two or
  * more dims is factored over its last two: view [P, R, C], exp_avg_sq_row [P, R] at state+row, exp_avg_sq_col [P, C] at state+col.
  * A 1-D tensor has exp_avg_sq [numel] at state+row, and is walked as P = 1, R = ceil(numel / 256), C = 256. */

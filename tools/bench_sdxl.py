@@ -2,13 +2,14 @@
 resnet / sampler convolutions (locon), batch 2, 1024x1024 (128x128 latent), 77 tokens x 2048.  Prints one JSON line with the step
 time.  Not the benchmark contract (bench.py measures config 2); a reference point for the SDXL rows of DESIGN.md.
 `--full-ft` trains every parameter of the UNet instead (reference cfgs/train/examples/FT_sdxl.yaml), with `--optimizer adamw`,
-`adafactor` (relative_step False, lr 1e-6, weight_decay 1e-3 as there) or `lion` (lr 1e-6, weight_decay 1e-2 as the reference's
-Lion_optimizer.yaml); the line then also gives the optimizer's own time per step.
+`adafactor` (relative_step False, lr 1e-6, weight_decay 1e-3 as there), `lion` (lr 1e-6, weight_decay 1e-2 as the reference's
+Lion_optimizer.yaml) or `adamw8bit` (bitsandbytes' AdamW8bit, weight_decay 1e-3 as cfgs/train/ft_adamw8bit_sdxl_synthetic.yaml);
+the line then also gives the optimizer's own time per step.
 `--lora-te` times, in the same run, the step above and then the same step with SDXL's two text encoders (CLIP-L + OpenCLIP-bigG,
 full size, random init) in front, LoRA rank 4 on their self_attn + mlp layers (reference cfgs/train/examples/lora_sdxl.yaml's
 lora_text_encoder item, clip_skip 1, no final norm): the line gives both step times, the card and its power limit.
 
-  python tools/bench_sdxl.py [--batch 2] [--steps 5] [--no-locon] [--full-ft --optimizer adafactor|lion] [--lora-te]
+  python tools/bench_sdxl.py [--batch 2] [--steps 5] [--no-locon] [--full-ft --optimizer adafactor|lion|adamw8bit] [--lora-te]
 """
 import argparse
 import json
@@ -31,7 +32,7 @@ ap.add_argument("--latent", type=int, default=128)
 ap.add_argument("--rank", type=int, default=16)
 ap.add_argument("--no-locon", action="store_true")
 ap.add_argument("--full-ft", action="store_true")
-ap.add_argument("--optimizer", choices=("adamw", "adafactor", "lion"), default="adamw")
+ap.add_argument("--optimizer", choices=("adamw", "adafactor", "lion", "adamw8bit"), default="adamw")
 ap.add_argument("--lora-te", action="store_true")
 args = ap.parse_args()
 if args.lora_te and (args.full_ft or args.optimizer != "adamw"):
@@ -89,6 +90,8 @@ if args.optimizer == "adafactor":
     step = LoraTrainStep(unet, groups, optimizer="adafactor", optimizer_kwargs={"relative_step": False, "weight_decay": 1e-3})
 elif args.optimizer == "lion":
     step = LoraTrainStep(unet, groups if args.full_ft else params, optimizer="lion", weight_decay=1e-2)
+elif args.optimizer == "adamw8bit":
+    step = LoraTrainStep(unet, groups if args.full_ft else params, optimizer="adamw8bit", weight_decay=1e-3)
 else:
     step = LoraTrainStep(unet, groups if args.full_ft else params)
 B, S = args.batch, args.latent
