@@ -151,7 +151,7 @@ EXPORTS = [
     "hcp_lora_pack", "hcp_lora_merge", "hcp_lora_pack_conv", "hcp_lora_grad", "hcp_lora_grad_pair", "hcp_lora_grad_conv3x3", "hcp_add_noise", "hcp_mse_loss", "hcp_sumsq", "hcp_adamw_flat",
     "hcp_adamw_flat_dev", "hcp_lion_flat_dev", "hcp_snr_mse_loss", "hcp_ema_flat", "hcp_dropout_bf16", "hcp_counter_add_u64", "hcp_cfg_mix_f32",
     "hcp_wgrad_bf16", "hcp_wgrad_conv3x3_bf16", "hcp_colsum_bf16", "hcp_norm_affine_grad_bf16", "hcp_small_linear_bwd_f32", "hcp_silu_f32",
-    "hcp_conv_in_wgrad_f32", "hcp_conv_out_wgrad_f32", "hcp_repack_weights", "hcp_adafactor_flat", "hcp_adamw8bit_flat",
+    "hcp_conv_in_wgrad_f32", "hcp_conv_out_wgrad_f32", "hcp_repack_weights", "hcp_adafactor_flat", "hcp_adamw8bit_flat", "hcp_prodigy_flat",
     "hcp_attn_fwd_causal_bf16", "hcp_attn_bwd_causal_bf16", "hcp_quick_gelu_fwd_bf16", "hcp_quick_gelu_bwd_bf16", "hcp_embed_gather_bf16",
     "hcp_sum_bf16_to_f32", "hcp_gelu_fwd_bf16", "hcp_gelu_bwd_bf16", "hcp_eps_loss_grouped_workspace_bytes", "hcp_eps_loss_grouped",
     "hcp_pyramid_plan", "hcp_pyramid_workspace_bytes", "hcp_pyramid_noise", "hcp_add_noise_scaled",
@@ -242,7 +242,8 @@ def lib() -> C.CDLL:
             l.hcp_repack_weights.argtypes = [vp, i64, vp]
             l.hcp_cfg_mix_f32.argtypes = [vp, vp, vp, i64, i64, f32, f32, C.c_int32, C.c_int32, vp, vp]
             f64 = C.c_double
-            l.hcp_pyramid_plan.argtypes = [vp, C.c_int32, C.c_int32, f64, i64, i64, vp, vp]
+            l.hcp_prodigy_flat.argtypes = [vp, vp, vp, vp, vp, vp, i64, vp, vp, C.c_int32, vp, vp, vp, C.c_size_t, f32, vp, f32, vp, vp]
+            l.hcp_pyramid_plan.argtypes =[vp, C.c_int32, C.c_int32, f64, i64, i64, vp, vp]
             l.hcp_pyramid_workspace_bytes.restype = C.c_size_t
             l.hcp_pyramid_workspace_bytes.argtypes = [i64, i64, i64, i64, C.c_int32, f64]
             l.hcp_pyramid_noise.argtypes = [vp, vp, vp, C.c_int32, vp, C.c_int32, f64, f64, i64, i64, i64, i64, vp, vp, vp, C.c_size_t, vp]

@@ -1,7 +1,7 @@
 // SPDX-License-Identifier: Apache-2.0
 // Adafactor (transformers.optimization.Adafactor.step) over the flat fp32 parameter buffer of the training step (sm_90a), and
-// Lion (lion_pytorch.Lion.step, one elementwise kernel) and AdamW8bit (bitsandbytes.optim.AdamW8bit, blockwise 8-bit moments), both
-// near the end of this file.
+// Lion (lion_pytorch.Lion.step, one elementwise kernel), Prodigy (prodigyopt.Prodigy, a device-side step size d from a global
+// reduction) and AdamW8bit (bitsandbytes.optim.AdamW8bit, blockwise 8-bit moments), near the end of this file.
 //
 // Every trainable tensor keeps its module shape: a tensor with two or more dims is factored over its LAST TWO dims, viewed as
 // [P, R, C] with the leading dims a batch (a Conv2d weight [O, I, 3, 3] is P = O*I slabs of 3 x 3); a 1-D tensor keeps an
@@ -491,6 +491,197 @@ __global__ void __launch_bounds__(A8_T, 4) adamw8bit_kernel(float* __restrict__ 
     }
 }
 
+// Prodigy (prodigyopt.Prodigy.step; Mishchenko & Defazio 2023) over segments of the flat buffer, in three launches:
+//   (1) prodigy_stats_kernel: per element of every segment, g' = g * gscale_clip (+ wd p when decay is coupled); on the first call
+//       p0 = p and s = m = v = 0; in a segment with lr > 0:  m = b1 m + d (1 - b1) g';  v = b2 v + d^2 (1 - b2) g'^2;
+//       s = b3 s + (d / d0) (safeguard_warmup ? d : dlr) g'.  Per-CTA fp64 partials of sum g' (p0 - p) and sum |s| go to the
+//       workspace (per thread in element order, then a fixed shuffle tree).
+//   (2) prodigy_scalars_kernel: one CTA sums the partials in a fixed order and updates d, d_max, D_num, k (or marks the call
+//       skipped when sum |s| == 0), and advances the EMA step counter.
+//   (3) prodigy_apply_kernel: unless skipped, p = p - wd dlr p (decoupled decay) and p = p - dlr m / (sqrt(v) + d eps) with the
+//       old dlr and the new d, read from the scalar block.
+// d, dlr and the other scalars are fp64 (the reference keeps them as Python floats); the coefficients an element sees are rounded
+// to fp32 once, as torch's fp32 ops round a Python scalar.  16-byte accesses, the count % 4 tail of a segment by one CTA.
+constexpr int PD_T = 256;
+enum { PD_BIAS_CORRECTION = 1, PD_SAFEGUARD_WARMUP = 2, PD_DECOUPLE = 4 };
+enum { PD_D = 0, PD_DMAX = 1, PD_DNUM = 2, PD_K = 3, PD_INIT = 4, PD_SKIP = 5, PD_DLR = 6 };
+
+// the largest segment lr, over the whole CTA (every thread gets it)
+__device__ __forceinline__ double pd_max_lr(const hcp_prodigy_segment* __restrict__ segs, int nsegs, double* s_red) {
+    double mx = 0.0;
+    for (int i = threadIdx.x; i < nsegs; i += PD_T) mx = fmax(mx, segs[i].lr);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mx = fmax(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = mx;
+    __syncthreads();
+    mx = s_red[0];
+    for (int w = 1; w < PD_T / 32; ++w) mx = fmax(mx, s_red[w]);
+    __syncthreads();
+    return mx;
+}
+
+// dlr = d lr bc of the step about to run (old d, k), identical in launches (1) and (2)
+__device__ __forceinline__ double pd_dlr(const double* __restrict__ hy, const double* __restrict__ st, double lr) {
+    double bc = 1.0;
+    if ((int)hy[7] & PD_BIAS_CORRECTION) {
+        const double k1 = st[PD_K] + 1.0;
+        bc = sqrt(1.0 - pow(hy[1], k1)) / (1.0 - pow(hy[0], k1));
+    }
+    return st[PD_D] * lr * bc;
+}
+
+template <typename TV>
+__device__ __forceinline__ TV pd_block_sum(TV v, TV* s_red) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    TV t = 0;
+    if (threadIdx.x == 0)
+        for (int w = 0; w < PD_T / 32; ++w) t += s_red[w];
+    __syncthreads();
+    return t;                                          // valid in thread 0
+}
+
+__global__ void __launch_bounds__(PD_T) prodigy_stats_kernel(const float* __restrict__ p, const float* __restrict__ g, float* __restrict__ p0,
+                                                             float* __restrict__ s, float* __restrict__ m, float* __restrict__ v,
+                                                             const hcp_prodigy_segment* __restrict__ segs, int nsegs,
+                                                             const double* __restrict__ hy, const double* __restrict__ st,
+                                                             double* __restrict__ work, float gscale, const float* __restrict__ sumsq,
+                                                             float max_norm) {
+    pdl_trigger();
+    pdl_wait();
+    __shared__ double s_red[PD_T / 32];
+    const double lr = pd_max_lr(segs, nsegs, s_red);
+    const double d = st[PD_D], dlr = pd_dlr(hy, st, lr), d0 = hy[4];
+    const int flags = (int)hy[7];
+    const bool first = st[PD_INIT] == 0.0, coupled = !(flags & PD_DECOUPLE);
+    const float b1 = (float)hy[0], b2 = (float)hy[1], b3 = (float)hy[2];
+    const float cm = (float)(d * (1.0 - hy[0])), cv = (float)(d * d * (1.0 - hy[1]));
+    const float cs = (float)((d / d0) * ((flags & PD_SAFEGUARD_WARMUP) ? d : dlr));
+    const float gs = af_grad_scale(gscale, sumsq, max_norm);
+    double dot = 0.0, den = 0.0;
+    for (int si = 0; si < nsegs; ++si) {
+        const hcp_prodigy_segment sg = segs[si];
+        const bool live = sg.lr > 0.0;
+        if (!live && !first) continue;                 // an lr-0 segment only decays, in (3)
+        const float wd = coupled ? (float)sg.weight_decay : 0.f;
+        auto upd = [&](float w, float gr, float& q0, float& si_, float& mi, float& vi) {
+            gr *= gs;
+            if (wd != 0.f) gr += wd * w;
+            if (first) { q0 = w; si_ = 0.f; mi = 0.f; vi = 0.f; }
+            if (live) {
+                dot += (double)gr * ((double)q0 - (double)w);
+                mi = b1 * mi + cm * gr;
+                vi = b2 * vi + cv * gr * gr;
+                si_ = b3 * si_ + cs * gr;
+                den += fabs((double)si_);
+            }
+        };
+        const float* ps = p + sg.offset;
+        const float* gg = g + sg.offset;
+        float *q = p0 + sg.offset, *ss = s + sg.offset, *ms = m + sg.offset, *vs = v + sg.offset;
+        const int64_t n4 = sg.count >> 2, stride = (int64_t)gridDim.x * PD_T;
+        for (int64_t i = blockIdx.x * (int64_t)PD_T + threadIdx.x; i < n4; i += stride) {
+            const float4 w4 = reinterpret_cast<const float4*>(ps)[i], g4 = reinterpret_cast<const float4*>(gg)[i];
+            float4 q4 = make_float4(0.f, 0.f, 0.f, 0.f), s4 = q4, m4 = q4, v4 = q4;
+            if (!first) {
+                q4 = reinterpret_cast<const float4*>(q)[i]; s4 = reinterpret_cast<const float4*>(ss)[i];
+                m4 = reinterpret_cast<const float4*>(ms)[i]; v4 = reinterpret_cast<const float4*>(vs)[i];
+            }
+            upd(w4.x, g4.x, q4.x, s4.x, m4.x, v4.x); upd(w4.y, g4.y, q4.y, s4.y, m4.y, v4.y);
+            upd(w4.z, g4.z, q4.z, s4.z, m4.z, v4.z); upd(w4.w, g4.w, q4.w, s4.w, m4.w, v4.w);
+            if (first) reinterpret_cast<float4*>(q)[i] = q4;
+            reinterpret_cast<float4*>(ss)[i] = s4; reinterpret_cast<float4*>(ms)[i] = m4; reinterpret_cast<float4*>(vs)[i] = v4;
+        }
+        if ((int)blockIdx.x == si % (int)gridDim.x && threadIdx.x < (sg.count & 3)) {
+            const int64_t i = (n4 << 2) + threadIdx.x;
+            float q0 = first ? 0.f : q[i], si_ = first ? 0.f : ss[i], mi = first ? 0.f : ms[i], vi = first ? 0.f : vs[i];
+            upd(ps[i], gg[i], q0, si_, mi, vi);
+            if (first) q[i] = q0;
+            ss[i] = si_; ms[i] = mi; vs[i] = vi;
+        }
+    }
+    dot = pd_block_sum(dot, s_red);
+    den = pd_block_sum(den, s_red);
+    if (threadIdx.x == 0) {
+        work[2 * blockIdx.x] = dot;
+        work[2 * blockIdx.x + 1] = den;
+    }
+}
+
+__global__ void __launch_bounds__(PD_T) prodigy_scalars_kernel(const hcp_prodigy_segment* __restrict__ segs, int nsegs,
+                                                               const double* __restrict__ hy, double* __restrict__ st,
+                                                               const double* __restrict__ work, int nblocks, int* __restrict__ step_ptr) {
+    pdl_trigger();
+    pdl_wait();
+    __shared__ double s_red[PD_T / 32];
+    const double lr = pd_max_lr(segs, nsegs, s_red);
+    double dot = 0.0, den = 0.0;
+    for (int b = threadIdx.x; b < nblocks; b += PD_T) {
+        dot += work[2 * b];
+        den += work[2 * b + 1];
+    }
+    dot = pd_block_sum(dot, s_red);
+    den = pd_block_sum(den, s_red);
+    if (threadIdx.x != 0) return;
+    *step_ptr += 1;                                    // ModelEMA counts every optimizer call, skipped or not
+    double d = st[PD_D], d_max = st[PD_DMAX];
+    const double d0 = hy[4], dlr = pd_dlr(hy, st, lr);
+    const double d_num = hy[2] * st[PD_DNUM] + (d / d0) * dlr * dot;
+    st[PD_INIT] = 1.0;
+    if (den == 0.0) {                                  // no progress: p, d, d_max, D_num and k stay
+        st[PD_SKIP] = 1.0;
+        return;
+    }
+    if (lr > 0.0) {
+        const double d_hat = hy[5] * d_num / den;
+        if (d == d0) d = fmax(d, d_hat);
+        d_max = fmax(d_max, d_hat);
+        d = fmin(d_max, d * hy[6]);
+    }
+    st[PD_D] = d;
+    st[PD_DMAX] = d_max;
+    st[PD_DNUM] = d_num;
+    st[PD_K] += 1.0;
+    st[PD_SKIP] = 0.0;
+    st[PD_DLR] = dlr;
+}
+
+__global__ void __launch_bounds__(PD_T) prodigy_apply_kernel(float* __restrict__ p, const float* __restrict__ m, const float* __restrict__ v,
+                                                             const hcp_prodigy_segment* __restrict__ segs, int nsegs,
+                                                             const double* __restrict__ hy, const double* __restrict__ st) {
+    pdl_trigger();
+    pdl_wait();
+    if (st[PD_SKIP] != 0.0) return;
+    const double dlr = st[PD_DLR];
+    const float step = (float)(-dlr), deps = (float)(st[PD_D] * hy[3]);
+    const bool decouple = (int)hy[7] & PD_DECOUPLE;
+    for (int si = 0; si < nsegs; ++si) {
+        const hcp_prodigy_segment sg = segs[si];
+        const float decay = (decouple && sg.weight_decay != 0.0) ? (float)(-sg.weight_decay * dlr) : 0.f;
+        auto upd = [&](float& w, float mi, float vi) {
+            if (decay != 0.f) w = w + w * decay;
+            w = w + step * (mi / (sqrtf(vi) + deps));
+        };
+        float* ps = p + sg.offset;
+        const float *ms = m + sg.offset, *vs = v + sg.offset;
+        const int64_t n4 = sg.count >> 2, stride = (int64_t)gridDim.x * PD_T;
+        for (int64_t i = blockIdx.x * (int64_t)PD_T + threadIdx.x; i < n4; i += stride) {
+            float4 w4 = reinterpret_cast<float4*>(ps)[i];
+            const float4 m4 = reinterpret_cast<const float4*>(ms)[i], v4 = reinterpret_cast<const float4*>(vs)[i];
+            upd(w4.x, m4.x, v4.x); upd(w4.y, m4.y, v4.y); upd(w4.z, m4.z, v4.z); upd(w4.w, m4.w, v4.w);
+            reinterpret_cast<float4*>(ps)[i] = w4;
+        }
+        if ((int)blockIdx.x == si % (int)gridDim.x && threadIdx.x < (sg.count & 3)) {
+            const int64_t i = (n4 << 2) + threadIdx.x;
+            float w = ps[i];
+            upd(w, ms[i], vs[i]);
+            ps[i] = w;
+        }
+    }
+}
+
 }  // namespace hcp
 
 using namespace hcp;
@@ -531,6 +722,44 @@ extern "C" int hcp_lion_flat_dev(float* p, const float* g, float* m, int64_t n, 
     launch_k(lion_flat_dev_kernel, dim3((unsigned)blocks), dim3(256), 0, (cudaStream_t)st, p, g, m, n, hyper_device, grad_scale,
              sumsq_device, max_norm, step_device);
     LAUNCH_CHECK("lion_dev launch");
+    return HCP_OK;
+}
+
+extern "C" int hcp_prodigy_flat(float* p, const float* g, float* p0, float* s, float* m, float* v, int64_t n,
+                                const hcp_prodigy_segment* segs_host, const hcp_prodigy_segment* segs_device, int32_t nsegs,
+                                const double* hyper_device, double* state_device, double* workspace, size_t workspace_bytes,
+                                float grad_scale, const float* sumsq_device, float max_norm, int* step_device, hcp_stream_t st) {
+    if (!p || !g || !p0 || !s || !m || !v || !segs_host || !segs_device || !hyper_device || !state_device || !workspace || !step_device)
+        return set_error(HCP_ERR_INVALID, "prodigy: null pointer");
+    if (n < 0 || nsegs < 0) return set_error(HCP_ERR_INVALID, "prodigy: negative size");
+    if (!aligned16(p, g, p0, s, m, v) || ((uintptr_t)workspace & 7) || ((uintptr_t)hyper_device & 7) || ((uintptr_t)state_device & 7) ||
+        ((uintptr_t)segs_device & 7))
+        return set_error(HCP_ERR_INVALID, "prodigy: p / g / p0 / s / m / v must be 16-byte aligned, the tables 8-byte aligned");
+    if (workspace_bytes < (size_t)HCP_PRODIGY_WORKSPACE_BYTES) return set_error(HCP_ERR_INVALID, "prodigy: workspace too small");
+    int64_t end = 0, total = 0;
+    for (int32_t i = 0; i < nsegs; ++i) {
+        const hcp_prodigy_segment& sg = segs_host[i];
+        if (sg.count < 0 || sg.offset < end || (sg.offset & 3) || sg.count > n - sg.offset)
+            return set_error(HCP_ERR_INVALID, "prodigy: segment outside [0, n), overlapping, negative or off 16-byte alignment");
+        end = sg.offset + sg.count;
+        total += sg.count;
+    }
+    if (total == 0) return HCP_OK;
+    const cudaStream_t cs = (cudaStream_t)st;
+    int64_t blocks = ((total >> 2) + PD_T - 1) / PD_T;
+    if (blocks > num_sms() * 4) blocks = num_sms() * 4;          // one resident wave: the partials are one per CTA
+    if (blocks > HCP_PRODIGY_WORKSPACE_BYTES / 16) blocks = HCP_PRODIGY_WORKSPACE_BYTES / 16;
+    if (blocks < 1) blocks = 1;
+    int64_t ablocks = ((total >> 2) + PD_T - 1) / PD_T;          // the update has no partials: lion's grid
+    if (ablocks > num_sms() * 16) ablocks = num_sms() * 16;
+    if (ablocks < 1) ablocks = 1;
+    launch_k(prodigy_stats_kernel, dim3((unsigned)blocks), dim3(PD_T), 0, cs, (const float*)p, g, p0, s, m, v, segs_device, (int)nsegs,
+             hyper_device, (const double*)state_device, workspace, grad_scale, sumsq_device, max_norm);
+    launch_k(prodigy_scalars_kernel, dim3(1), dim3(PD_T), 0, cs, segs_device, (int)nsegs, hyper_device, state_device,
+             (const double*)workspace, (int)blocks, step_device);
+    launch_k(prodigy_apply_kernel, dim3((unsigned)ablocks), dim3(PD_T), 0, cs, p, (const float*)m, (const float*)v, segs_device, (int)nsegs,
+             hyper_device, (const double*)state_device);
+    LAUNCH_CHECK("prodigy launch");
     return HCP_OK;
 }
 

@@ -24,7 +24,7 @@ import torch
 import torch.distributed as dist
 from torch import nn
 
-from . import _lib, adafactor, adamw8bit, ops
+from . import _lib, adafactor, adamw8bit, ops, prodigy
 from ._lib import call, stream_ptr
 from .models.clip import SDXLTextEncoder, encode_prompt, encode_prompt_sdxl
 from .noise import resolve as resolve_noise_schedule
@@ -165,7 +165,7 @@ class _CfgMixFn(torch.autograd.Function):
 
 class LoraTrainStep:
     """One optimisation step of LoRA (or full) training on a `UNet2DConditionModel`: eps-prediction loss, grad-norm clip, AdamW
-    (or Adafactor, Lion or AdamW8bit).
+    (or Adafactor, Lion, AdamW8bit or Prodigy).
 
     `params`: parameters, or optimizer-style groups [{'params': [...], 'lr': ..., 'weight_decay': ...}] (one per `lora_unet:` /
     `unet:` config item, reference cfg_net_tools.py:96-127).  `grad_accum_steps`: micro-batches per optimizer step
@@ -183,7 +183,11 @@ class LoraTrainStep:
     (`lr`, `betas`, `eps`, `weight_decay` with AdamW's defaults; `optimizer_kwargs` takes its constructor keys -- those four win
     over the arguments when given, and `min_8bit_size`, default 4096 -- and refuses the options adamw8bit.check_options refuses):
     tensors of at least min_8bit_size elements keep both moments as 8-bit codes with one fp32 scale per 256-element block (about
-    2 B per parameter), smaller ones fp32 moments; weight decay is applied after the step, as bitsandbytes applies it.
+    2 B per parameter), smaller ones fp32 moments; weight decay is applied after the step, as bitsandbytes applies it.  'prodigy'
+    is prodigyopt.Prodigy (`lr`, `betas`, `eps`, `weight_decay` with its defaults 1.0, (0.9, 0.999), 1e-8, 0.0; `optimizer_kwargs`
+    takes `beta3`, `d0`, `d_coef`, `growth_rate`, `use_bias_correction`, `safeguard_warmup`, `decouple`): p0, s, m, v per
+    parameter (16 B) and the step size d estimated on the device; every group's lr must be the largest lr or 0, as prodigyopt
+    requires.
 
     `text_encoder`: a `models.CLIPTextModel` whose LoRA adapters train together with the UNet's (the reference's `lora_text_encoder`,
     `TEUnetWrapper`); its adapter parameters must be among `params` (their own groups), so they share the flat buffer: one all-reduce,
@@ -203,7 +207,7 @@ class LoraTrainStep:
     micro-step (`ops.PyramidNoise`; seed it with `set_noise_seed`), and the loss target is the un-normalised pyramid sum, as in the
     reference."""
 
-    def __init__(self, unet: nn.Module, params: Union[Iterable[nn.Parameter], Sequence[dict]], lr: float = 1e-4, betas=None,
+    def __init__(self, unet: nn.Module, params: Union[Iterable[nn.Parameter], Sequence[dict]], lr: Optional[float] = None, betas=None,
                  eps: float = 1e-8, weight_decay: Optional[float] = None, max_grad_norm: float = 1.0, use_cuda_graph: bool = True,
                  process_group: Optional[dist.ProcessGroup] = None, side_stream: bool = True, grad_accum_steps: int = 1,
                  loss: Union[None, str, dict] = None, ema: Optional[dict] = None, cfg_scale=None,
@@ -233,14 +237,17 @@ class LoraTrainStep:
                     "SDXL with n_repeats > 1 (tokenizer_repeats) is not supported: the reference pools bigG's text_embeds at the "
                     "largest id of the raw tokenizer output before it is cut into 77-token chunks, which pre-chunked ids cannot "
                     "express (the reference's SDXL config uses tokenizer_repeats: 1)")
-        if optimizer not in ("adamw", "adafactor", "lion", "adamw8bit"):
-            raise ValueError(f"optimizer {optimizer!r}: one of 'adamw', 'adafactor', 'lion', 'adamw8bit'")
+        if optimizer not in ("adamw", "adafactor", "lion", "adamw8bit", "prodigy"):
+            raise ValueError(f"optimizer {optimizer!r}: one of 'adamw', 'adafactor', 'lion', 'adamw8bit', 'prodigy'")
         self.optimizer = optimizer
-        default_betas, default_wd = ((0.9, 0.99), 0.0) if optimizer == "lion" else ((0.9, 0.999), 1e-2)
+        default_betas, default_wd = {"lion": ((0.9, 0.99), 0.0), "prodigy": ((0.9, 0.999), 0.0)}.get(optimizer, ((0.9, 0.999), 1e-2))
         betas = default_betas if betas is None else tuple(betas)
         weight_decay = default_wd if weight_decay is None else weight_decay
-        af_opts = a8_opts = None
-        if optimizer == "adamw8bit":
+        lr = (1.0 if optimizer == "prodigy" else 1e-4) if lr is None else lr
+        af_opts = a8_opts = pd_opts = None
+        if optimizer == "prodigy":
+            pd_opts = prodigy.engine_options(optimizer_kwargs)
+        elif optimizer == "adamw8bit":
             given = dict(optimizer_kwargs or {})
             a8_opts = adamw8bit.check_options(given)
             lr = a8_opts["lr"] if "lr" in given else lr
@@ -260,6 +267,8 @@ class LoraTrainStep:
                       for g in params if len(list(g["params"]))]
         else:
             groups = [{"params": params, "lr": float(lr), "weight_decay": float(weight_decay)}]
+        if pd_opts is not None:
+            prodigy.check_lrs([g["lr"] for g in groups])
         seen, flat_list = set(), []
         for g in groups:                                   # a parameter belongs to the first group that names it (torch.optim raises)
             g["params"] = [p for p in dict.fromkeys(g["params"]) if id(p) not in seen]
@@ -277,6 +286,8 @@ class LoraTrainStep:
             self._init_adafactor(groups, af_opts)
         elif a8_opts is not None:
             self._init_adamw8bit(groups, a8_opts, betas, eps)
+        elif pd_opts is not None:
+            self._init_prodigy(groups, pd_opts, betas, eps)
         else:
             self.m = torch.zeros_like(self.flat.data)
             self.v = torch.zeros_like(self.flat.data) if optimizer == "adamw" else None
@@ -293,6 +304,9 @@ class LoraTrainStep:
             elif a8_opts is not None:                      # rows of the [groups, 5] table the AdamW8bit kernel reads
                 gi = len(self.segments)
                 hyper, step = self.a8_hyper[gi], self.a8_steps[gi:gi + 1]
+            elif pd_opts is not None:                      # {offset, count, lr, weight_decay} rows the Prodigy kernels read
+                gi = len(self.segments)
+                hyper, step = self.pd_segs_f64[gi, 2:], self.pd_step
             else:
                 hyper = torch.tensor([g["lr"], betas[0], betas[1], eps, g["weight_decay"]], dtype=torch.float32, device=dev)
                 step = torch.zeros(1, dtype=torch.int32, device=dev)
@@ -383,6 +397,24 @@ class LoraTrainStep:
         to_dev = lambda a: torch.from_numpy(a.view(np.uint8).copy()).to(dev)      # noqa: E731  (packed C structs)
         self.a8_tensors, self.a8_items = to_dev(lay.tensors), to_dev(lay.items)
 
+    def _init_prodigy(self, groups, opts, betas, eps):
+        dev = self.flat.data.device
+        groups = [g for g in groups if g["params"]]          # the segments: a group emptied by de-duplication has none
+        rows, i0 = [], 0
+        for g in groups:
+            lo, hi = self.flat.offsets[i0], self.flat.end_of(i0 + len(g["params"]) - 1)
+            rows.append((lo, hi - lo, g["lr"], g["weight_decay"]))
+            i0 += len(g["params"])
+        self.pd_segs_host = prodigy.segment_table(rows)
+        self.pd_segs = torch.from_numpy(self.pd_segs_host.view(np.int64).reshape(len(rows), 4).copy()).to(dev)
+        self.pd_segs_f64 = self.pd_segs.view(torch.float64)  # columns 2, 3: lr, weight_decay (set_lr / set_hyper write lr here)
+        self.pd_hyper = torch.tensor(prodigy.hyper_row(opts, betas[0], betas[1], eps), dtype=torch.float64, device=dev)
+        self.pd_state = torch.tensor(prodigy.initial_state(opts["d0"]), dtype=torch.float64, device=dev)
+        self.pd_work = torch.zeros(prodigy.WORKSPACE_BYTES // 8, dtype=torch.float64, device=dev)
+        self.pd_step = torch.zeros(1, dtype=torch.int32, device=dev)   # optimizer calls, skipped ones included (ModelEMA's step)
+        self.pd_p0, self.pd_s = torch.zeros_like(self.flat.data), torch.zeros_like(self.flat.data)
+        self.m, self.v = torch.zeros_like(self.flat.data), torch.zeros_like(self.flat.data)
+
     @property
     def optimizer_state_bytes(self) -> int:
         """Bytes of optimizer state (moments; not the parameters, gradients or scratch)."""
@@ -390,11 +422,15 @@ class LoraTrainStep:
             return sum(b.numel() * b.element_size() for b in (self.a8_codes, self.a8_absmax, self.a8_state32))
         if self.optimizer == "adafactor":
             return 4 * (self.af_state.numel() + (0 if self.af_exp_avg is None else self.af_exp_avg.numel()))
+        if self.optimizer == "prodigy":
+            return 4 * sum(b.numel() for b in (self.pd_p0, self.pd_s, self.m, self.v))
         return 4 * sum(b.numel() for b in (self.m, self.v) if b is not None)
 
     def _opt_buffers(self) -> List[torch.Tensor]:
         if self.optimizer == "adamw8bit":
             return [self.a8_codes, self.a8_absmax, self.a8_state32, self.a8_steps]
+        if self.optimizer == "prodigy":
+            return [self.pd_p0, self.pd_s, self.m, self.v, self.pd_state, self.pd_step]
         if self.optimizer == "adafactor":
             return [self.af_state, self.af_steps] + ([] if self.af_exp_avg is None else [self.af_exp_avg])
         return [b for b in (self.m, self.v) if b is not None] + [s["step"] for s in self.segments]
@@ -409,8 +445,14 @@ class LoraTrainStep:
             s["lr"].fill_(s["base_lr"] * ratio)
 
     def set_hyper(self, group: int, lr: Optional[float] = None, beta1: Optional[float] = None):
-        """What an LR scheduler writes per step (OneCycleLR cycles the lr and, for AdamW, AdamW8bit and Lion, beta1): device-side,
-        graph-replay safe."""
+        """What an LR scheduler writes per step (OneCycleLR cycles the lr and, for AdamW, AdamW8bit, Lion and Prodigy, beta1):
+        device-side, graph-replay safe.  Prodigy reads the betas of group 0 only, as prodigyopt does."""
+        if self.optimizer == "prodigy":
+            if lr is not None:
+                self.segments[group]["lr"].fill_(lr)
+            if beta1 is not None and group == 0:
+                self.pd_hyper[0:1].fill_(beta1)
+            return
         h = self.segments[group]["hyper"]
         if lr is not None:
             h[0:1].fill_(lr)
@@ -510,6 +552,11 @@ class LoraTrainStep:
                  self.a8_items.data_ptr(), lay.items.size, n, lay.code_bytes, lay.nblocks, lay.small_numel, self.a8_hyper.data_ptr(),
                  self.a8_steps.data_ptr(), len(self.segments), 1.0 / self.world, self.gsq.data_ptr(), float(self.max_norm or 0.0),
                  stream_ptr())
+        elif self.optimizer == "prodigy":
+            call("hcp_prodigy_flat", self.flat.data.data_ptr(), self.flat.grad.data_ptr(), self.pd_p0.data_ptr(), self.pd_s.data_ptr(),
+                 self.m.data_ptr(), self.v.data_ptr(), n, self.pd_segs_host.ctypes.data, self.pd_segs.data_ptr(), len(self.segments),
+                 self.pd_hyper.data_ptr(), self.pd_state.data_ptr(), self.pd_work.data_ptr(), self.pd_work.numel() * 8, 1.0 / self.world,
+                 self.gsq.data_ptr(), float(self.max_norm or 0.0), self.pd_step.data_ptr(), stream_ptr())
         for s in (self.segments if self.optimizer in ("adamw", "lion") else ()):
             lo, cnt = s["lo"], s["hi"] - s["lo"]
             p, g, m = (b.data_ptr() + 4 * lo for b in (self.flat.data, self.flat.grad, self.m))

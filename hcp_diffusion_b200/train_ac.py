@@ -9,7 +9,9 @@ weight_decay, betas, eps}` for `torch.optim.AdamW` (the default `_target_`), the
 `transformers.optimization.Adafactor` (reference cfgs/train/examples/FT_sdxl.yaml) or of `lion_pytorch.Lion` (`lr, betas,
 weight_decay`, reference cfgs/train/examples/Lion_optimizer.yaml; `use_triton` is accepted and changes nothing, since it only picks
 lion-pytorch's Triton kernel for the same arithmetic) or of `bitsandbytes.optim.AdamW8bit` (`lr, betas, eps, weight_decay,
-min_8bit_size`; percentile clipping, non-blockwise or paged state, AMSGrad and `args` are refused), `scheduler.{name, num_warmup_steps, num_training_steps, scheduler_kwargs}` (one_cycle / constant /
+min_8bit_size`; percentile clipping, non-blockwise or paged state, AMSGrad and `args` are refused) or of `prodigyopt.Prodigy`
+(`lr, betas, beta3, eps, weight_decay, decouple, use_bias_correction, safeguard_warmup, d0, d_coef, growth_rate`; `fsdp_in_use:
+true` and `slice_p` other than 1 are refused), `scheduler.{name, num_warmup_steps, num_training_steps, scheduler_kwargs}` (one_cycle / constant /
 constant_with_warmup), `loss.criterion` (`torch.nn.MSELoss` or `hcpdiff.loss.MinSNRLoss`-family `_target_` + `gamma`), `cfg_scale`
 (DreamArtist), `resume.{ckpt_path.unet, start_step}`; `model.ema` (`decay_max`, `inv_gamma`, `power`); `model.noise_scheduler`
 (`noise.resolve`: DDPMScheduler / .from_pretrained, ZeroTerminalScheduler, PyramidNoiseScheduler; `t` is drawn from [0, its
@@ -53,7 +55,7 @@ import time
 import torch
 import torch.distributed as dist
 
-from . import adafactor, adamw8bit
+from . import adafactor, adamw8bit, prodigy
 from .ckpt_manager import CkptManagerPKL, CkptManagerSafe, auto_manager
 from .engine import LoraTrainStep
 from .noise import resolve as resolve_noise_schedule
@@ -89,7 +91,8 @@ def optimizer_from_cfg(opt_cfg):
     `lr` with `relative_step: True` is refused, as transformers refuses it); lion_pytorch.Lion: {'lr', 'betas', 'weight_decay'}
     with Lion's defaults (an unknown key is a TypeError, as Lion's constructor raises; `decoupled_weight_decay: True` is refused);
     bitsandbytes.optim.AdamW8bit: adamw8bit.check_options (its constructor keys and defaults; the other bitsandbytes optimizers
-    are refused)."""
+    are refused); prodigyopt.Prodigy: prodigy.check_options (its constructor keys and defaults, lr 1.0; an unknown key is a
+    TypeError, `fsdp_in_use: True` and `slice_p` other than 1 are refused)."""
     target = str((opt_cfg or {}).get("_target_", "torch.optim.AdamW"))
     name = target.rsplit(".", 1)[-1]
     if name == "AdamW" and target.startswith("torch."):
@@ -115,8 +118,10 @@ def optimizer_from_cfg(opt_cfg):
             raise NotImplementedError(f"train.optimizer._target_={target!r}: of bitsandbytes' optimizers only "
                                       "bitsandbytes.optim.AdamW8bit is supported")
         return "adamw8bit", adamw8bit.check_options(kw)
+    if name == "Prodigy" and target.startswith("prodigyopt."):
+        return "prodigy", prodigy.check_options(kw)
     raise NotImplementedError(f"train.optimizer._target_={target!r}: torch.optim.AdamW, transformers.optimization.Adafactor, "
-                              "lion_pytorch.Lion or bitsandbytes.optim.AdamW8bit")
+                              "lion_pytorch.Lion, bitsandbytes.optim.AdamW8bit or prodigyopt.Prodigy")
 
 
 def data_groups(data_cfg):
@@ -156,8 +161,9 @@ class _LrOnly(torch.optim.Optimizer):
 
 def make_scheduler(cfg, step_fn: LoraTrainStep):
     """Reference get_scheduler_with_name (hcpdiff/utils/net_utils.py:22-82) driven on a stand-in optimizer with the engine's groups:
-    the real torch schedulers produce the numbers, `step()` copies lr (and OneCycleLR's cycled beta1) to the device.  AdamW and
-    Lion have `betas` (OneCycleLR cycles beta1 on both), so an AdamW stand-in with the engine's betas serves for either."""
+    the real torch schedulers produce the numbers, `step()` copies lr (and OneCycleLR's cycled beta1) to the device.  AdamW,
+    Lion, AdamW8bit and Prodigy have `betas` (OneCycleLR cycles beta1 on each), so an AdamW stand-in with the engine's betas serves
+    for any of them."""
     if not cfg or not cfg.get("name"):
         return None
     name = cfg["name"]
@@ -230,12 +236,13 @@ class Trainer:
         opt_cfg = tr.get("optimizer") or {}
         opt_name, opt_opts = optimizer_from_cfg(opt_cfg)
         eps = float(opt_cfg.get("eps", 1e-8))
-        if opt_name in ("lion", "adamw8bit"):
+        if opt_name in ("lion", "adamw8bit", "prodigy"):
             betas, weight_decay = opt_opts["betas"], opt_opts["weight_decay"]
             eps = opt_opts.get("eps", eps)          # Lion has none: the engine's default, unread by its kernel
         else:
             betas, weight_decay = tuple(opt_cfg.get("betas", (0.9, 0.999))), float(opt_cfg.get("weight_decay", 1e-2))
-        groups, self.lora = make_hcpdiff(self.unet, cfgs.get("unet"), cfgs.get("lora_unet"), default_lr=float(opt_cfg.get("lr", 1e-4)))
+        default_lr = opt_opts["lr"] if opt_name == "prodigy" else float(opt_cfg.get("lr", 1e-4))
+        groups, self.lora = make_hcpdiff(self.unet, cfgs.get("unet"), cfgs.get("lora_unet"), default_lr=default_lr)
         groups = [{"params": g["params"], "lr": float(g["lr"]) * lr_scale} for g in groups if len(g["params"])]
         self.te, self.te_lora, te_opts = self._build_text_encoder(cfgs)
         if self.te is not None:
@@ -264,7 +271,8 @@ class Trainer:
         loss = loss_from_cfg(tr.get("loss"))
         self.noise_sched = resolve_noise_schedule(cfgs.model.get("noise_scheduler"), loss)
         self.T = self.noise_sched.num_train_timesteps
-        opt_kwargs = {"adafactor": opt_opts, "adamw8bit": {"min_8bit_size": (opt_opts or {}).get("min_8bit_size")}}.get(opt_name)
+        opt_kwargs = {"adafactor": opt_opts, "adamw8bit": {"min_8bit_size": (opt_opts or {}).get("min_8bit_size")},
+                      "prodigy": {k: (opt_opts or {}).get(k) for k in prodigy.ENGINE_KEYS}}.get(opt_name)
         self.step_fn = LoraTrainStep(self.unet, groups, weight_decay=weight_decay, betas=betas, eps=eps,
                                      max_grad_norm=float(tr.get("max_grad_norm", 1.0)), use_cuda_graph=bool(tr.get("cuda_graph", True)),
                                      grad_accum_steps=accum, loss=loss, ema=ema,

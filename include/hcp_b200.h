@@ -382,6 +382,39 @@ int hcp_adamw_flat_dev(float* p, const float* g, float* m, float* v, int64_t n, 
 int hcp_lion_flat_dev(float* p, const float* g, float* m, int64_t n, const float* hyper_device, float grad_scale,
                       const float* sumsq_device, float max_norm, int* step_device, hcp_stream_t stream);
 
+/* Prodigy (prodigyopt.Prodigy.step) over segments (parameter groups) of the flat buffers p, g, p0, s, m, v (fp32, 16-byte
+ * aligned; p0 / s / m / v are Prodigy's per-element state).  segs: [nsegs] in increasing, non-overlapping order inside [0, n), each
+ * offset a multiple of 4; segs_host is checked before any launch, segs_device (its device copy) is what the kernels read, so a
+ * scheduler rewrites `lr` there between CUDA-graph replays.  Every segment's lr must be the table's largest lr or 0 (prodigyopt
+ * raises otherwise; the caller keeps that rule).
+ * hyper_device fp64 [HCP_PRODIGY_HYPER] = {beta1, beta2, beta3, eps, d0, d_coef, growth_rate, flags}, flags = 1 use_bias_correction
+ * | 2 safeguard_warmup | 4 decouple (beta1 may be rewritten between replays: OneCycleLR).  state_device fp64 [HCP_PRODIGY_STATE] =
+ * {d, d_max, D_num, k, initialised, skipped, dlr, unused}, set to {d0, d0, 0, 0, 0, 0, 0, 0} before the first call.  Per call, with
+ * g' = g * grad_scale clipped to max_norm with the device-side sumsq (as hcp_adamw_flat_dev), lr = the largest segment lr and
+ * dlr = d lr (use_bias_correction ? sqrt(1 - beta2^(k+1)) / (1 - beta1^(k+1)) : 1):
+ *   coupled decay (decouple == 0): g' += wd p.  First call: p0 = p, s = m = v = 0 (every segment).
+ *   segments with lr > 0: D_num' = beta3 D_num + (d / d0) dlr sum g' (p0 - p);  m = beta1 m + d (1 - beta1) g';
+ *     v = beta2 v + d^2 (1 - beta2) g'^2;  s = beta3 s + (d / d0) (safeguard_warmup ? d : dlr) g';  D_den = sum |s|.
+ *   D_den == 0: nothing else changes (p, d, d_max, D_num, k stay; "skipped" is set).  Otherwise, when lr > 0:
+ *     d_hat = d_coef D_num' / D_den;  d = max(d, d_hat) if d == d0;  d_max = max(d_max, d_hat);  d = min(d_max, d growth_rate);
+ *     then every segment: p = p - wd dlr p (decouple), p = p - dlr m / (sqrt(v) + d eps) (old dlr, new d);  k += 1.
+ * *step_device (hcp_ema_flat's counter) is advanced on every call, skipped or not.  The sums are fp64 partials per CTA in
+ * `workspace` (at least HCP_PRODIGY_WORKSPACE_BYTES, 8-byte aligned), added in a fixed order: replays are bit-identical.  An
+ * empty table is a no-op.  Three launches; no host synchronisation (CUDA-graph capturable). */
+typedef struct {
+    int64_t offset;
+    int64_t count;
+    double lr;
+    double weight_decay;
+} hcp_prodigy_segment;
+#define HCP_PRODIGY_HYPER 8
+#define HCP_PRODIGY_STATE 8
+#define HCP_PRODIGY_WORKSPACE_BYTES 16384
+int hcp_prodigy_flat(float* p, const float* g, float* p0, float* s, float* m, float* v, int64_t n, const hcp_prodigy_segment* segs_host,
+                     const hcp_prodigy_segment* segs_device, int32_t nsegs, const double* hyper_device, double* state_device,
+                     double* workspace, size_t workspace_bytes, float grad_scale, const float* sumsq_device, float max_norm,
+                     int* step_device, hcp_stream_t stream);
+
 /* AdamW8bit (bitsandbytes.optim.AdamW8bit: blockwise 8-bit Adam moments) over the tensors of a table.  A tensor in mode 1 keeps
  * its first and second moments as uint8 codes, code1 at codes + state and code2 at codes + code_bytes + state (numel each), with one
  * fp32 scale per 256-element block counted from the tensor's first element: absmax1 at absmax + absmax_row, absmax2 at absmax +

@@ -1,11 +1,12 @@
-"""The optimizer pass alone on one GPU: hcp_adamw_flat_dev, hcp_lion_flat_dev and hcp_adamw8bit_flat over flat fp32 buffers of a
-whole UNet, each captured in a CUDA graph and timed alternately in one process (CUDA events around `--reps` replays, `--rounds`
+"""The optimizer pass alone on one GPU: hcp_adamw_flat_dev, hcp_lion_flat_dev, hcp_adamw8bit_flat and hcp_prodigy_flat over flat
+fp32 buffers of a whole UNet, each captured in a CUDA graph and timed alternately in one process (CUDA events around `--reps` replays, `--rounds`
 rounds, median).  AdamW8bit walks a table that cuts the buffer like a UNet: 1280 x 1280 weights (8-bit) each followed by a
 1280-element bias (fp32 moments), the remainder one more 8-bit tensor.
 
 Traffic is counted from the kernels: AdamW reads p, g, m, v and writes p, m, v (28 B per parameter); Lion reads p, g, m and writes
 p, m (20 B); AdamW8bit is adamw8bit.Layout.bytes_per_step (16 B per 8-bit parameter plus 16 B per 256-element block, 28 B per
-parameter of the biases).  The step counter, the hyper row and the clip's sum of squares are a few bytes.  Prints one JSON line per size with
+parameter of the biases); Prodigy reads p, g, p0, s, m, v and writes s, m, v, then reads p, m, v and writes p (52 B, one
+segment; its fp64 scalars and per-CTA partials are a few kB).  The step counter, the hyper row and the clip's sum of squares are a few bytes.  Prints one JSON line per size with
 ms, achieved GB/s and the share of the H100 SXM data-sheet HBM3 bandwidth (3.35 TB/s), plus the card name and power limit.
 
   python tools/bench_optim.py [--sizes 859520964 2567463684] [--reps 5] [--rounds 5]
@@ -20,11 +21,11 @@ import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch  # noqa: E402
 
-from hcp_diffusion_b200 import adamw8bit  # noqa: E402
+from hcp_diffusion_b200 import adamw8bit, prodigy  # noqa: E402
 from hcp_diffusion_b200._lib import call, stream_ptr  # noqa: E402
 
 SD15, SDXL = 859_520_964, 2_567_463_684          # trainable parameters of the SD1.5 and SDXL-base UNets
-BYTES = {"adamw": 28, "lion": 20}
+BYTES = {"adamw": 28, "lion": 20, "prodigy": 52}
 W, B = 1280 * 1280, 1280
 
 
@@ -88,6 +89,13 @@ for n in args.sizes:
     hyper8 = torch.tensor([[1e-6, 0.9, 0.999, 1e-8, 1e-2]], device="cuda")
     steps8 = torch.zeros(1, dtype=torch.int32, device="cuda")
     BYTES["adamw8bit"] = lay.bytes_per_step() / n
+    p0, s = torch.zeros_like(p), torch.zeros_like(p)
+    pd_segs = prodigy.segment_table([(0, n, 1.0, 1e-2)])
+    pd_segs_d = torch.from_numpy(pd_segs.view("int64").copy()).cuda()
+    pd_hyper = torch.tensor(prodigy.hyper_row(prodigy.check_options({"use_bias_correction": True}), 0.9, 0.999, 1e-8),
+                            dtype=torch.float64, device="cuda")
+    pd_state = torch.tensor(prodigy.initial_state(1e-6), dtype=torch.float64, device="cuda")
+    pd_work = torch.zeros(prodigy.WORKSPACE_BYTES // 8, dtype=torch.float64, device="cuda")
     graphs = {
         "adamw": graph_of(lambda: call("hcp_adamw_flat_dev", p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), n,
                                        hyper["adamw"].data_ptr(), *tail())),
@@ -97,6 +105,10 @@ for n in args.sizes:
                                            len(lay.tensors), lay.items.ctypes.data, items_d.data_ptr(), lay.items.size, nflat,
                                            lay.code_bytes, lay.nblocks, lay.small_numel, hyper8.data_ptr(), steps8.data_ptr(), 1, 1.0,
                                            sumsq.data_ptr(), 1.0, stream_ptr())),
+        "prodigy": graph_of(lambda: call("hcp_prodigy_flat", p.data_ptr(), g.data_ptr(), p0.data_ptr(), s.data_ptr(), m.data_ptr(),
+                                         v.data_ptr(), n, pd_segs.ctypes.data, pd_segs_d.data_ptr(), 1, pd_hyper.data_ptr(),
+                                         pd_state.data_ptr(), pd_work.data_ptr(), prodigy.WORKSPACE_BYTES, 1.0, sumsq.data_ptr(), 1.0,
+                                         step.data_ptr(), stream_ptr())),
     }
     times = {k: [] for k in graphs}
     for _ in range(args.rounds):
@@ -117,5 +129,5 @@ for n in args.sizes:
         out[name] = {"ms": round(ms, 3), "ms_min": round(min(ts), 3), "ms_max": round(max(ts), 3), "bytes_per_param": round(BYTES[name], 3),
                      "GB_s": round(gbs, 1), "share_of_3.35TBs": round(gbs / (HBM_TBS * 1e3), 3)}
     print(json.dumps(out), flush=True)
-    del p, g, m, v, codes, absmax, state32, graphs
+    del p, g, m, v, p0, s, codes, absmax, state32, graphs
     torch.cuda.empty_cache()
