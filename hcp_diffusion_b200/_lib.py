@@ -155,6 +155,7 @@ EXPORTS = [
     "hcp_attn_fwd_causal_bf16", "hcp_attn_bwd_causal_bf16", "hcp_quick_gelu_fwd_bf16", "hcp_quick_gelu_bwd_bf16", "hcp_embed_gather_bf16",
     "hcp_sum_bf16_to_f32", "hcp_gelu_fwd_bf16", "hcp_gelu_bwd_bf16", "hcp_eps_loss_grouped_workspace_bytes", "hcp_eps_loss_grouped",
     "hcp_pyramid_plan", "hcp_pyramid_workspace_bytes", "hcp_pyramid_noise", "hcp_add_noise_scaled",
+    "hcp_embed_grad_workspace_bytes", "hcp_embed_grad_bf16",
 ]
 PYRAMID_MAX_LEVEL, PYRAMID_MAX_GROUPS, PYRAMID_PLAN_INTS = 16, 64, 32       # HCP_PYRAMID_* of include/hcp_b200.h
 
@@ -200,6 +201,9 @@ def lib() -> C.CDLL:
             l.hcp_gelu_bwd_bf16.argtypes = [vp, vp, i64, i64, vp, vp]
             l.hcp_sum_bf16_to_f32.argtypes = [C.POINTER(C.c_void_p), i64, i64, vp, vp]
             l.hcp_embed_gather_bf16.argtypes = [vp, vp, vp, i64, vp, i64, i64, i64, i64, vp, vp]
+            l.hcp_embed_grad_workspace_bytes.restype = C.c_size_t
+            l.hcp_embed_grad_workspace_bytes.argtypes = [i64, i64, i64]
+            l.hcp_embed_grad_bf16.argtypes = [vp, vp, vp, i64, i64, i64, vp, i64, vp, i64, vp, C.c_size_t, vp]
             l.hcp_upsample2x_fwd_bf16.argtypes = [vp, i64, i64, i64, i64, vp, vp]
             l.hcp_upsample2x_bwd_bf16.argtypes = [vp, i64, i64, i64, i64, vp, vp]
             l.hcp_add_bf16.argtypes = [vp, vp, i64, vp, vp]

@@ -1064,6 +1064,158 @@ __global__ void embed_gather_kernel(const int64_t* __restrict__ ids, const int64
 }
 
 // =============================================================================================
+// backward of the gather: dtok[id] += sum of dH over the rows holding id, dpos[p] += sum over the rows at position p, without float
+// atomics.  Table `tab` (0 token, 1 position) keys row r by its clamped table row.  Three launches:
+//   rank     the stable order of the rows by (key, row): order[rank(r)] = r, skey[rank] = key(r)  (rank = #rows before r in that order)
+//   partial  sorted positions in chunks of kEmbChunk; each chunk sums its runs of equal keys in row order; a run whose key lives
+//            only in this chunk is added to the table, a run that continues across a chunk edge leaves its sum in part[chunk][slot]
+//   combine  the CTA of the chunk where such a key starts adds the chunk partials in chunk order and adds the total to the table
+// So a table row gets dst += s, s = sum of its pieces in order, each piece (its rows inside one chunk) summed from 0 in row order.
+// =============================================================================================
+constexpr int kEmbChunk = 32;
+
+__device__ __forceinline__ int embed_key(const int64_t* __restrict__ ids, const int64_t* __restrict__ pos_ids, int64_t V, int64_t P,
+                                         int L, int tab, int r) {
+    if (tab == 0) return (int)min(max(ids[r], (int64_t)0), V - 1);
+    const int l = r % L;
+    return (int)min(max(pos_ids ? pos_ids[l] : (int64_t)l, (int64_t)0), P - 1);
+}
+
+// 32 rows per CTA; warp w counts the rows ordered before them in slice w of every 1024-key tile (integer counts: any order is exact)
+__global__ void __launch_bounds__(256) embed_rank_kernel(const int64_t* __restrict__ ids, const int64_t* __restrict__ pos_ids, int64_t V,
+                                                         int64_t P, int L, int N, int tab0, int* __restrict__ ws) {
+    pdl_trigger();
+    pdl_wait();
+    __shared__ int tile[1024];
+    __shared__ int cnt[8][32];
+    const int tab = tab0 + (int)blockIdx.z;
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const int r = blockIdx.x * 32 + lane;
+    const int k = r < N ? embed_key(ids, pos_ids, V, P, L, tab, r) : 0;
+    int c = 0;
+    for (int t0 = 0; t0 < N; t0 += 1024) {
+        for (int i = threadIdx.x; i < 1024; i += 256)
+            tile[i] = t0 + i < N ? embed_key(ids, pos_ids, V, P, L, tab, t0 + i) : 0;
+        __syncthreads();
+        const int hi = min(w * 128 + 128, N - t0);
+        for (int i = w * 128; i < hi; ++i) {
+            const int kk = tile[i];
+            c += (kk < k) | ((kk == k) & (t0 + i < r));
+        }
+        __syncthreads();
+    }
+    cnt[w][lane] = c;
+    __syncthreads();
+    if (w == 0 && r < N) {
+        int s = 0;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) s += cnt[j][lane];
+        int* order = ws + (size_t)tab * 2 * N;
+        order[s] = r;
+        order[N + s] = k;
+    }
+}
+
+__device__ __forceinline__ void add8_to(float* __restrict__ dst, const float* s) {
+    float4* d = reinterpret_cast<float4*>(dst);
+    const float4 a = d[0], b = d[1];
+    d[0] = make_float4(a.x + s[0], a.y + s[1], a.z + s[2], a.w + s[3]);
+    d[1] = make_float4(b.x + s[4], b.y + s[5], b.z + s[6], b.w + s[7]);
+}
+
+__device__ __forceinline__ void store8(float* __restrict__ dst, const float* s) {
+    float4* d = reinterpret_cast<float4*>(dst);
+    d[0] = make_float4(s[0], s[1], s[2], s[3]);
+    d[1] = make_float4(s[4], s[5], s[6], s[7]);
+}
+
+// one warp per (chunk, 256 channels, table); lane j holds the row and key of sorted position chunk * 32 + j
+__global__ void __launch_bounds__(32) embed_grad_partial_kernel(const __nv_bfloat16* __restrict__ dH, int N, int C, int tab0,
+                                                                const int* __restrict__ ws, float* __restrict__ part, float* __restrict__ dtok,
+                                                                float* __restrict__ dpos) {
+    pdl_trigger();
+    pdl_wait();
+    const int tab = tab0 + (int)blockIdx.z;
+    const int* order = ws + (size_t)tab * 2 * N;
+    const int* skey = order + N;
+    float* dst = tab == 0 ? dtok : dpos;
+    const int nch = (N + kEmbChunk - 1) / kEmbChunk;
+    const int q = blockIdx.x, k0 = q * kEmbChunk, n = min(kEmbChunk, N - k0);
+    const int lane = threadIdx.x;
+    const int my_row = lane < n ? order[k0 + lane] : 0, my_key = lane < n ? skey[k0 + lane] : 0;
+    const bool from_prev = k0 > 0 && skey[k0 - 1] == skey[k0];
+    const bool to_next = k0 + n < N && skey[k0 + n] == skey[k0 + n - 1];
+    const int c = (blockIdx.y * 32 + lane) * 8;
+    const bool active = c < C;
+    float* my_part = part + (((size_t)tab * nch + q) * 2) * C + c;
+    float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    int run0 = 0;
+    for (int j0 = 0; j0 < n; j0 += 8) {
+        uint4 v[8];
+#pragma unroll
+        for (int u = 0; u < 8; ++u) {
+            const int row = __shfl_sync(0xffffffffu, my_row, (j0 + u) & 31);
+            if (active && j0 + u < n) v[u] = *reinterpret_cast<const uint4*>(dH + (size_t)row * C + c);
+        }
+#pragma unroll
+        for (int u = 0; u < 8; ++u) {
+            const int j = j0 + u;
+            const int key = __shfl_sync(0xffffffffu, my_key, j & 31);
+            const int next = __shfl_sync(0xffffffffu, my_key, (j + 1) & 31);
+            if (j >= n) continue;
+            if (active) {
+                float f[8];
+                unpack8(v[u], f);
+#pragma unroll
+                for (int e = 0; e < 8; ++e) acc[e] += f[e];
+            }
+            if (j + 1 < n && next == key) continue;
+            // end of a run: positions [run0, j] of this chunk
+            const bool head = run0 == 0 && from_prev, tail = j == n - 1 && to_next;
+            if (active) {
+                if (head || tail) store8(my_part + (run0 == 0 ? 0 : C), acc);
+                else add8_to(dst + (size_t)key * C + c, acc);
+            }
+#pragma unroll
+            for (int e = 0; e < 8; ++e) acc[e] = 0.f;
+            run0 = j + 1;
+        }
+    }
+}
+
+// the key whose run ends this chunk and continues into the next one, if it starts in this chunk: its pieces, in chunk order
+__global__ void __launch_bounds__(32) embed_grad_combine_kernel(int N, int C, int tab0, const int* __restrict__ ws,
+                                                                const float* __restrict__ part, float* __restrict__ dtok,
+                                                                float* __restrict__ dpos) {
+    pdl_trigger();
+    pdl_wait();
+    const int tab = tab0 + (int)blockIdx.z;
+    const int* skey = ws + (size_t)tab * 2 * N + N;
+    float* dst = tab == 0 ? dtok : dpos;
+    const int nch = (N + kEmbChunk - 1) / kEmbChunk;
+    const int q = blockIdx.x, k0 = q * kEmbChunk, k1 = min(k0 + kEmbChunk, N);
+    const int key = skey[k1 - 1];
+    if (k1 >= N || skey[k1] != key) return;
+    const bool whole = skey[k0] == key;                      // the chunk is one run: slot 0, and the key may have started earlier
+    if (whole && k0 > 0 && skey[k0 - 1] == key) return;
+    const int c = (blockIdx.y * 32 + threadIdx.x) * 8;
+    if (c >= C) return;
+    const float* p = part + ((size_t)tab * nch * 2) * C + c;
+    float s[8];
+    {
+        const float4* a = reinterpret_cast<const float4*>(p + ((size_t)q * 2 + (whole ? 0 : 1)) * C);
+        const float4 x = a[0], y = a[1];
+        s[0] = x.x; s[1] = x.y; s[2] = x.z; s[3] = x.w; s[4] = y.x; s[5] = y.y; s[6] = y.z; s[7] = y.w;
+    }
+    for (int qq = q + 1; qq < nch && skey[qq * kEmbChunk] == key; ++qq) {
+        const float4* a = reinterpret_cast<const float4*>(p + (size_t)qq * 2 * C);
+        const float4 x = a[0], y = a[1];
+        s[0] += x.x; s[1] += x.y; s[2] += x.z; s[3] += x.w; s[4] += y.x; s[5] += y.y; s[6] += y.z; s[7] += y.w;
+    }
+    add8_to(dst + (size_t)key * C + c, s);
+}
+
+// =============================================================================================
 // nearest 2x upsample (NHWC) and its backward (sum of the 2x2 block)
 // =============================================================================================
 __global__ void upsample2x_fwd_kernel(const __nv_bfloat16* __restrict__ x, int B, int H, int W, int C, __nv_bfloat16* __restrict__ y) {
@@ -1317,6 +1469,39 @@ extern "C" int hcp_embed_gather_bf16(const int64_t* ids, const int64_t* pos_ids,
     launch_k(embed_gather_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, (cudaStream_t)stream_, ids, pos_ids, tok_emb, V, pos_emb, P,
              B * L, (int)L, (int)C, (__nv_bfloat16*)out);
     LAUNCH_CHECK("embed_gather launch");
+    return HCP_OK;
+}
+extern "C" size_t hcp_embed_grad_workspace_bytes(int64_t B, int64_t L, int64_t C) {
+    if (B <= 0 || L <= 0 || C <= 0) return 0;
+    const int64_t N = B * L, nch = (N + kEmbChunk - 1) / kEmbChunk;
+    return (size_t)(2 * 2 * N) * sizeof(int) + (size_t)(2 * nch * 2 * C) * sizeof(float);
+}
+extern "C" int hcp_embed_grad_bf16(const int64_t* ids, const int64_t* pos_ids, const void* dH, int64_t B, int64_t L, int64_t C, float* dtok,
+                                   int64_t V, float* dpos, int64_t P, void* workspace, size_t workspace_bytes, hcp_stream_t stream_) {
+    if (!ids || !dH || !workspace) return set_error(HCP_ERR_INVALID, "embed_grad: null pointer");
+    if (!dtok && !dpos) return set_error(HCP_ERR_INVALID, "embed_grad: no destination (dtok and dpos are both NULL)");
+    if (B <= 0 || L <= 0 || C <= 0 || C % 8 != 0 || V <= 0 || P <= 0)
+        return set_error(HCP_ERR_INVALID, "embed_grad: non-positive size, empty table or C not a multiple of 8");
+    if (V > INT32_MAX || P > INT32_MAX || B * L > INT32_MAX / 2 || C > INT32_MAX / 8)
+        return set_error(HCP_ERR_INVALID, "embed_grad: size too large");
+    if (dpos && !pos_ids && L > P) return set_error(HCP_ERR_INVALID, "embed_grad: sequence longer than the position table");
+    if (!aligned16(dH, workspace) || (dtok && !aligned16(dtok)) || (dpos && !aligned16(dpos)) || ((uintptr_t)ids & 7) ||
+        ((uintptr_t)pos_ids & 7))
+        return set_error(HCP_ERR_INVALID, "embed_grad: dH, dtok, dpos and workspace must be 16-byte aligned, ids 8-byte");
+    if (workspace_bytes < hcp_embed_grad_workspace_bytes(B, L, C))
+        return set_error(HCP_ERR_INVALID, "embed_grad: workspace smaller than hcp_embed_grad_workspace_bytes");
+    const int N = (int)(B * L), nch = (N + kEmbChunk - 1) / kEmbChunk;
+    const int tab0 = dtok ? 0 : 1, ntab = (dtok && dpos) ? 2 : 1;
+    int* ws = (int*)workspace;
+    float* part = (float*)(ws + 4 * (size_t)N);
+    cudaStream_t s = (cudaStream_t)stream_;
+    launch_k(embed_rank_kernel, dim3((unsigned)((N + 31) / 32), 1, ntab), dim3(256), 0, s, ids, pos_ids, V, P, (int)L, N, tab0, ws);
+    LAUNCH_CHECK("embed_grad rank launch");
+    const dim3 grid((unsigned)nch, (unsigned)((C / 8 + 31) / 32), (unsigned)ntab);
+    launch_k(embed_grad_partial_kernel, grid, dim3(32), 0, s, (const __nv_bfloat16*)dH, N, (int)C, tab0, (const int*)ws, part, dtok, dpos);
+    LAUNCH_CHECK("embed_grad partial launch");
+    launch_k(embed_grad_combine_kernel, grid, dim3(32), 0, s, N, (int)C, tab0, (const int*)ws, (const float*)part, dtok, dpos);
+    LAUNCH_CHECK("embed_grad combine launch");
     return HCP_OK;
 }
 extern "C" int hcp_upsample2x_fwd_bf16(const void* x, int64_t B, int64_t H, int64_t W, int64_t C, void* y, hcp_stream_t stream_) {

@@ -189,9 +189,13 @@ class LoraTrainStep:
     parameter (16 B) and the step size d estimated on the device; every group's lr must be the largest lr or 0, as prodigyopt
     requires.
 
-    `text_encoder`: a `models.CLIPTextModel` whose LoRA adapters train together with the UNet's (the reference's `lora_text_encoder`,
-    `TEUnetWrapper`); its adapter parameters must be among `params` (their own groups), so they share the flat buffer: one all-reduce,
-    one global-norm clip over both models, the same optimizer and EMA.  `step()` then takes int64 token ids [B, 77 R] in place of the
+    `text_encoder`: a `models.CLIPTextModel` whose LoRA adapters (the reference's `lora_text_encoder`) and / or base parameters
+    (`text_encoder:`, full fine-tuning) train together with the UNet (`TEUnetWrapper`); every trainable text-encoder parameter must be
+    among `params` (their own groups), so they share the flat buffer: one all-reduce, one global-norm clip over both models, the same
+    optimizer and EMA.  The token table [vocab, C] is one tensor of the flat buffer like any other: the rows no prompt used get a
+    zero gradient, and every optimizer treats them as it treats any zero gradient (AdamW / Lion / AdamW8bit / Prodigy still move
+    them by their moments and weight decay, Adafactor's factored second moment spans the whole table), as torch.optim does with
+    a dense nn.Embedding gradient.  `step()` then takes int64 token ids [B, 77 R] in place of the
     text embedding, and the text encoder runs forward and backward inside the same graph.  `text_encoder_opts`: {'n_repeats',
     'clip_skip', 'clip_final_norm'} of `models.encode_prompt`.  With an SDXL (text_time) UNet the text encoder is a
     `models.SDXLTextEncoder` (SDXLTEUnetWrapper): `step()` takes ids [B, 2 x 77] and `added_cond_kwargs={'time_ids'}`, and
@@ -278,7 +282,7 @@ class LoraTrainStep:
             missing = [n for n, p in text_encoder.named_parameters() if p.requires_grad and id(p) not in seen]
             if missing:
                 raise ValueError(f"text-encoder parameters {missing[:3]}... are trainable but not in `params`: pass the "
-                                 "lora_text_encoder groups too (they share the flat buffer, the clip and the optimizer)")
+                                 "text_encoder / lora_text_encoder groups too (they share the flat buffer, the clip and the optimizer)")
         self.flat = FlatParams(flat_list)
         dev = self.flat.data.device
         self.m = self.v = None

@@ -21,9 +21,8 @@ import torch
 from torch import nn
 
 from .. import _lib, ops
-from ..runtime import LinearGroup, _JobTable, pack_lora
+from ..runtime import LinearGroup, _JobTable, pack_lora, repack_trained
 from .lora import DAPPPatchContainer
-from .plugin import BasePluginBlock
 
 
 @dataclass
@@ -165,6 +164,7 @@ class CLIPTextModel(nn.Module):
                                       eos_token_id=eos_token_id)
         self.text_model = CLIPTextTransformer(self.config)
         self.__dict__["_jobs"] = _JobTable()
+        self.__dict__["_repack"] = _JobTable()
 
     @property
     def dtype(self) -> torch.dtype:
@@ -181,18 +181,11 @@ class CLIPTextModel(nn.Module):
         return out
 
     def _check_trainable(self) -> None:
-        """Only LoRA adapters train here: a base parameter that requires a gradient (full fine-tune) or a DreamArtist++ container is
-        refused instead of being silently frozen."""
+        """LoRA adapters and base parameters (the `text_encoder:` full fine-tune list) train; a DreamArtist++ container is refused
+        instead of being silently run as a plain LoRA."""
         for name, m in self.named_modules():
             if isinstance(m, DAPPPatchContainer):
                 raise NotImplementedError(f"DreamArtist++ adapters on the text encoder ({name}) are not supported")
-        if not torch.is_grad_enabled():
-            return
-        plugin_params = {id(p) for m in self.modules() if isinstance(m, BasePluginBlock) for p in m.parameters()}
-        for name, p in self.named_parameters():
-            if p.requires_grad and id(p) not in plugin_params:
-                raise NotImplementedError(f"{name} requires a gradient: full fine-tuning of the text encoder is not supported "
-                                          "(freeze the base model with requires_grad_(False); LoRA adapters train)")
 
     def run_layers(self, input_ids: torch.Tensor, n_layers: int, position_ids: Optional[torch.Tensor] = None) -> List[torch.Tensor]:
         """[embeddings, output of layer 1, ..., output of layer n_layers] as bf16 [B, L, C]; only the first n_layers layers run."""
@@ -206,6 +199,8 @@ class CLIPTextModel(nn.Module):
         for g in groups:
             g.prepare()
         pack_lora(groups, self.__dict__["_jobs"])
+        # full fine-tune: one launch re-casts the trained fp32 masters the optimizer updated into the GEMMs' bf16 operands
+        repack_trained(groups, self.__dict__["_repack"])
         emb = self.text_model.embeddings
         h = ops.embed_tokens(input_ids.long(), emb.token_embedding.weight, emb.position_embedding.weight, position_ids)
         out = [h]
@@ -239,8 +234,9 @@ def encode_prompt(te: CLIPTextModel, input_ids: torch.Tensor, n_repeats: int = 1
     `clip_final_norm`), and the R chunks are rejoined as BOS + R x 75 middle rows + EOS -> bf16 [B, 75 R + 2, C].
 
     Only the first num_hidden_layers - clip_skip layers run.  The reference keeps the skipped layers in its graph with gradient 0; here
-    their adapters receive no gradient contribution.  In `LoraTrainStep` their gradients live in the flat buffer, which is zeroed
-    every step, so they get the reference's zero gradient and AdamW still decays them."""
+    their adapters (and, under full fine-tuning, their base parameters) receive no gradient contribution.  In `LoraTrainStep` their
+    gradients live in the flat buffer, which is zeroed every step, so they get the reference's zero gradient and AdamW still decays
+    them."""
     n_total = len(te.text_model.encoder.layers)
     if not 0 <= clip_skip < n_total:
         raise ValueError(f"clip_skip must be in [0, {n_total})")
@@ -281,6 +277,7 @@ class CLIPTextModelWithProjection(CLIPTextModel):
         self.text_projection = nn.Linear(hidden_size, projection_dim, bias=False)
         self.__dict__["_proj"] = LinearGroup([])
         self.__dict__["_proj_jobs"] = _JobTable()
+        self.__dict__["_proj_repack"] = _JobTable()
 
     def linear_groups(self) -> List[LinearGroup]:
         return super().linear_groups() + [self._proj_group()]
@@ -298,6 +295,7 @@ class CLIPTextModelWithProjection(CLIPTextModel):
         g = self._proj_group()
         g.prepare()
         pack_lora([g], self.__dict__["_proj_jobs"])
+        repack_trained([g], self.__dict__["_proj_repack"])
         return g([pooled.contiguous()]).float()
 
     def forward(self, input_ids: torch.Tensor, attention_mask: Optional[torch.Tensor] = None, position_ids: Optional[torch.Tensor] = None,

@@ -1164,25 +1164,63 @@ class GeluFn(torch.autograd.Function):
         return dx
 
 
+def _embed_gather(ids, pos_ids, tok, pos):
+    B, L = ids.shape
+    out = torch.empty((B, L, tok.shape[1]), dtype=BF16, device=ids.device)
+    call("hcp_embed_gather_bf16", ids.data_ptr(), ptr(pos_ids), tok.data_ptr(), tok.shape[0], pos.data_ptr(), pos.shape[0], B, L,
+         tok.shape[1], out.data_ptr(), stream_ptr())
+    return out
+
+
+class EmbedFn(torch.autograd.Function):
+    """The gather with trained tables: the backward accumulates dtok / dpos in place into the tables' fp32 .grad (the flat gradient
+    buffer under LoraTrainStep) with hcp_embed_grad_bf16, which sums each table row's gradient in a fixed order without atomics."""
+
+    @staticmethod
+    def forward(ctx, ids, pos_ids, tok_emb, pos_emb):
+        tok, pos = tok_emb.detach().contiguous(), pos_emb.detach().contiguous()
+        ctx.save_for_backward(ids, pos_ids)
+        ctx.tables = (tok_emb, pos_emb)
+        return _embed_gather(ids, pos_ids, tok, pos)
+
+    @staticmethod
+    def backward(ctx, dh):
+        ids, pos_ids = ctx.saved_tensors
+        tok_emb, pos_emb = ctx.tables
+        dh = _chk(dh, "embedding grad")
+        B, L = ids.shape
+        C_ = tok_emb.shape[1]
+        dtok = _acc_grad(tok_emb) if tok_emb.requires_grad else None
+        dpos = _acc_grad(pos_emb) if pos_emb.requires_grad else None
+        for g in (dtok, dpos):
+            if g is not None and not g.is_contiguous():
+                raise _lib.HcpError("embed_tokens: an embedding table's .grad must be contiguous")
+        nbytes = _lib.lib().hcp_embed_grad_workspace_bytes(B, L, C_)
+        ws = torch.empty(((nbytes + 15) // 16 * 4,), dtype=torch.float32, device=dh.device)
+        call("hcp_embed_grad_bf16", ids.data_ptr(), ptr(pos_ids), dh.data_ptr(), B, L, C_, ptr(dtok), tok_emb.shape[0], ptr(dpos),
+             pos_emb.shape[0], ws.data_ptr(), ws.numel() * 4, stream_ptr())
+        notify_grad(*(p for p in (tok_emb, pos_emb) if p.requires_grad))
+        return None, None, None, None
+
+
 def embed_tokens(ids: torch.Tensor, tok_emb: torch.Tensor, pos_emb: torch.Tensor, pos_ids: Optional[torch.Tensor] = None) -> torch.Tensor:
     """bf16 [B, L, C] = tok_emb[ids] + pos_emb[pos_ids or arange(L)] (fp32 tables, int64 ids on the device; ids outside the tables
-    are clamped to the nearest row, see hcp_embed_gather_bf16).  No gradient: the embedding tables are frozen."""
+    are clamped to the nearest row, see hcp_embed_gather_bf16).  When either table requires a gradient (and grad mode is on) the
+    result carries an autograd node whose backward accumulates into that table's .grad (EmbedFn); frozen tables take the plain
+    gather."""
     if ids.dtype != torch.int64 or not ids.is_cuda or ids.dim() != 2:
         raise _lib.HcpError(f"embed_tokens: expected CUDA int64 ids [B, L], got {ids.dtype} {tuple(ids.shape)} on {ids.device}")
     if tok_emb.dtype != torch.float32 or pos_emb.dtype != torch.float32:
         raise _lib.HcpError("embed_tokens: the embedding tables must be fp32")
     ids = ids.contiguous()
-    tok, pos = tok_emb.detach().contiguous(), pos_emb.detach().contiguous()
-    B, L = ids.shape
-    C_ = tok.shape[1]
+    L = ids.shape[1]
     if pos_ids is not None:
         pos_ids = pos_ids.to(ids.device, torch.int64).reshape(-1).contiguous()
         if pos_ids.numel() != L:
             raise _lib.HcpError(f"embed_tokens: position_ids must hold {L} entries (one row shared by the batch)")
-    out = torch.empty((B, L, C_), dtype=BF16, device=ids.device)
-    call("hcp_embed_gather_bf16", ids.data_ptr(), ptr(pos_ids), tok.data_ptr(), tok.shape[0], pos.data_ptr(), pos.shape[0], B, L, C_,
-         out.data_ptr(), stream_ptr())
-    return out
+    if torch.is_grad_enabled() and (tok_emb.requires_grad or pos_emb.requires_grad):
+        return EmbedFn.apply(ids, pos_ids, tok_emb, pos_emb)
+    return _embed_gather(ids, pos_ids, tok_emb.detach().contiguous(), pos_emb.detach().contiguous())
 
 
 class Upsample2xFn(torch.autograd.Function):

@@ -17,15 +17,19 @@ constant_with_warmup), `loss.criterion` (`torch.nn.MSELoss` or `hcpdiff.loss.Min
 (`noise.resolve`: DDPMScheduler / .from_pretrained, ZeroTerminalScheduler, PyramidNoiseScheduler; `t` is drawn from [0, its
 num_train_timesteps), and null keeps SD1.x's DDPM table).
 
-Text encoder (SD1.x CLIP): `lora_text_encoder` items train LoRA on it next to the UNet (reference train_ac.py:61,335):
-`model.text_encoder` (instantiable, default CLIP-L) with weights from `model.text_encoder_init`, `model.clip_skip`,
-`model.clip_final_norm`, `model.tokenizer_repeats`; `ckpts/text_encoder-<step>` is saved next to `unet-<step>` and
-`resume.ckpt_path.TE` is loaded.  A `text_encoder:` full fine-tune list, a non-null `tokenizer_pt.train` and DreamArtist++ items in
-`lora_text_encoder` raise NotImplementedError (so `train.optimizer_pt`, the prompt-tuning optimizer, is never read).  The ids
-are given (no tokenizer): `data.path` holds 'input_ids' [N, 77 R], or synthetic prompts are BOS 49406, random tokens, EOS 49407 padding.  With an SDXL ('text_time') UNet the default text encoder is
-SDXL's pair (`models.SDXLTextEncoder`, CLIP-L + OpenCLIP-bigG, reference cfgs/train/examples/lora_sdxl.yaml): ids are [N, 2 x 77]
-(clip_B's chunk, then bigG's; synthetic bigG chunks carry the same words and are padded with id 0 after EOS, as SDXL's second
-tokenizer pads), `text_embeds` comes from the encoder and the data holds only 'time_ids'.
+Text encoder (SD1.x CLIP): `lora_text_encoder` items train LoRA on it and `text_encoder` items (reference
+cfgs/train/examples/fine-tuning.yaml: `{lr, layers}` selecting whole layers, default lr 1e-5) train its base parameters, next to the
+UNet, both through `make_hcpdiff` as for the UNet (reference train_ac.py:61,324-340): `model.text_encoder` (instantiable, default
+CLIP-L) with weights from `model.text_encoder_init`, `model.clip_skip`, `model.clip_final_norm`, `model.tokenizer_repeats`;
+`ckpts/text_encoder-<step>` is saved next to `unet-<step>` ('base' holds the trained base parameters under transformers' names,
+'lora' the adapters, and 'base_ema' / 'lora_ema' their EMA) and `resume.ckpt_path.TE` loads both parts.  A non-null
+`tokenizer_pt.train` and DreamArtist++ items in `lora_text_encoder` raise NotImplementedError (so `train.optimizer_pt`, the
+prompt-tuning optimizer, is never read), as does either list on a CPU device (the text encoder runs on CUDA only).  The ids are
+given (no tokenizer): `data.path` holds 'input_ids' [N, 77 R], or synthetic prompts are BOS 49406, random tokens, EOS 49407
+padding.  With an SDXL ('text_time') UNet the default text encoder is SDXL's pair (`models.SDXLTextEncoder`, CLIP-L +
+OpenCLIP-bigG, reference cfgs/train/examples/lora_sdxl.yaml): ids are [N, 2 x 77] (clip_B's chunk, then bigG's; synthetic bigG
+chunks carry the same words and are padded with id 0 after EOS, as SDXL's second tokenizer pads), `text_embeds` comes from the
+encoder and the data holds only 'time_ids'.
 
 Out of the hot path and therefore NOT here: datasets / buckets / captions, a tokenizer, VAE, loggers, DeepSpeed /
 Colossal-AI trainers.  Inputs are the synthetic latents / text embeddings of SURVEY.md 8d (`data.synthetic`), or tensors saved
@@ -246,7 +250,7 @@ class Trainer:
         groups = [{"params": g["params"], "lr": float(g["lr"]) * lr_scale} for g in groups if len(g["params"])]
         self.te, self.te_lora, te_opts = self._build_text_encoder(cfgs)
         if self.te is not None:
-            te_groups, self.te_lora = make_hcpdiff(self.te, None, cfgs.get("lora_text_encoder"), default_lr=1e-5)
+            te_groups, self.te_lora = make_hcpdiff(self.te, cfgs.get("text_encoder"), cfgs.get("lora_text_encoder"), default_lr=1e-5)
             groups += [{"params": g["params"], "lr": float(g["lr"]) * lr_scale} for g in te_groups if len(g["params"])]
         resume = tr.get("resume")
         self.start_step = 0
@@ -260,6 +264,8 @@ class Trainer:
                     self.unet.load_state_dict(sd["lora"], strict=False)   # raw-key checkpoints (plugin_from_raw), as the reference does
             for path in ((resume.get("ckpt_path", {}) or {}).get("TE", []) or []) if self.te is not None else []:
                 sd = auto_manager(path).load_ckpt(path)
+                if "base" in sd:
+                    self.te.load_state_dict(sd["base"], strict=False)
                 if "lora" in sd:
                     load_lora_state(self.te_lora, sd["lora"])
             self.start_step = int(resume.get("start_step", 0) or 0)
@@ -294,18 +300,21 @@ class Trainer:
         self._load_data(seed)
 
     def _build_text_encoder(self, cfgs):
-        """(text encoder, None, encode_prompt options) when `lora_text_encoder` is set, else (None, None, None)."""
-        if cfgs.get("text_encoder"):
-            raise NotImplementedError("`text_encoder:` (full fine-tuning of the text encoder) is not supported; use lora_text_encoder")
+        """(text encoder, None, encode_prompt options) when `text_encoder` or `lora_text_encoder` is set, else (None, None, None)."""
         tpt = cfgs.get("tokenizer_pt")
         if tpt and tpt.get("train") is not None:
             raise NotImplementedError("`tokenizer_pt.train` (prompt tuning / textual inversion) is not supported")
-        items = cfgs.get("lora_text_encoder")
-        if not items:
+        items = cfgs.get("lora_text_encoder") or []
+        if not items and not cfgs.get("text_encoder"):
             return None, None, None
         for item in items:
             if str(item.get("type", "lora")) != "lora":
                 raise NotImplementedError(f"lora_text_encoder item type {item.get('type')!r} (DreamArtist++ adapters) is not supported")
+        if torch.device(self.device).type == "cpu":
+            # the text encoder's forward and backward are CUDA kernels only: refuse before a full-size encoder is built on the host
+            # (a 'meta' device only lays out the modules)
+            raise NotImplementedError("training the text encoder (`text_encoder:` / `lora_text_encoder:` items) on the CPU is not "
+                                      "supported: it runs on a CUDA (sm_90a) device only, there is no CPU path")
         from .models import CLIPTextModel, SDXLTextEncoder
         te = cfgs.model.get("text_encoder")
         if isinstance(te, dict):
@@ -424,7 +433,8 @@ class Trainer:
         path = self.ckpt.save_model_with_lora(self.unet if base_trained else None, self.lora, "unet", step,
                                               ema_state=self.step_fn.ema_state() if self.step_fn.ema is not None else None)
         if self.te is not None:
-            self.ckpt.save_model_with_lora(None, self.te_lora, "text_encoder", step,
+            te_base = any(p.requires_grad for n, p in self.te.named_parameters() if "lora_block_" not in n)
+            self.ckpt.save_model_with_lora(self.te if te_base else None, self.te_lora, "text_encoder", step,
                                            ema_state=self.step_fn.ema_state() if self.step_fn.ema is not None else None)
         return path
 

@@ -242,6 +242,20 @@ int hcp_sum_bf16_to_f32(const void* const* srcs, int64_t nsrc, int64_t n, float*
 int hcp_embed_gather_bf16(const int64_t* ids, const int64_t* pos_ids, const float* tok_emb, int64_t V, const float* pos_emb, int64_t P,
                           int64_t B, int64_t L, int64_t C, void* out, hcp_stream_t stream);
 
+/* Backward of hcp_embed_gather_bf16 (the embedding tables trained: `text_encoder:` full fine-tuning, reference
+ * hcpdiff/train_ac.py:324-340 through autograd's embedding backward).  dH bf16 [B, L, C]; with ids and positions clamped as the gather
+ * clamps them:  dtok[v, :] += sum of dH[r, :] over the rows r = b L + l with id v   (fp32 [V, C], or NULL: not trained)
+ *               dpos[p, :] += sum of dH[r, :] over the rows at position p           (fp32 [P, C], or NULL), at least one given.
+ * Deterministic without float atomics: the rows of one table row are taken in row order and cut into pieces at every multiple of 32
+ * of their position in the stable (table row, row) order of all B L rows; each piece is summed from 0 in row order, the pieces are
+ * added in order, and the total is added to the table row once.  Repeats and graph replays are bit-identical.  Ids stay on the
+ * device (no host sync, graph-capturable).  C % 8 == 0, V, P <= INT32_MAX; without pos_ids (and dpos given) L <= P.  dH, dtok,
+ * dpos and the workspace 16-byte aligned, ids / pos_ids 8-byte; workspace_bytes >= hcp_embed_grad_workspace_bytes(B, L, C)
+ * (0 for a non-positive size).  Three launches. */
+size_t hcp_embed_grad_workspace_bytes(int64_t B, int64_t L, int64_t C);
+int hcp_embed_grad_bf16(const int64_t* ids, const int64_t* pos_ids, const void* dH, int64_t B, int64_t L, int64_t C, float* dtok, int64_t V,
+                        float* dpos, int64_t P, void* workspace, size_t workspace_bytes, hcp_stream_t stream);
+
 /* nearest x2 upsample of NHWC bf16 [B,H,W,C] (Upsample2D, cfgs/unet_struct.txt:392) and its backward */
 int hcp_upsample2x_fwd_bf16(const void* x, int64_t B, int64_t H, int64_t W, int64_t C, void* y, hcp_stream_t stream);
 int hcp_upsample2x_bwd_bf16(const void* dy, int64_t B, int64_t H, int64_t W, int64_t C, void* dx, hcp_stream_t stream);

@@ -8,8 +8,10 @@ the line then also gives the optimizer's own time per step.
 `--lora-te` times, in the same run, the step above and then the same step with SDXL's two text encoders (CLIP-L + OpenCLIP-bigG,
 full size, random init) in front, LoRA rank 4 on their self_attn + mlp layers (reference cfgs/train/examples/lora_sdxl.yaml's
 lora_text_encoder item, clip_skip 1, no final norm): the line gives both step times, the card and its power limit.
+`--full-te` does the same with every parameter of both text encoders trained instead (`text_encoder: [{lr: 1e-6, layers: ['']}]`,
+reference cfgs/train/examples/fine-tuning.yaml), keys `*_full_te`.
 
-  python tools/bench_sdxl.py [--batch 2] [--steps 5] [--no-locon] [--full-ft --optimizer adafactor|lion|adamw8bit] [--lora-te]
+  python tools/bench_sdxl.py [--batch 2] [--steps 5] [--no-locon] [--full-ft --optimizer adafactor|lion|adamw8bit] [--lora-te | --full-te]
 """
 import argparse
 import json
@@ -34,9 +36,12 @@ ap.add_argument("--no-locon", action="store_true")
 ap.add_argument("--full-ft", action="store_true")
 ap.add_argument("--optimizer", choices=("adamw", "adafactor", "lion", "adamw8bit"), default="adamw")
 ap.add_argument("--lora-te", action="store_true")
+ap.add_argument("--full-te", action="store_true")
 args = ap.parse_args()
-if args.lora_te and (args.full_ft or args.optimizer != "adamw"):
-    ap.error("--lora-te times the LoRA step with AdamW")
+if (args.lora_te or args.full_te) and (args.full_ft or args.optimizer != "adamw"):
+    ap.error("--lora-te / --full-te time the UNet LoRA step with AdamW")
+if args.lora_te and args.full_te:
+    ap.error("--lora-te and --full-te are two runs")
 
 
 def random_init(module):
@@ -117,7 +122,7 @@ out = {"workload": workload + f", bs={B}, {S * 8}x{S * 8}", "ms_per_step": ms, "
        "optimizer_state_bytes": step.optimizer_state_bytes, "launches_per_step": step.launches_per_step,
        "loss": float(step.loss.cpu()), "build_s": round(build_s, 1),
        "max_mem_gb": round(torch.cuda.max_memory_allocated() / 2 ** 30, 1), "gpu": props.name}
-if args.lora_te:
+if args.lora_te or args.full_te:
     # the same UNet and adapters, with SDXL's text encoders in front: ids [B, 2 x 77] (same words, bigG's chunk padded with id 0
     # after EOS), text_embeds from bigG's projected pooled row; the step above is released first
     del step
@@ -127,7 +132,10 @@ if args.lora_te:
     te = te.to_empty(device="cuda")
     random_init(te)
     te.requires_grad_(False).eval()
-    te_groups, te_lora = make_hcpdiff(te, None, [{"lr": 1e-5, "rank": 4, "layers": [r"re:.*self_attn$", r"re:.*mlp$"]}], default_lr=1e-5)
+    if args.full_te:
+        te_groups, te_lora = make_hcpdiff(te, [{"lr": 1e-6, "layers": [""]}], None, default_lr=1e-5)
+    else:
+        te_groups, te_lora = make_hcpdiff(te, None, [{"lr": 1e-5, "rank": 4, "layers": [r"re:.*self_attn$", r"re:.*mlp$"]}], default_lr=1e-5)
     step_te = LoraTrainStep(unet, [{"params": params}] + te_groups, text_encoder=te, text_encoder_opts={"clip_skip": 1, "clip_final_norm": False})
     g = torch.Generator().manual_seed(1)
     n_words = torch.randint(5, 70, (B,), generator=g)
@@ -147,11 +155,12 @@ if args.lora_te:
         C_, F_ = enc.config.hidden_size, enc.config.intermediate_size
         gflop[name] = n_layers * 2 * L * (4 * C_ * C_ + 2 * C_ * F_) / 1e9
     gflop["clip_bigG"] += 2 * 1280 * 1280 / 1e9
-    out.update({"ms_per_step_lora_te": ms_te, "images_per_s_lora_te": B / ms_te * 1e3,
-                "te_lora_params": sum(p.numel() for g in te_groups for p in g["params"]),
+    sfx = "full_te" if args.full_te else "lora_te"
+    out.update({f"ms_per_step_{sfx}": ms_te, f"images_per_s_{sfx}": B / ms_te * 1e3,
+                f"te_{'trained' if args.full_te else 'lora'}_params": sum(p.numel() for g in te_groups for p in g["params"]),
                 "te_forward_gemm_gflop_per_prompt": {k: round(v, 1) for k, v in gflop.items()},
-                "launches_per_step_lora_te": step_te.launches_per_step,
-                "loss_lora_te": float(step_te.loss.cpu()), "max_mem_gb": round(torch.cuda.max_memory_allocated() / 2 ** 30, 1)})
+                f"launches_per_step_{sfx}": step_te.launches_per_step, f"optimizer_state_bytes_{sfx}": step_te.optimizer_state_bytes,
+                f"loss_{sfx}": float(step_te.loss.cpu()), "max_mem_gb": round(torch.cuda.max_memory_allocated() / 2 ** 30, 1)})
 try:
     out["power_limit_w"] = float(subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", "0"],
                                                 capture_output=True, text=True, timeout=30).stdout.split()[0])
