@@ -116,53 +116,64 @@ __global__ void conv_out_dgrad_kernel(const float* __restrict__ dy, const float*
 }
 
 // ---------------------------------------------------------------------------------------------
-// skinny linear for M <= 16 rows: y[m,n] = sum_k f(x[m,k]) * W[n,k] + bias[n]   (one warp per output column n)
+// skinny linear over M rows: y[m,n] = sum_k f(x[m,k]) * W[n,k] + bias[n]   (one warp per output column n, 16 rows per CTA row)
 // in_mode: 0 identity, 1 SiLU, 2 x is the timestep [M] and the K inputs are its sinusoidal embedding
 //          ([cos | sin], flip_sin_to_cos=True, downscale_freq_shift=0 -- diffusers Timesteps for SD1.x)
+// blockIdx.y picks 16 rows; the transformed inputs are staged SK_KC columns at a time.  SK_KC is a multiple of 64, so every lane
+// still adds its k = lane*2 + 64 i terms in increasing k, and every row's sum is the same whatever M is.
 // ---------------------------------------------------------------------------------------------
-constexpr int SK_MAX_M = 16;
+constexpr int SK_ROWS = 16;
+constexpr int SK_KC = 512;
 __global__ void skinny_linear_kernel(const float* __restrict__ x, const __nv_bfloat16* __restrict__ Wt, const float* __restrict__ bias,
                                      int M, int K, int N, int in_mode, int out_silu, float* __restrict__ y) {
     pdl_trigger();
     pdl_wait();
-    extern __shared__ float sx[];   // [M][K] transformed inputs
-    for (int i = threadIdx.x; i < M * K; i += blockDim.x) {
-        const int m = i / K, k = i % K;
-        float v;
-        if (in_mode == 2) {
-            const int half = K / 2;
-            const int j = (k < half) ? k : k - half;
-            const float freq = expf(-9.210340371976184f * (float)j / (float)half);   // ln(10000)
-            const float a = x[m] * freq;
-            v = (k < half) ? cosf(a) : sinf(a);
-        } else {
-            v = x[(int64_t)m * K + k];
-            if (in_mode == 1) v = v / (1.f + __expf(-v));
-        }
-        sx[i] = v;
-    }
-    __syncthreads();
+    __shared__ float sx[SK_ROWS * SK_KC];   // [rows][kc] transformed inputs of one K chunk
+    const int m0 = blockIdx.y * SK_ROWS;
+    const int rows = min(SK_ROWS, M - m0);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int n = blockIdx.x * (blockDim.x >> 5) + warp;
-    if (n >= N) return;
-    float acc[SK_MAX_M];
+    const __nv_bfloat16* wr = Wt + (int64_t)min(n, N - 1) * K;
+    float acc[SK_ROWS];
 #pragma unroll
-    for (int m = 0; m < SK_MAX_M; ++m) acc[m] = 0.f;
-    const __nv_bfloat16* wr = Wt + (int64_t)n * K;
-    for (int k = lane * 2; k < K; k += 64) {
-        const float2 wv = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(wr + k));
+    for (int m = 0; m < SK_ROWS; ++m) acc[m] = 0.f;
+    for (int k0 = 0; k0 < K; k0 += SK_KC) {
+        const int kc = min(SK_KC, K - k0);
+        if (k0) __syncthreads();
+        for (int i = threadIdx.x; i < rows * kc; i += blockDim.x) {
+            const int m = i / kc, k = k0 + i % kc;
+            float v;
+            if (in_mode == 2) {
+                const int half = K / 2;
+                const int j = (k < half) ? k : k - half;
+                const float freq = expf(-9.210340371976184f * (float)j / (float)half);   // ln(10000)
+                const float a = x[m0 + m] * freq;
+                v = (k < half) ? cosf(a) : sinf(a);
+            } else {
+                v = x[(int64_t)(m0 + m) * K + k];
+                if (in_mode == 1) v = v / (1.f + __expf(-v));
+            }
+            sx[m * kc + (k - k0)] = v;
+        }
+        __syncthreads();
+        if (n < N) {
+            for (int k = lane * 2; k < kc; k += 64) {
+                const float2 wv = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(wr + k0 + k));
 #pragma unroll
-        for (int m = 0; m < SK_MAX_M; ++m)
-            if (m < M) acc[m] += sx[m * K + k] * wv.x + sx[m * K + k + 1] * wv.y;
+                for (int m = 0; m < SK_ROWS; ++m)
+                    if (m < rows) acc[m] += sx[m * kc + k] * wv.x + sx[m * kc + k + 1] * wv.y;
+            }
+        }
     }
+    if (n >= N) return;
 #pragma unroll
-    for (int m = 0; m < SK_MAX_M; ++m) {
-        if (m < M) {
+    for (int m = 0; m < SK_ROWS; ++m) {
+        if (m < rows) {
             float s = warp_sum(acc[m]);
             if (lane == 0) {
                 s += bias ? bias[n] : 0.f;
                 if (out_silu) s = s / (1.f + __expf(-s));
-                y[(int64_t)m * N + n] = s;
+                y[(int64_t)(m0 + m) * N + n] = s;
             }
         }
     }
@@ -544,18 +555,12 @@ extern "C" int hcp_conv_out_dgrad_f32(const float* dy, const float* w, int64_t B
 extern "C" int hcp_skinny_linear(const float* x, const void* w_bf16, const float* bias, int64_t M, int64_t K, int64_t N, int in_mode,
                                  int out_silu, float* y, hcp_stream_t st) {
     if (!x || !w_bf16 || !y) return set_error(HCP_ERR_INVALID, "skinny_linear: null pointer");
-    if (M < 1 || M > SK_MAX_M || (K & 1)) return set_error(HCP_ERR_INVALID, "skinny_linear: 1 <= M <= 16, even K");
-    const size_t smem = (size_t)M * K * sizeof(float);
-    if (smem > 96 * 1024) return set_error(HCP_ERR_INVALID, "skinny_linear: M*K too large");
-    static bool configured = false;
-    if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(skinny_linear_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
-        if (e != cudaSuccess) return set_cuda_error(e, "cudaFuncSetAttribute(skinny_linear)");
-        configured = true;
-    }
+    if (M < 1 || (K & 1)) return set_error(HCP_ERR_INVALID, "skinny_linear: M >= 1, even K");
+    if ((M + SK_ROWS - 1) / SK_ROWS > 65535 || M * K > INT32_MAX || N > INT32_MAX - 8)
+        return set_error(HCP_ERR_INVALID, "skinny_linear: M, K or N too large");
     const int warps = 8;
-    launch_k(skinny_linear_kernel, dim3((unsigned)((N + warps - 1) / warps)), dim3(warps * 32), smem, (cudaStream_t)st, 
-        x, (const __nv_bfloat16*)w_bf16, bias, (int)M, (int)K, (int)N, in_mode, out_silu, y);
+    launch_k(skinny_linear_kernel, dim3((unsigned)((N + warps - 1) / warps), (unsigned)((M + SK_ROWS - 1) / SK_ROWS)), dim3(warps * 32), 0,
+             (cudaStream_t)st, x, (const __nv_bfloat16*)w_bf16, bias, (int)M, (int)K, (int)N, in_mode, out_silu, y);
     LAUNCH_CHECK("skinny_linear launch");
     return HCP_OK;
 }

@@ -122,9 +122,10 @@ class Attention(nn.Module):
         g = self._groups()
         return [g.kv, g.q, g.out] if self.is_cross else [g.qkv, g.out]
 
-    def run(self, x: torch.Tensor, residual: torch.Tensor, context, kv_bias: Optional[torch.Tensor]) -> torch.Tensor:
+    def run(self, x: torch.Tensor, residual: torch.Tensor, context, kv_bias: Optional[torch.Tensor],
+            kv: Optional[torch.Tensor] = None) -> torch.Tensor:
         """`context`: the text embedding [B, Lc, ctx], a `_PerAttnContext` (one alias per cross-attention, when the embedding carries
-        a gradient) or a `_HoistedKV` holding the k/v projections computed ahead of time."""
+        a gradient) or a `_HoistedKV` holding the k/v projections computed ahead of time; `kv`: those projections, already taken."""
         g = self._groups()
         C_ = self.inner_dim
         if not self.is_cross:
@@ -132,7 +133,9 @@ class Attention(nn.Module):
             o = ops.attention(self.heads, C_, (0, C_, 2 * C_), qkv, None, None)
         else:
             q = g.q([x])
-            if isinstance(context, _HoistedKV):
+            if kv is not None:
+                pass
+            elif isinstance(context, _HoistedKV):
                 kv = context.take(self)
             else:
                 kv = g.kv([context.take(self) if isinstance(context, _PerAttnContext) else context])   # [B, Lc, 2C]
@@ -201,10 +204,15 @@ class FeedForward(nn.Module):
         g = self._groups()
         return [g.proj, g.out]
 
-    def run(self, x: torch.Tensor, residual: torch.Tensor) -> torch.Tensor:
+    def run(self, x: torch.Tensor, residual: torch.Tensor, skip_out: bool = False) -> torch.Tensor:
+        """`skip_out`: the rerun of a recompute region, where the out-projection's forward GEMM is needed only when it also produces
+        the merged-LoRA rank rows its backward reads."""
         g = self._groups()
         u = g.proj([x])
         h = ops.GegluFn.apply(u)
+        if skip_out:
+            with ops.skip_output():
+                return g.out([h], residual=residual)
         return g.out([h], residual=residual)
 
 
@@ -218,13 +226,30 @@ class BasicTransformerBlock(nn.Module):
         self.norm2 = nn.LayerNorm(dim, eps=ln_eps)
         self.norm3 = nn.LayerNorm(dim, eps=ln_eps)
 
-    def run(self, h: torch.Tensor, context: torch.Tensor, kv_bias: Optional[torch.Tensor]) -> torch.Tensor:
+    def run(self, h: torch.Tensor, context, kv_bias: Optional[torch.Tensor], checkpoint: bool = False) -> torch.Tensor:
+        """`checkpoint`: run the block as one recompute region (ops.checkpoint).  The first pass keeps the block's input, the
+        cross-attention's context (or its hoisted k/v) and each attention's output and LSE rows; the backward reruns the block from
+        them.  The context enters the region as a tensor taken once, so the hoisted k/v projections are not recomputed."""
+        if not checkpoint:
+            return self._run(h, context, None, kv_bias)
+        kv = context.take(self.attn2) if isinstance(context, _HoistedKV) else None
+        c = kv if kv is not None else (context.take(self.attn2) if isinstance(context, _PerAttnContext) else context)
+        params = [p for p in self.parameters() if p.requires_grad]
+        if not (params or h.requires_grad or c.requires_grad):
+            return self._run(h, c, kv, kv_bias)
+        hoisted = kv is not None
+
+        def region(h, c, recompute):
+            return self._run(h, c, c if hoisted else None, kv_bias, recompute)
+        return ops.checkpoint(region, (h, c), params)
+
+    def _run(self, h, context, kv, kv_bias, recompute: bool = False) -> torch.Tensor:
         n, a = ops.layer_norm(self.norm1.weight, self.norm1.bias, self.norm1.eps, h)
         h = self.attn1.run(n, a, None, None)
         n, a = ops.layer_norm(self.norm2.weight, self.norm2.bias, self.norm2.eps, h)
-        h = self.attn2.run(n, a, context, kv_bias)
+        h = self.attn2.run(n, a, context, kv_bias, kv=kv)
         n, a = ops.layer_norm(self.norm3.weight, self.norm3.bias, self.norm3.eps, h)
-        return self.ff.run(n, a)
+        return self.ff.run(n, a, skip_out=recompute)
 
 
 class Transformer2DModel(nn.Module):
@@ -253,13 +278,13 @@ class Transformer2DModel(nn.Module):
         g = self._groups()
         return [g.proj_in, g.proj_out]
 
-    def run(self, x: torch.Tensor, context: torch.Tensor, kv_bias: Optional[torch.Tensor]) -> torch.Tensor:
+    def run(self, x: torch.Tensor, context: torch.Tensor, kv_bias: Optional[torch.Tensor], checkpoint: bool = False) -> torch.Tensor:
         g = self._groups()
         n = self.norm
         y, alias = ops.group_norm(n.weight, n.bias, n.num_groups, n.eps, False, x, None)
         h = g.proj_in([y])                      # NHWC tokens: the 1x1 conv is a GEMM, the permute is free
         for blk in self.transformer_blocks:
-            h = blk.run(h, context, kv_bias)
+            h = blk.run(h, context, kv_bias, checkpoint)
         return g.proj_out([h], residual=alias)
 
 
@@ -413,8 +438,15 @@ class UNet2DConditionModel(nn.Module):
         return self.conv_in.weight.device
 
     def enable_gradient_checkpointing(self):
-        """Accepted for config compatibility (reference cfgs/train/train_base.yaml:69).  Activation recomputation is not used:
-        an H100 holds the SD1.5 activations of the benchmark batch sizes many times over."""
+        """Recompute every BasicTransformerBlock in the backward instead of keeping its intermediates (the reference turns this on
+        with `model.gradient_checkpointing`, cfgs/train/train_base.yaml:69).
+
+        With the flag set, a training forward keeps per block only its input, its two attention outputs and their LSE rows; the
+        backward reruns the block's LayerNorms and linears on the same kernels (the attention forward is not rerun, the
+        feed-forward out-projection's GEMM only when merged LoRA rank rows ride it) and then runs the block's backward.  Results are
+        bit-identical to the flag off.  ResnetBlocks, the Transformer2DModel's GroupNorm / proj_in / proj_out, the time embedding and
+        the text encoder keep their activations.  The flag costs the recompute's time and lowers the activation memory of each image,
+        which lets larger batches fit; it has no effect without grad mode."""
         self.gradient_checkpointing = True
 
     def enable_xformers_memory_efficient_attention(self, *args, **kwargs):
@@ -663,6 +695,7 @@ class UNet2DConditionModel(nn.Module):
             ctx = _PerAttnContext(encoder_hidden_states, attn2s)
         else:
             ctx = ops.cast_bf16(encoder_hidden_states)
+        ckpt = self.gradient_checkpointing and torch.is_grad_enabled()
         kv_bias = None
         if encoder_attention_mask is not None:
             kv_bias = ((1.0 - encoder_attention_mask.to(torch.float32)) * -10000.0).contiguous()
@@ -685,20 +718,20 @@ class UNet2DConditionModel(nn.Module):
             for j, res in enumerate(blk.resnets):
                 h = res.run([h], geom, next(tembs))
                 if blk.has_attn:
-                    h = blk.attentions[j].run(h, ctx, kv_bias)
+                    h = blk.attentions[j].run(h, ctx, kv_bias, ckpt)
                 h = push(h)
             if hasattr(blk, "downsamplers"):
                 h = blk.downsamplers[0].run(h, geom)
                 geom = (B, geom[1] // 2, geom[2] // 2)
                 h = push(h)
         h = self.mid_block.resnets[0].run([h], geom, next(tembs))
-        h = self.mid_block.attentions[0].run(h, ctx, kv_bias)
+        h = self.mid_block.attentions[0].run(h, ctx, kv_bias, ckpt)
         h = self.mid_block.resnets[1].run([h], geom, next(tembs))
         for blk in self.up_blocks:
             for j, res in enumerate(blk.resnets):
                 h = res.run([h, skips.pop()], geom, next(tembs))
                 if blk.has_attn:
-                    h = blk.attentions[j].run(h, ctx, kv_bias)
+                    h = blk.attentions[j].run(h, ctx, kv_bias, ckpt)
             if hasattr(blk, "upsamplers"):
                 h = blk.upsamplers[0].run(h, geom)
                 geom = (B, geom[1] * 2, geom[2] * 2)

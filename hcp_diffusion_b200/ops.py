@@ -221,6 +221,77 @@ def dropout_cols(y, ranges, residual=None, rowbias=None, rows_per_group=0):
 
 
 # ----------------------------------------------------------------------------------------------------------------------
+# recompute regions (UNet2DConditionModel.gradient_checkpointing): the first pass runs a region without recording autograd nodes and
+# keeps its inputs plus each attention's (o, lse); the backward reruns the region with grad enabled and back-propagates through it.
+# The attentions of the rerun hand back the kept (o, lse) instead of launching the forward kernel again, and the region's last linear
+# skips its GEMM when its backward reads only its input (`skip_output`).
+# ----------------------------------------------------------------------------------------------------------------------
+class _Region:
+    record: Optional[list] = None      # first pass: AttentionFn appends (o, lse) here
+    replay = None                      # rerun: iterator of the kept (o, lse), in launch order
+    skip_gemm = False
+
+
+class skip_output:
+    """Inside a region's rerun: the linear called under this context leaves its output unwritten (its value is never read, only its
+    autograd node is) unless the GEMM also produces a tensor its backward reads (the merged-LoRA rank rows)."""
+
+    def __enter__(self):
+        _Region.skip_gemm = True
+
+    def __exit__(self, *exc):
+        _Region.skip_gemm = False
+
+
+class CheckpointFn(torch.autograd.Function):
+    """out = run(*inputs) with the intermediates recomputed in the backward.  `inputs`: the tensors `run` reads that come from outside
+    the region (their gradients are returned); `params`: the trained parameters inside it (autograd inputs so that the node exists
+    when no input carries a gradient; their kernels accumulate into .grad in place, as without the region).  `run(*inputs,
+    recompute=bool)` must launch the same work both times; dropout masks repeat because the rerun starts from the same call-site
+    number."""
+
+    @staticmethod
+    def forward(ctx, run, n_in: int, *args):
+        ins = args[:n_in]
+        ctx.run, ctx.n_in, ctx.n_params, ctx.site = run, n_in, len(args) - n_in, _Drop.site
+        kept, outer = [], _Region.record
+        _Region.record = kept
+        try:
+            out = run(*ins, recompute=False)
+        finally:
+            _Region.record = outer
+        ctx.save_for_backward(*ins, *(t for pair in kept for t in pair))
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        saved = ctx.saved_tensors
+        ins = [None if t is None else t.detach().requires_grad_(bool(need))
+               for t, need in zip(saved[:ctx.n_in], ctx.needs_input_grad[2:2 + ctx.n_in])]
+        kept = saved[ctx.n_in:]
+        n_keep = len(_Side.keep)
+        site, outer = _Drop.site, _Region.replay
+        _Drop.site, _Region.replay = ctx.site, iter(zip(kept[0::2], kept[1::2]))
+        try:
+            with torch.enable_grad():
+                out = ctx.run(*ins, recompute=True)
+        finally:
+            _Drop.site, _Region.replay = site, outer
+        torch.autograd.backward(out, dout)
+        del out
+        if _Side.used:
+            # the side stream's LoRA-gradient kernels read the recomputed tensors: the main stream waits for them here, so that the
+            # tensors are released now instead of at the end of the backward (the region would otherwise keep them all alive)
+            torch.cuda.current_stream().wait_stream(_Side.stream)
+            del _Side.keep[n_keep:]
+        return (None, None, *(t.grad if t is not None and t.requires_grad else None for t in ins), *([None] * ctx.n_params))
+
+
+def checkpoint(run, inputs: Sequence[Optional[torch.Tensor]], params: Sequence[torch.Tensor]) -> torch.Tensor:
+    return CheckpointFn.apply(run, len(inputs), *inputs, *params)
+
+
+# ----------------------------------------------------------------------------------------------------------------------
 # gradient-ready notifications (full fine-tune, data parallel): the engine buckets the flat gradient buffer and all-reduces a bucket
 # as soon as the kernels producing its last parameter gradient have been enqueued (the reference's DDP reducer hooks).
 # ----------------------------------------------------------------------------------------------------------------------
@@ -661,7 +732,10 @@ class FusedLinearFn(torch.autograd.Function):
         res = None
         if residual is not None:
             res = _chk(residual, "linear residual")
-        if pack.ext_rp and any(ctx.needs_input_grad[3 + n_x:]):
+        ext = pack.ext_rp and any(ctx.needs_input_grad[3 + n_x:])
+        if _Region.skip_gemm and not ext:
+            pass                                # a region's rerun: nothing reads this output, only the node and its saved inputs count
+        elif ext:
             # the factor gradients will need T = x W_down^T: it rides this GEMM as ext_rp extra output columns
             T = torch.empty((M, pack.R), dtype=BF16, device=xs[0].device)
             gemm_raw(a_list, [(pack.W, pack.K, N + pack.ext_rp, 0)], M, N + pack.ext_rp, out, N, bias=pack.bias, residual=res, ldr=N,
@@ -1047,17 +1121,22 @@ class AttentionFn(torch.autograd.Function):
         _, Lkv, ldkv = kvt.shape
         d = C_ // heads
         scale = 1.0 / math.sqrt(d)
-        o = torch.empty((B, Lq, C_), dtype=BF16, device=q_src.device)
-        lse = torch.empty((B, heads, Lq), dtype=torch.float32, device=q_src.device)
-        a = AttnArgs()
-        a.q, a.ldq = q_src.data_ptr() + 2 * offs[0], ldq
-        a.k, a.ldk = kvt.data_ptr() + 2 * offs[1], ldkv
-        a.v, a.ldv = kvt.data_ptr() + 2 * offs[2], ldkv
-        a.B, a.H, a.Lq, a.Lkv, a.d = B, heads, Lq, Lkv, d
-        a.scale = scale
-        a.kv_bias = ptr(kv_bias)
-        a.o, a.ldo, a.lse = o.data_ptr(), C_, lse.data_ptr()
-        call("hcp_attn_fwd_causal_bf16" if causal else "hcp_attn_fwd_bf16", C.byref(a), stream_ptr())
+        if _Region.replay is not None:          # rerun of a recompute region: the first pass's output and row statistics
+            o, lse = (t.detach() for t in next(_Region.replay))
+        else:
+            o = torch.empty((B, Lq, C_), dtype=BF16, device=q_src.device)
+            lse = torch.empty((B, heads, Lq), dtype=torch.float32, device=q_src.device)
+            a = AttnArgs()
+            a.q, a.ldq = q_src.data_ptr() + 2 * offs[0], ldq
+            a.k, a.ldk = kvt.data_ptr() + 2 * offs[1], ldkv
+            a.v, a.ldv = kvt.data_ptr() + 2 * offs[2], ldkv
+            a.B, a.H, a.Lq, a.Lkv, a.d = B, heads, Lq, Lkv, d
+            a.scale = scale
+            a.kv_bias = ptr(kv_bias)
+            a.o, a.ldo, a.lse = o.data_ptr(), C_, lse.data_ptr()
+            call("hcp_attn_fwd_causal_bf16" if causal else "hcp_attn_fwd_bf16", C.byref(a), stream_ptr())
+            if _Region.record is not None:
+                _Region.record.append((o, lse))
         ctx.save_for_backward(q_src, kvt, o, lse, kv_bias)
         ctx.cfg = (heads, C_, offs, same, scale, causal)
         return o
@@ -1403,7 +1482,7 @@ def small_linear(x, w_bf16, bias, silu, train=None):
 
 
 def skinny_linear(x: torch.Tensor, w_bf16: torch.Tensor, bias: Optional[torch.Tensor], in_mode: int, out_silu: bool) -> torch.Tensor:
-    """fp32 [M<=16, K] (or timesteps [M] when in_mode == 2) -> fp32 [M, N]."""
+    """fp32 [M, K] (or timesteps [M] when in_mode == 2) -> fp32 [M, N]."""
     N, K = w_bf16.shape
     M = x.shape[0]
     y = torch.empty((M, N), dtype=torch.float32, device=w_bf16.device)

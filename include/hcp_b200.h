@@ -277,7 +277,8 @@ int hcp_conv_out_f32(const void* x_nhwc_bf16, const float* w, const float* bias,
                      int64_t Cout, float* y_nchw, hcp_stream_t stream);
 int hcp_conv_out_dgrad_f32(const float* dy_nchw, const float* w, int64_t B, int64_t H, int64_t W, int64_t Cin, int64_t Cout,
                            void* dx_nhwc_bf16, hcp_stream_t stream);
-/* y[M,N] fp32 = f(x)[M,K] . W[N,K]^T + bias, M <= 16.  in_mode 0: f = id, 1: f = SiLU, 2: x is timesteps [M] and f is the
+/* y[M,N] fp32 = f(x)[M,K] . W[N,K]^T + bias, any M >= 1 (16 rows per CTA row of the grid, K staged in 512-column chunks; every row
+ * is summed in the same order whatever M is, so a row's result does not depend on the rows launched with it).  in_mode 0: f = id, 1: f = SiLU, 2: x is timesteps [M] and f is the
  * sinusoidal embedding (diffusers Timesteps: [cos | sin], freq = exp(-ln(1e4) * j / (K/2))).  W is bf16. */
 int hcp_skinny_linear(const float* x, const void* w_bf16, const float* bias, int64_t M, int64_t K, int64_t N, int in_mode,
                       int out_silu, float* y, hcp_stream_t stream);

@@ -6,7 +6,7 @@ Workloads (SD1.5 UNet, 512x512 = 64x64 latents, 77 x 768 text, synthetic weights
   ft          full fine-tune of every UNet parameter, batch 16 (BASELINE config 3 shapes)
   ft4         full fine-tune, instance batch 4 (DreamBooth.yaml's dataset1)
   ft4+class   the same with a masked class group of 1 (DreamBooth.yaml's dataset_class)
-(The UNet's time-embedding kernel takes at most 16 images per pass, so the class group rides on DreamBooth's batch 4, not on 16.)
+(One UNet pass takes any number of images; the class group rides on DreamBooth.yaml's instance batch 4.)
 One JSON line per workload: ms per step (CUDA events around K steps, each ending with the D2H read of the logged loss, as the
 reference's loss.item()) and images/s counting every group's images, with the card's name and power limit read in the same run.
 """
