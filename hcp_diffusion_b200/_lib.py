@@ -148,8 +148,8 @@ EXPORTS = [
     "hcp_layernorm_fwd_bf16", "hcp_layernorm_bwd_bf16", "hcp_geglu_fwd_bf16", "hcp_geglu_bwd_bf16",
     "hcp_upsample2x_fwd_bf16", "hcp_upsample2x_bwd_bf16", "hcp_add_bf16",
     "hcp_sinusoid_f32", "hcp_conv_in_f32", "hcp_conv_out_f32", "hcp_conv_out_dgrad_f32", "hcp_skinny_linear", "hcp_cast_f32_to_bf16",
-    "hcp_lora_pack", "hcp_lora_merge", "hcp_lora_pack_conv", "hcp_lora_grad", "hcp_lora_grad_pair", "hcp_lora_grad_conv3x3", "hcp_add_noise", "hcp_mse_loss", "hcp_sumsq", "hcp_adamw_flat",
-    "hcp_adamw_flat_dev", "hcp_lion_flat_dev", "hcp_snr_mse_loss", "hcp_ema_flat", "hcp_dropout_bf16", "hcp_counter_add_u64", "hcp_cfg_mix_f32",
+    "hcp_lora_pack", "hcp_lora_merge", "hcp_lora_pack_conv", "hcp_lora_grad", "hcp_lora_grad_pair", "hcp_lora_grad_conv3x3", "hcp_sumsq", "hcp_adamw_flat",
+    "hcp_adamw_flat_dev", "hcp_lion_flat_dev", "hcp_ema_flat", "hcp_dropout_bf16", "hcp_counter_add_u64", "hcp_cfg_mix_f32",
     "hcp_wgrad_bf16", "hcp_wgrad_conv3x3_bf16", "hcp_colsum_bf16", "hcp_norm_affine_grad_bf16", "hcp_small_linear_bwd_f32", "hcp_silu_f32",
     "hcp_conv_in_wgrad_f32", "hcp_conv_out_wgrad_f32", "hcp_repack_weights", "hcp_adafactor_flat", "hcp_adamw8bit_flat", "hcp_prodigy_flat",
     "hcp_attn_fwd_causal_bf16", "hcp_attn_bwd_causal_bf16", "hcp_quick_gelu_fwd_bf16", "hcp_quick_gelu_bwd_bf16", "hcp_embed_gather_bf16",
@@ -220,8 +220,6 @@ def lib() -> C.CDLL:
             l.hcp_lora_grad.argtypes = [vp, i64, vp, i64, i64, i64, i64, C.POINTER(LoraGradBlock), C.c_int32, vp]
             l.hcp_lora_grad_pair.argtypes = [vp, vp, i64, i64, C.POINTER(LoraGradBlock), vp, vp, i64, i64, C.POINTER(LoraGradBlock),
                                              C.c_int32, i64, i64, vp]
-            l.hcp_add_noise.argtypes = [vp, vp, vp, vp, i64, i64, vp, vp]
-            l.hcp_mse_loss.argtypes = [vp, vp, i64, f32, vp, vp, vp]
             l.hcp_sumsq.argtypes = [vp, i64, vp, vp]
             l.hcp_adamw_flat.argtypes = [vp, vp, vp, vp, i64, vp, f32, f32, f32, f32, f32, vp, f32, vp, vp]
             l.hcp_adamw_flat_dev.argtypes = [vp, vp, vp, vp, i64, vp, f32, vp, f32, vp, vp]
@@ -229,7 +227,6 @@ def lib() -> C.CDLL:
             l.hcp_adafactor_flat.argtypes = [vp, vp, vp, vp, vp, vp, vp, i64, vp, i64, vp, vp, C.c_int32, f32, vp, f32, vp]
             l.hcp_adamw8bit_flat.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, C.c_int32, vp, vp, i64, i64, i64, i64, i64, vp, vp,
                                              C.c_int32, f32, vp, f32, vp]
-            l.hcp_snr_mse_loss.argtypes = [vp, vp, vp, vp, f32, C.c_int32, i64, i64, f32, vp, vp, vp]
             l.hcp_eps_loss_grouped.argtypes = [vp, vp, vp, vp, vp, vp, vp, C.c_int32, C.c_int32, f32, i64, i64, i64, f32, vp, vp, vp,
                                                C.c_size_t, vp]
             l.hcp_ema_flat.argtypes = [vp, vp, i64, vp, f32, f32, f32, vp]

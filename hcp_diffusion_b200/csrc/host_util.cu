@@ -149,7 +149,7 @@ ConvTap conv_tap(int kh, int kw, int stride, int64_t C) {
 
 }  // namespace hcp
 
-extern "C" int hcp_version(void) { return 2; }
+extern "C" int hcp_version(void) { return 3; }
 extern "C" unsigned long long hcp_launch_count(void) { return hcp::g_launches.load(std::memory_order_relaxed); }
 extern "C" const char* hcp_last_error_string(void) { return hcp::g_err; }
 extern "C" int hcp_device_check(void) {

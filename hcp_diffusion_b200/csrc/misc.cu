@@ -1,13 +1,13 @@
 // SPDX-License-Identifier: Apache-2.0
 // Small kernels at the edges of the UNet hot path (sm_90a): the 4-channel convolutions conv_in / conv_out
 // (NCHW fp32 at the module boundary <-> bf16 NHWC inside), the timestep-embedding MLP and all ResnetBlock2D
-// time_emb_proj layers as one skinny linear, LoRA parameter packing and LoRA gradient reduction, and the loss /
-// optimizer kernels either side of the UNet call.
+// time_emb_proj layers as one skinny linear, LoRA parameter packing and LoRA gradient reduction, and the
+// gradient-norm / optimizer kernels after the UNet call.
 //
 // Replaces (reference): diffusers conv_in / conv_out / Timesteps / TimestepEmbedding / time_emb_proj
 // (cfgs/unet_struct.txt:2-8,95,931); LoraBlock.get_weight's alpha*W_up@W_down materialisation
 // (hcpdiff/models/lora_base_patch.py:61-62) -> packed low-rank operands; autograd of W_down/W_up;
-// Trainer.get_loss (hcpdiff/train_ac.py:506-515) and the AdamW step on the LoRA parameters (train_ac.py:485-494).
+// clip_grad_norm_ and the AdamW step on the LoRA parameters (train_ac.py:485-494).
 #include "common.cuh"
 #include "host_util.h"
 #include "../../include/hcp_b200.h"
@@ -388,41 +388,6 @@ __global__ void __launch_bounds__(256) lora_merge_kernel(const hcp_lora_merge_jo
 
 #undef s_up
 
-// ---------------------------------------------------------------------------------------------
-// loss = mean((pred - target)^2) (fp32, reference train_ac.py:506-515 with loss.type == 'eps'), dpred = 2(pred-target)/n
-// ---------------------------------------------------------------------------------------------
-__global__ void mse_loss_kernel(const float* __restrict__ pred, const float* __restrict__ target, int64_t n, float grad_scale,
-                                float* __restrict__ loss_sum, float* __restrict__ dpred) {
-    pdl_trigger();
-    pdl_wait();
-    __shared__ float s_part[8];
-    float acc = 0.f;
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-        const float d = pred[i] - target[i];
-        acc += d * d;
-        if (dpred) dpred[i] = 2.f * d * grad_scale / (float)n;
-    }
-    acc = warp_sum(acc);
-    if ((threadIdx.x & 31) == 0) s_part[threadIdx.x >> 5] = acc;
-    __syncthreads();
-    if (threadIdx.x < 32) {
-        float v = (threadIdx.x < (blockDim.x >> 5)) ? s_part[threadIdx.x] : 0.f;
-        v = warp_sum(v);
-        if (threadIdx.x == 0) atomicAdd(loss_sum, v / (float)n);
-    }
-}
-
-// x_t = sqrt(acp[t]) * x0 + sqrt(1 - acp[t]) * noise   (DDPMScheduler.add_noise, reference train_ac.py:437-447)
-__global__ void add_noise_kernel(const float* __restrict__ x0, const float* __restrict__ noise, const int64_t* __restrict__ t,
-                                 const float* __restrict__ acp, int64_t per_image, int64_t n, float* __restrict__ xt) {
-    pdl_trigger();
-    pdl_wait();
-    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const float a = acp[t[i / per_image]];
-    xt[i] = sqrtf(a) * x0[i] + sqrtf(1.f - a) * noise[i];
-}
-
 // sum of squares of a flat fp32 buffer (for clip_grad_norm_, reference train_ac.py:485-490)
 __global__ void sumsq_kernel(const float* __restrict__ g, int64_t n, float* __restrict__ out) {
     pdl_trigger();
@@ -611,29 +576,6 @@ extern "C" int hcp_lora_pack_conv(const hcp_lora_conv_job* jobs_device, int64_t 
     dim3 grid(16, (unsigned)njobs);
     launch_k(lora_pack_conv_kernel, dim3(grid), dim3(256), 0, (cudaStream_t)st, jobs_device, (int)njobs);
     LAUNCH_CHECK("lora_pack_conv launch");
-    return HCP_OK;
-}
-
-extern "C" int hcp_mse_loss(const float* pred, const float* target, int64_t n, float grad_scale, float* loss_sum, float* dpred,
-                            hcp_stream_t st) {
-    if (!pred || !target || !loss_sum) return set_error(HCP_ERR_INVALID, "mse_loss: null pointer");
-    if (n < 0) return set_error(HCP_ERR_INVALID, "mse_loss: negative size");
-    if (n == 0) return HCP_OK;
-    int blocks = (int)((n + 255) / 256);
-    if (blocks > 592) blocks = 592;
-    launch_k(mse_loss_kernel, dim3(blocks), dim3(256), 0, (cudaStream_t)st, pred, target, n, grad_scale, loss_sum, dpred);
-    LAUNCH_CHECK("mse_loss launch");
-    return HCP_OK;
-}
-
-extern "C" int hcp_add_noise(const float* x0, const float* noise, const int64_t* t, const float* alphas_cumprod, int64_t B,
-                             int64_t per_image, float* xt, hcp_stream_t st) {
-    if (!x0 || !noise || !t || !alphas_cumprod || !xt) return set_error(HCP_ERR_INVALID, "add_noise: null pointer");
-    if (B < 0 || per_image < 0) return set_error(HCP_ERR_INVALID, "add_noise: negative size");
-    const int64_t n = B * per_image;
-    if (n == 0) return HCP_OK;
-    launch_k(add_noise_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, (cudaStream_t)st, x0, noise, t, alphas_cumprod, per_image, n, xt);
-    LAUNCH_CHECK("add_noise launch");
     return HCP_OK;
 }
 

@@ -1,14 +1,14 @@
 // SPDX-License-Identifier: Apache-2.0
-// Training-step kernels either side of the UNet call that the plain MSE / AdamW pair of misc.cu does not cover (sm_90a):
-//   * SNR-weighted eps loss (reference hcpdiff/loss/min_snr_loss.py:5-52: MinSNR / SoftMinSNR / KDiffMinSNR / EDM weights)
-//   * the same loss over several data groups of one step with per-sample weights and a per-pixel mask (prior preservation,
-//     att_mask; reference hcpdiff/train_ac.py:467-482, 506-515), reduced in a fixed order
+// Training-step kernels either side of the UNet call (sm_90a; the clip and optimizer kernels are in misc.cu and optim.cu):
+//   * the eps loss, plain MSE or SNR-weighted (reference hcpdiff/loss/min_snr_loss.py:5-52: MinSNR / SoftMinSNR / KDiffMinSNR /
+//     EDM weights), over the data groups of one step with per-sample weights and a per-pixel mask (prior preservation, att_mask;
+//     reference hcpdiff/train_ac.py:467-482, 506-515), reduced in a fixed order
 //   * exponential moving average of the flat trainable buffer (reference hcpdiff/utils/ema.py:18-32)
 //   * nn.Dropout on a patched layer's output (reference hcpdiff/models/lora_base_patch.py:74), counter-based RNG so that the
 //     backward pass regenerates the forward mask instead of storing it, and CUDA-graph replays draw fresh masks
 //   * the DreamArtist classifier-free-guidance mix of the two UNet halves (reference hcpdiff/models/cfg_context.py:23-39)
 //   * pyramid noise (reference hcpdiff/noise/pyramid_noise.py:17-32): device-drawn level sizes, the level grids, their bilinear
-//     sum onto the base noise with a per-group std, and add_noise on the normalised sum
+//     sum onto the base noise with a per-group std, and add_noise on the normalised sum (1/std = 1: DDPMScheduler.add_noise)
 // All of them are HBM-bound elementwise kernels over at most a few MB.
 #include <algorithm>
 #include <cmath>
@@ -26,7 +26,7 @@ namespace hcp {
     } while (0)
 
 // ---------------------------------------------------------------------------------------------
-// loss = mean_i( w(t_b) * (pred_i - target_i)^2 ),  dpred_i = 2 w d grad_scale / n
+// Min-SNR family loss weights w(t_b) of the eps loss below:
 //   snr = acp / (1 - acp)  ( = (alpha/sigma)^2 of min_snr_loss.py:16-19 )
 //   mode 0 MinSNR      w = min(gamma / snr, 1)
 //   mode 1 SoftMinSNR  w = gamma^3 / (snr^2 + gamma^3)
@@ -40,29 +40,6 @@ __device__ __forceinline__ float snr_weight(float acp, float gamma, int mode) {
     if (mode == 2) { const float a = gamma * snr, b = snr * snr + gamma * gamma; return 4.f * (a * a) / (b * b); }
     const float s2 = 1.f - acp;
     return (s2 + gamma * gamma) / (snr * (s2 * gamma * gamma));
-}
-
-__global__ void snr_mse_loss_kernel(const float* __restrict__ pred, const float* __restrict__ target, const int64_t* __restrict__ t,
-                                    const float* __restrict__ acp, float gamma, int mode, int64_t per_image, int64_t n, float grad_scale,
-                                    float* __restrict__ loss_sum, float* __restrict__ dpred) {
-    pdl_trigger();
-    pdl_wait();
-    __shared__ float s_part[8];
-    float acc = 0.f;
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-        const float w = snr_weight(acp[t[i / per_image]], gamma, mode);
-        const float d = pred[i] - target[i];
-        acc += w * d * d;
-        if (dpred) dpred[i] = 2.f * w * d * grad_scale / (float)n;
-    }
-    acc = warp_sum(acc);
-    if ((threadIdx.x & 31) == 0) s_part[threadIdx.x >> 5] = acc;
-    __syncthreads();
-    if (threadIdx.x < 32) {
-        float v = (threadIdx.x < (blockDim.x >> 5)) ? s_part[threadIdx.x] : 0.f;
-        v = warp_sum(v);
-        if (threadIdx.x == 0) atomicAdd(loss_sum, v / (float)n);
-    }
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -523,19 +500,6 @@ __global__ void add_noise_scaled_kernel(const float* __restrict__ x0, const floa
 }  // namespace hcp
 
 using namespace hcp;
-
-extern "C" int hcp_snr_mse_loss(const float* pred, const float* target, const int64_t* t, const float* alphas_cumprod, float gamma,
-                                int32_t mode, int64_t per_image, int64_t n, float grad_scale, float* loss_sum, float* dpred,
-                                hcp_stream_t st) {
-    if (!pred || !target || !t || !alphas_cumprod || !loss_sum) return set_error(HCP_ERR_INVALID, "snr_mse_loss: null pointer");
-    if (mode < 0 || mode > 3 || per_image <= 0 || n <= 0 || gamma <= 0.f) return set_error(HCP_ERR_INVALID, "snr_mse_loss: arguments");
-    int blocks = (int)((n + 255) / 256);
-    if (blocks > 592) blocks = 592;
-    launch_k(snr_mse_loss_kernel, dim3(blocks), dim3(256), 0, (cudaStream_t)st, pred, target, t, alphas_cumprod, gamma, (int)mode, per_image, n,
-             grad_scale, loss_sum, dpred);
-    LAUNCH_CHECK("snr_mse_loss launch");
-    return HCP_OK;
-}
 
 extern "C" size_t hcp_eps_loss_grouped_workspace_bytes(int64_t B, int64_t per_image) {
     if (B <= 0 || per_image <= 0) return 0;

@@ -221,7 +221,6 @@ class LoraTrainStep:
         self.unet = unet
         self.loss_weights = None if loss_weights is None else [float(w) for w in loss_weights]
         self._group_tables: Dict[tuple, dict] = {}
-        self._graph_kind = None                            # 'step' or 'groups': which public call the CUDA graphs were captured for
         self.te, self.te_opts, self.sdxl = text_encoder, None, False
         if text_encoder is not None:
             if cfg_scale is not None:
@@ -353,7 +352,7 @@ class LoraTrainStep:
             self.acp = self.noise_sched.alphas_cumprod.to(dev)
         pyr = None if self.noise_sched is None else self.noise_sched.pyramid
         self.pyramid = None if pyr is None else ops.PyramidNoise(pyr["level"], pyr["discount"], pyr["step_size"], dev)
-        self.loss = torch.zeros(1, dtype=torch.float32, device=dev)
+        self.loss: Optional[torch.Tensor] = None           # the loss tensor of the last micro-step ([1] after step(), [G] after step_groups())
         self.noise_pred: Optional[torch.Tensor] = None     # the UNet output of the last micro-step (kept alive across graph replays)
         self.gsq = torch.zeros(1, dtype=torch.float32, device=dev)
         self.use_graph = use_cuda_graph
@@ -474,18 +473,20 @@ class LoraTrainStep:
                 self.ema.copy_(self.flat.data)
 
     # ---- pieces ------------------------------------------------------------------------------------------------------
-    def _forward_backward(self, latents, noise, t, ehs, added=None, grouped=None):
-        """x_t = add_noise, pred = unet(x_t, t, ehs), loss, backward (gradients ACCUMULATE into the flat buffer).  `grouped`: the
-        device tables of `step_groups()` (per-group weighted, masked loss into grouped['loss'])."""
+    def _forward_backward(self, latents, noise, t, ehs, added=None, tables=None, mask=None):
+        """x_t = add_noise, pred = unet(x_t, t, ehs), loss, backward (gradients ACCUMULATE into the flat buffer).  `tables`: the
+        device tables of the batch's group layout (`_tables`; None: one group of weight 1), `mask` fp32 [B, HW] or None; the
+        per-group weighted, masked loss goes to tables['loss'], which becomes `self.loss`."""
+        if tables is None:
+            tables = self._tables((latents.shape[0],), (1.0,), latents.shape[1], latents[0, 0].numel())
+        self.loss = tables["loss"]
         self.loss.zero_()
-        if grouped is not None:
-            grouped["loss"].zero_()
         ops.set_side_stream(self.side_stream)
         overlap = self.buckets is not None and self._micro == self.accum - 1      # DDP no_sync on all but the last micro-step
         if overlap:
             ops.set_grad_ready_callback(self.buckets.on_grad)
         try:
-            self._fb_body(latents, noise, t, ehs, added, grouped)
+            self._fb_body(latents, noise, t, ehs, added, tables, mask)
         finally:
             ops.set_grad_ready_callback(None)
             ops.join_side()
@@ -499,15 +500,15 @@ class LoraTrainStep:
         if self.pyramid is not None:
             self.pyramid.set_seed(seed)
 
-    def _fb_body(self, latents, noise, t, ehs, added=None, grouped=None):
-        B = latents.shape[0]
-        per_image = latents[0].numel()
+    def _fb_body(self, latents, noise, t, ehs, added, tables, mask):
+        B, C = latents.shape[:2]
+        HW = latents[0, 0].numel()
         if self.pyramid is not None:                       # PyramidNoiseScheduler.add_noise per group; the loss target is its sum
-            x_t, noise = self.pyramid.add_noise(latents, noise, t, self.acp, (B,) if grouped is None else grouped["sizes"])
+            x_t, noise = self.pyramid.add_noise(latents, noise, t, self.acp, tables["sizes"])
         else:
             x_t = torch.empty_like(latents)
-            call("hcp_add_noise", latents.data_ptr(), noise.data_ptr(), t.data_ptr(), self.acp.data_ptr(), B, per_image, x_t.data_ptr(),
-                 stream_ptr())
+            call("hcp_add_noise_scaled", latents.data_ptr(), noise.data_ptr(), t.data_ptr(), self.acp.data_ptr(), tables["inv_std"].data_ptr(),
+                 tables["group_start"].data_ptr(), 1, B, C * HW, x_t.data_ptr(), stream_ptr())
         x_in, t_in = x_t, t
         if self.cfg_ctx is not None:                       # DreamArtistPTContext.pre: 'b c h w -> (pn b) c h w', timesteps.repeat(2)
             x_in, t_in = torch.cat([x_t, x_t], 0), torch.cat([t, t], 0)
@@ -523,19 +524,11 @@ class LoraTrainStep:
         self.noise_pred = leaf
         dpred = torch.empty_like(leaf)
         gscale = 1.0 / self.accum                          # accelerator.backward: loss / gradient_accumulation_steps
-        if grouped is not None:                            # sum_g loss_weight_g * (criterion * mask).mean() over the groups' samples
-            mode, gamma = self.loss_cfg if self.loss_cfg is not None else (-1, 1.0)
-            C = leaf.shape[1]
-            ws = grouped["ws"]
-            call("hcp_eps_loss_grouped", leaf.data_ptr(), noise.data_ptr(), t.data_ptr(), self.acp.data_ptr(), _lib.ptr(grouped["mask"]),
-                 grouped["scale"].data_ptr(), grouped["group"].data_ptr(), grouped["loss"].numel(), mode, gamma, B, C, per_image // C,
-                 gscale, grouped["loss"].data_ptr(), dpred.data_ptr(), ws.data_ptr(), ws.numel() * 4, stream_ptr())
-        elif self.loss_cfg is None:
-            call("hcp_mse_loss", leaf.data_ptr(), noise.data_ptr(), leaf.numel(), gscale, self.loss.data_ptr(), dpred.data_ptr(), stream_ptr())
-        else:
-            mode, gamma = self.loss_cfg
-            call("hcp_snr_mse_loss", leaf.data_ptr(), noise.data_ptr(), t.data_ptr(), self.acp.data_ptr(), gamma, mode, per_image, leaf.numel(),
-                 gscale, self.loss.data_ptr(), dpred.data_ptr(), stream_ptr())
+        mode, gamma = self.loss_cfg if self.loss_cfg is not None else (-1, 1.0)
+        ws = tables["ws"]                                  # sum_g loss_weight_g * (criterion * mask).mean() over the groups' samples
+        call("hcp_eps_loss_grouped", leaf.data_ptr(), noise.data_ptr(), t.data_ptr(), self.acp.data_ptr(), _lib.ptr(mask),
+             tables["scale"].data_ptr(), tables["group"].data_ptr(), tables["loss"].numel(), mode, gamma, B, C, HW,
+             gscale, tables["loss"].data_ptr(), dpred.data_ptr(), ws.data_ptr(), ws.numel() * 4, stream_ptr())
         pred.backward(dpred)
 
     def _optimizer(self):
@@ -593,37 +586,12 @@ class LoraTrainStep:
         """One micro-step: latents/noise fp32 [B,4,H,W], t int64 [B], ehs fp32 [B,L,ctx] ([2B,L,ctx] = [negative | positive] with
         `cfg_scale`), or int64 token ids [B, 77 R] with a `text_encoder` (host-pinned or device); `added_cond_kwargs` ({'text_embeds' [B,P], 'time_ids' [B,6]}) for SDXL UNets
         (reference wrapper.py:66; {'time_ids'} only, with ids [B, 2 x 77], when an SDXLTextEncoder is trained).  The optimizer runs on every `grad_accum_steps`-th call.  Returns the device loss tensor
-        (shape [1]) of this micro-batch; reading it is the caller's D2H."""
-        dev = self.flat.data.device
-        if self.sdxl:
-            if not added_cond_kwargs or "time_ids" not in added_cond_kwargs:
-                raise ValueError("an SDXL UNet with a text encoder needs added_cond_kwargs={'time_ids': [B, 6]}")
-            if "text_embeds" in added_cond_kwargs:
-                raise ValueError("text_embeds is computed by the trained SDXL text encoder (bigG's projected pooled row): pass "
-                                 "added_cond_kwargs={'time_ids'} only")
-        if not self.use_graph:
-            added = None if added_cond_kwargs is None else {k: v.to(dev, non_blocking=True) for k, v in added_cond_kwargs.items()}
-            self._forward_backward(latents.to(dev, non_blocking=True), noise.to(dev, non_blocking=True), t.to(dev, non_blocking=True),
-                                   ehs.to(dev, non_blocking=True), added)
-            self._finish_micro(self._optimizer)
-            return self.loss
-        if self._graph_kind == "groups":
-            raise RuntimeError("this LoraTrainStep captured its CUDA graphs for step_groups(); call step_groups() (one group for a "
-                               "single batch) or use a separate instance for step()")
-        if self._static is None:
-            self._capture(latents, noise, t, ehs, added_cond_kwargs)
-            self._graph_kind = "step"
-        s = self._static
-        s["latents"].copy_(latents, non_blocking=True)
-        s["noise"].copy_(noise, non_blocking=True)
-        s["t"].copy_(t, non_blocking=True)
-        s["ehs"].copy_(ehs, non_blocking=True)
-        if s["added"] is not None:
-            for k, v in s["added"].items():
-                v.copy_(added_cond_kwargs[k], non_blocking=True)
-        self._graph_fb.replay()
-        self._finish_micro(self._graph_opt.replay)
-        return self.loss
+        (shape [1]) of this micro-batch; reading it is the caller's D2H.  This is `step_groups()` with one group of weight 1.0
+        (`loss_weights` does not apply), and shares its CUDA graphs when that layout was captured."""
+        batch = {"latents": latents, "noise": noise, "t": t, "ehs": ehs}
+        if added_cond_kwargs is not None:
+            batch["added_cond_kwargs"] = added_cond_kwargs
+        return self._run([batch], (1.0,))
 
     def step_groups(self, batches: Sequence[Dict[str, torch.Tensor]]) -> torch.Tensor:
         """One micro-step over several data groups (the reference's `cfgs.data` datasets, e.g. DreamBooth's instance set next to its
@@ -634,104 +602,102 @@ class LoraTrainStep:
         mean, so the gradient is the reference's sum over per-group backward passes.  Groups share the latent shape, the text
         width and the added-cond layout.  Returns the device tensor fp32 [G] of the weighted per-group losses of this micro-step
         (the reference logs the last one)."""
-        G = len(batches)
-        weights = self.loss_weights if self.loss_weights is not None else [1.0] * G
-        if G == 0 or len(weights) != G:
-            raise ValueError(f"step_groups: {G} batches for {len(weights)} loss_weights")
+        weights = self.loss_weights if self.loss_weights is not None else [1.0] * len(batches)
+        if not batches or len(weights) != len(batches):
+            raise ValueError(f"step_groups: {len(batches)} batches for {len(weights)} loss_weights")
+        return self._run(batches, weights)
+
+    def _run(self, batches, weights) -> torch.Tensor:
+        """The micro-step of `step()` and `step_groups()`.  With CUDA graphs the first call captures them for its layout (group batch
+        sizes, loss weights, mask or not); every later call of that layout copies its inputs into the captured buffers and replays."""
         lat, noise, t, ehs, added, mask, sizes = self._concat_groups(batches)
-        dev = self.flat.data.device
+        layout = (sizes, tuple(weights), mask is not None)
+        if self._static is not None and layout != self._static["layout"]:
+            raise ValueError(f"the CUDA graphs were captured for the layout {self._static['layout']} (group batch sizes, loss weights, "
+                             f"mask); this call's is {layout}: use one LoraTrainStep per layout")
         C, HW = lat.shape[1], lat[0, 0].numel()
         if not self.use_graph:
-            tables = self._tables(sizes, weights, C, HW)
-            mask_dev = None if mask is None else mask.to(dev, non_blocking=True)
-            added = None if added is None else {k: v.to(dev, non_blocking=True) for k, v in added.items()}
-            self._forward_backward(lat.to(dev, non_blocking=True), noise.to(dev, non_blocking=True), t.to(dev, non_blocking=True),
-                                   ehs.to(dev, non_blocking=True), added, {**tables, "mask": mask_dev, "sizes": sizes})
+            dev = self.flat.data.device
+            to_dev = lambda x: None if x is None else x.to(dev, non_blocking=True).contiguous()      # noqa: E731
+            self._forward_backward(to_dev(lat), to_dev(noise), to_dev(t), to_dev(ehs),
+                                   None if added is None else {k: to_dev(v) for k, v in added.items()},
+                                   self._tables(sizes, weights, C, HW), to_dev(mask))
             self._finish_micro(self._optimizer)
-            return tables["loss"]
-        if self._graph_kind == "step":
-            raise RuntimeError("this LoraTrainStep captured its CUDA graphs for step(); use a separate instance for step_groups()")
+            return self.loss
         if self._static is None:
-            tables = self._tables(sizes, weights, C, HW)
-            self._capture(lat, noise, t, ehs, added, grouped={**tables, "mask": None if mask is None else mask.to(dev).float().clone(),
-                                                              "sizes": sizes})
-            self._graph_kind = "groups"
+            self._capture(lat, noise, t, ehs, added, self._tables(sizes, weights, C, HW), mask, layout)
         s = self._static
-        grouped = s["grouped"]
-        if sizes != grouped["sizes"]:
-            raise ValueError(f"step_groups: group batch sizes {sizes} differ from the captured {grouped['sizes']}")
-        if mask is not None and grouped["mask"] is None:
-            raise ValueError("step_groups: a mask is given but the CUDA graphs were captured without one (pass a ones mask on the "
-                             "first call to train with masks later)")
-        s["latents"].copy_(lat, non_blocking=True)
-        s["noise"].copy_(noise, non_blocking=True)
-        s["t"].copy_(t, non_blocking=True)
-        s["ehs"].copy_(ehs, non_blocking=True)
+        for k, x in (("latents", lat), ("noise", noise), ("t", t), ("ehs", ehs), ("mask", mask)):
+            if x is not None:
+                s[k].copy_(x, non_blocking=True)
         if s["added"] is not None:
             for k, v in s["added"].items():
                 v.copy_(added[k], non_blocking=True)
-        if grouped["mask"] is not None:
-            if mask is None:
-                grouped["mask"].fill_(1.0)
-            else:
-                grouped["mask"].copy_(mask, non_blocking=True)
-        self._graph_fb.replay()
-        self._finish_micro(self._graph_opt.replay)
-        return grouped["loss"]
+        return self.step_resident()
 
     def _concat_groups(self, batches):
-        """Concatenate the groups' tensors along the batch in the layouts the step expects; refuse groups that cannot share a pass."""
+        """Concatenate the groups' tensors along the batch in the layouts the step expects; refuse groups that cannot share a pass.
+        One group's tensors are handed through as they are: torch.cat of one pinned host tensor returns pageable memory, which
+        would make the H2D copies synchronous."""
         allowed = {"latents", "noise", "t", "ehs", "added_cond_kwargs", "mask"}
         sizes, lats, noises, ts, ehss, addeds, masks = [], [], [], [], [], [], []
         for g, b in enumerate(batches):
             unknown = set(b) - allowed
             if unknown:
-                raise ValueError(f"step_groups: group {g} has unknown keys {sorted(unknown)} (allowed: {sorted(allowed)})")
+                raise ValueError(f"group {g} has unknown keys {sorted(unknown)} (allowed: {sorted(allowed)})")
             lat, nz, tt, eh = b["latents"], b["noise"], b["t"], b["ehs"]
             B = lat.shape[0]
             if lat.dim() != 4 or tuple(nz.shape) != tuple(lat.shape) or tuple(tt.shape) != (B,):
-                raise ValueError(f"step_groups: group {g}: latents [B,C,h,w], noise of the same shape and t [B] (got "
+                raise ValueError(f"group {g}: latents [B,C,h,w], noise of the same shape and t [B] (got "
                                  f"{tuple(lat.shape)}, {tuple(nz.shape)}, {tuple(tt.shape)})")
             if lats and tuple(lat.shape[1:]) != tuple(lats[0].shape[1:]):
-                raise ValueError(f"step_groups: group {g} latents {tuple(lat.shape[1:])} differ from group 0's "
+                raise ValueError(f"group {g} latents {tuple(lat.shape[1:])} differ from group 0's "
                                  f"{tuple(lats[0].shape[1:])}: groups share one latent shape (buckets are not supported)")
             rows = 2 * B if self.cfg_ctx is not None else B
             if eh.shape[0] != rows:
-                raise ValueError(f"step_groups: group {g}: ehs has {eh.shape[0]} rows, expected {rows}"
+                raise ValueError(f"group {g}: ehs has {eh.shape[0]} rows, expected {rows}"
                                  + (" ([negative | positive] with cfg_scale)" if self.cfg_ctx is not None else ""))
             if ehss and tuple(eh.shape[1:]) != tuple(ehss[0].shape[1:]):
-                raise ValueError(f"step_groups: group {g} ehs {tuple(eh.shape[1:])} differs from group 0's {tuple(ehss[0].shape[1:])}")
+                raise ValueError(f"group {g} ehs {tuple(eh.shape[1:])} differs from group 0's {tuple(ehss[0].shape[1:])}")
             ad = b.get("added_cond_kwargs")
+            if self.sdxl:
+                if not ad or "time_ids" not in ad:
+                    raise ValueError(f"group {g}: an SDXL UNet with a text encoder needs added_cond_kwargs={{'time_ids': [B, 6]}}")
+                if "text_embeds" in ad:
+                    raise ValueError(f"group {g}: text_embeds is computed by the trained SDXL text encoder (bigG's projected pooled "
+                                     "row): pass added_cond_kwargs={'time_ids'} only")
             if addeds and (ad is None) != (addeds[0] is None):
-                raise ValueError(f"step_groups: group {g}: added_cond_kwargs must be given for every group or for none")
+                raise ValueError(f"group {g}: added_cond_kwargs must be given for every group or for none")
             if ad is not None:
                 if any(v.shape[0] != B for v in ad.values()):
-                    raise ValueError(f"step_groups: group {g}: added_cond_kwargs rows differ from its batch {B}")
+                    raise ValueError(f"group {g}: added_cond_kwargs rows differ from its batch {B}")
                 if addeds and ({k: tuple(v.shape[1:]) for k, v in ad.items()} != {k: tuple(v.shape[1:]) for k, v in addeds[0].items()}):
-                    raise ValueError(f"step_groups: group {g}: added_cond_kwargs layout differs from group 0's")
+                    raise ValueError(f"group {g}: added_cond_kwargs layout differs from group 0's")
             m = b.get("mask")
             if m is not None:
                 if tuple(m.shape) not in ((B,) + tuple(lat.shape[2:]), (B, 1) + tuple(lat.shape[2:])):
-                    raise ValueError(f"step_groups: group {g}: mask {tuple(m.shape)}, expected [{B}, h, w] or [{B}, 1, h, w] at latent "
+                    raise ValueError(f"group {g}: mask {tuple(m.shape)}, expected [{B}, h, w] or [{B}, 1, h, w] at latent "
                                      f"resolution {tuple(lat.shape[2:])}")
                 m = m.reshape(B, -1).float()
             sizes.append(B)
             lats.append(lat), noises.append(nz), ts.append(tt), ehss.append(eh), addeds.append(ad), masks.append(m)
-        if self.cfg_ctx is not None:                       # [neg_1 .. neg_G | pos_1 .. pos_G], the layout _CfgMixFn expects
+        cat = (lambda xs: xs[0]) if len(sizes) == 1 else (lambda xs: torch.cat(xs, 0))      # noqa: E731
+        if self.cfg_ctx is not None and len(sizes) > 1:    # [neg_1 .. neg_G | pos_1 .. pos_G], the layout _CfgMixFn expects
             ehs = torch.cat([e[:B] for e, B in zip(ehss, sizes)] + [e[B:] for e, B in zip(ehss, sizes)], 0)
         else:
-            ehs = torch.cat(ehss, 0)
-        added = None if addeds[0] is None else {k: torch.cat([a[k] for a in addeds], 0) for k in addeds[0]}
+            ehs = cat(ehss)
+        added = None if addeds[0] is None else {k: cat([a[k] for a in addeds]) for k in addeds[0]}
         mask = None
         if any(m is not None for m in masks):
             HW = lats[0][0, 0].numel()
-            mask = torch.cat([m if m is not None else torch.ones((B, HW), dtype=torch.float32, device=lats[g].device)
-                              for g, (m, B) in enumerate(zip(masks, sizes))], 0)
-        return (torch.cat(lats, 0), torch.cat(noises, 0), torch.cat(ts, 0), ehs, added, mask, tuple(sizes))
+            mask = cat([m if m is not None else torch.ones((B, HW), dtype=torch.float32, device=lats[g].device)
+                        for g, (m, B) in enumerate(zip(masks, sizes))])
+        return (cat(lats), cat(noises), cat(ts), ehs, added, mask, tuple(sizes))
 
     def _tables(self, sizes, weights, C, HW):
-        """Device tables of the grouped loss for these group sizes (built once per layout): sample_scale fp32 [B] = w_g / (B_g C HW),
-        sample_group int32 [B], the per-group loss fp32 [G] and the kernel's workspace."""
+        """Device tables of one group layout (built once per layout): its sizes, sample_scale fp32 [B] = w_g / (B_g C HW),
+        sample_group int32 [B], the per-group loss fp32 [G], the loss kernel's workspace, and the inv_std / group_start tables of
+        add_noise without a pyramid: every 1/std is 1, so one group spans the batch whatever G is."""
         key = (sizes, tuple(weights), C, HW)
         tab = self._group_tables.get(key)
         if tab is None:
@@ -739,9 +705,11 @@ class LoraTrainStep:
             scale = [w / (B * C * HW) for w, B in zip(weights, sizes) for _ in range(B)]
             group = [g for g, B in enumerate(sizes) for _ in range(B)]
             nbytes = _lib.lib().hcp_eps_loss_grouped_workspace_bytes(sum(sizes), C * HW)
-            tab = {"scale": torch.tensor(scale, dtype=torch.float32, device=dev), "group": torch.tensor(group, dtype=torch.int32, device=dev),
-                   "loss": torch.zeros(len(sizes), dtype=torch.float32, device=dev),
-                   "ws": torch.zeros((nbytes + 3) // 4, dtype=torch.float32, device=dev)}
+            tab = {"sizes": sizes, "scale": torch.tensor(scale, dtype=torch.float32, device=dev),
+                   "group": torch.tensor(group, dtype=torch.int32, device=dev), "loss": torch.zeros(len(sizes), dtype=torch.float32, device=dev),
+                   "ws": torch.zeros((nbytes + 3) // 4, dtype=torch.float32, device=dev),
+                   "inv_std": torch.ones(1, dtype=torch.float32, device=dev),
+                   "group_start": torch.tensor([0, sum(sizes)], dtype=torch.int32, device=dev)}
             self._group_tables[key] = tab
         return tab
 
@@ -751,7 +719,7 @@ class LoraTrainStep:
             raise RuntimeError("call step() once before step_resident()")
         self._graph_fb.replay()
         self._finish_micro(self._graph_opt.replay)
-        return self.loss if self._graph_kind != "groups" else self._static["grouped"]["loss"]
+        return self.loss
 
     def ema_state(self) -> Dict[nn.Parameter, torch.Tensor]:
         """{parameter: EMA tensor view} (what ModelEMA.state_dict() holds for the trainable parameters)."""
@@ -775,14 +743,15 @@ class LoraTrainStep:
             self.pyramid.state.copy_(saved[4])
         self.flat.grad.zero_()
 
-    def _capture(self, latents, noise, t, ehs, added=None, grouped=None):
+    def _capture(self, latents, noise, t, ehs, added, tables, mask, layout):
         dev = self.flat.data.device
         self._static = {
             "latents": latents.to(dev).float().contiguous().clone(), "noise": noise.to(dev).float().contiguous().clone(),
             "t": t.to(dev).long().contiguous().clone(),
             "ehs": (ehs.to(dev).long() if self.te is not None else ehs.to(dev).float()).contiguous().clone(),
             "added": None if added is None else {k: v.to(dev).float().contiguous().clone() for k, v in added.items()},
-            "grouped": grouped,
+            "mask": None if mask is None else mask.to(dev).float().contiguous().clone(),
+            "tables": tables, "layout": layout,
         }
         s = self._static
         # warm-up on a side stream (builds the packed weights, tensor maps, autograd metadata) -- parameters, optimizer state and
@@ -794,7 +763,7 @@ class LoraTrainStep:
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
             for _ in range(2):
-                self._forward_backward(s["latents"], s["noise"], s["t"], s["ehs"], s["added"], s["grouped"])
+                self._forward_backward(s["latents"], s["noise"], s["t"], s["ehs"], s["added"], s["tables"], s["mask"])
                 self._optimizer()
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
@@ -802,7 +771,7 @@ class LoraTrainStep:
         before = _lib.launch_count
         self._graph_fb = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self._graph_fb):
-            self._forward_backward(s["latents"], s["noise"], s["t"], s["ehs"], s["added"], s["grouped"])
+            self._forward_backward(s["latents"], s["noise"], s["t"], s["ehs"], s["added"], s["tables"], s["mask"])
         self._graph_opt = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self._graph_opt):
             self._optimizer()

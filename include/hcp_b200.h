@@ -376,10 +376,6 @@ int hcp_lora_grad_pair(const void* U, const void* x, int64_t ldx, int64_t K, con
 /* ------------------------------------------------------------------------------------------------
  * The step either side of the UNet call (reference hcpdiff/train_ac.py:437-447, 485-494, 506-515).
  * ---------------------------------------------------------------------------------------------- */
-int hcp_add_noise(const float* x0, const float* noise, const int64_t* t, const float* alphas_cumprod, int64_t B,
-                  int64_t per_image, float* xt, hcp_stream_t stream);
-int hcp_mse_loss(const float* pred, const float* target, int64_t n, float grad_scale, float* loss_sum /* += mean */,
-                 float* dpred /* may be NULL */, hcp_stream_t stream);
 int hcp_sumsq(const float* g, int64_t n, float* out /* += */, hcp_stream_t stream);
 int hcp_adamw_flat(float* p, const float* g, float* m, float* v, int64_t n, const float* lr_device, float beta1, float beta2,
                    float eps, float weight_decay, float grad_scale, const float* sumsq_device, float max_norm,
@@ -495,19 +491,14 @@ int hcp_adafactor_flat(float* p, const float* g, float* state, float* exp_avg, f
                        int64_t nfactor_items, const float* hyper_device, int* steps_device, int32_t ngroups, float grad_scale,
                        const float* sumsq_device, float max_norm, hcp_stream_t stream);
 
-/* SNR-weighted eps loss (reference hcpdiff/loss/min_snr_loss.py:5-52): loss_sum += mean_i(w(t_b) (pred_i - target_i)^2),
- * dpred_i = 2 w d grad_scale / n;  snr = acp/(1-acp);  mode 0 MinSNRLoss w = min(gamma/snr, 1), 1 SoftMinSNRLoss, 2 KDiffMinSNRLoss,
- * 3 EDMLoss.  t int64 [n / per_image]. */
-int hcp_snr_mse_loss(const float* pred, const float* target, const int64_t* t, const float* alphas_cumprod, float gamma, int32_t mode,
-                     int64_t per_image, int64_t n, float grad_scale, float* loss_sum /* += */, float* dpred /* may be NULL */,
-                     hcp_stream_t stream);
 /* The eps loss over the data groups of one step (reference train_ac.py:467-482, get_loss :506-515 with its per-pixel mask):
  *   group_loss[g] += sum_{b: sample_group[b] == g} sample_scale[b] * sum_{c,p} w(t_b) mask[b,p] (pred - target)^2
  *   dpred = 2 w(t_b) mask[b,p] (pred - target) sample_scale[b] grad_scale
  * pred / target / dpred fp32 [B, C, HW]; mask fp32 [B, HW] broadcast over channels (NULL = ones); sample_scale fp32 [B] =
  * loss_weight_g / (B_g C HW) (mean over all elements, not over the mask); sample_group int32 [B] in [0, ngroups); mode -1 plain
- * MSE (t / alphas_cumprod unused, may be NULL), 0..3 the weights of hcp_snr_mse_loss.  All tables are in device memory (CUDA-graph
- * capturable).  workspace: hcp_eps_loss_grouped_workspace_bytes(B, C * HW) bytes of block partials, summed per group in a fixed
+ * MSE, w = 1 (t / alphas_cumprod unused, may be NULL); modes 0..3 the SNR weights of reference hcpdiff/loss/min_snr_loss.py:5-52,
+ * snr = acp/(1-acp): 0 MinSNRLoss w = min(gamma/snr, 1), 1 SoftMinSNRLoss, 2 KDiffMinSNRLoss, 3 EDMLoss (t int64 [B]).  All
+ * tables are in device memory (CUDA-graph capturable).  workspace: hcp_eps_loss_grouped_workspace_bytes(B, C * HW) bytes of block partials, summed per group in a fixed
  * order by a second launch, so repeated calls give bit-identical losses. */
 size_t hcp_eps_loss_grouped_workspace_bytes(int64_t B, int64_t per_image);
 int hcp_eps_loss_grouped(const float* pred, const float* target, const int64_t* t, const float* alphas_cumprod, const float* mask,
@@ -562,7 +553,8 @@ int hcp_pyramid_noise(const float* noise, const int32_t* plan, const int32_t* gr
                       int32_t level, double discount, double step_size, int64_t B, int64_t C, int64_t H, int64_t W, float* target,
                       float* inv_std /* fp32 [ngroups] */, void* workspace, size_t workspace_bytes, hcp_stream_t stream);
 /* x_t = sqrt(acp[t]) x0 + sqrt(1 - acp[t]) (noise * inv_std[g(b)])  (the base scheduler's DDPMScheduler.add_noise on the normalised
- * pyramid noise, pyramid_noise.py:32), g(b) from group_start as above.  hcp_add_noise is the same with inv_std = 1. */
+ * pyramid noise, pyramid_noise.py:32), g(b) from group_start as above.  With inv_std = 1 it is DDPMScheduler.add_noise (reference
+ * make_noise, train_ac.py:437-447), bit for bit. */
 int hcp_add_noise_scaled(const float* x0, const float* noise, const int64_t* t, const float* alphas_cumprod, const float* inv_std,
                          const int32_t* group_start, int32_t ngroups, int64_t B, int64_t per_image, float* xt, hcp_stream_t stream);
 

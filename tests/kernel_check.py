@@ -68,8 +68,8 @@ per element against float64 (worst over all cases and two runs -- the atomics' o
           1 - beta2^step loses digits at small steps)
   EMA / (|e| + |p - e|)                                 1.07e-7                                  3e-7
   add_noise / (sqrt(a) |x0| + sqrt(1 - a) |noise|)      1.30e-7                                  3e-7
-  MSE / Min-SNR loss / mean (592 fp32 atomics)          7.02e-6                                  2e-5
-  dpred (relative)                                      4.51e-7                                  1e-6
+  MSE / Min-SNR loss / mean (fixed-order sums)          2.85e-7                                  1e-6
+  dpred (relative)                                      4.38e-7                                  1e-6
   CFG mix / (|u| + |s| (|u| + |c|))                     1.55e-7                                  4e-7
   GEGLU, exact GELU, quick-GELU fwd / bwd, in bf16     0.503 (not correctly rounded: at most    1
           ulps of the exact value                       1.6e-4 of the elements)

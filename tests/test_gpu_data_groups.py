@@ -8,6 +8,7 @@ bf16 step vs fp32 oracle loss 2e-2, gradients rel-L2 5e-2, update cosine >= 0.9.
 product run as one pass per group: rel-L2 1e-2 (the same bf16 arithmetic per sample, reductions over a different batch)."""
 import math
 import os
+import re
 import subprocess
 import sys
 
@@ -112,26 +113,6 @@ def test_grouped_loss_kernel_matches_fp64(golden_dir, B, HW):
                     l1, d1 = run_kernel(pred, target, t, torch.ones((B, HW), device=DEV), groups, weights, mode, gamma, grad_scale=0.5)
                     l2, _ = run_kernel(pred, target, t, None, groups, weights, mode, gamma, grad_scale=0.5)
                     assert torch.equal(loss, l1) and torch.equal(d, d1) and torch.equal(loss, l2), key
-
-
-def test_grouped_loss_kernel_one_group_matches_existing_losses(golden_dir):
-    fx = torch.load(os.path.join(golden_dir, "ref_step.pt"))["loss"]
-    pred, target, t = fx["pred"].to(DEV), fx["target"].to(DEV), fx["t"].to(DEV)
-    B, per = pred.shape[0], pred[0].numel()
-    acp = U.ddpm_alphas_cumprod().to(DEV)
-    groups = [0] * B
-    loss, d = run_kernel(pred, target, t, None, groups, [1.0], -1, 1.0, grad_scale=0.5)
-    l0, d0 = torch.zeros(1, device=DEV), torch.empty_like(pred)
-    call("hcp_mse_loss", pred.data_ptr(), target.data_ptr(), pred.numel(), 0.5, l0.data_ptr(), d0.data_ptr(), stream_ptr())
-    assert abs(float(loss) - float(l0)) <= 1e-6 * float(l0) and rel_l2(d, d0) <= 1e-6
-    for key in fx["out"]:
-        kind, gamma = key.split(":")
-        mode = {v: k for k, v in MODES.items()}[kind]
-        loss, d = run_kernel(pred, target, t, None, groups, [1.0], mode, float(gamma))
-        l0.zero_()
-        call("hcp_snr_mse_loss", pred.data_ptr(), target.data_ptr(), t.data_ptr(), acp.data_ptr(), float(gamma), mode, per, pred.numel(), 1.0,
-             l0.data_ptr(), d0.data_ptr(), stream_ptr())
-        assert abs(float(loss) - float(l0)) <= 1e-6 * abs(float(l0)) and rel_l2(d, d0) <= 1e-6, key
 
 
 def test_grouped_loss_kernel_refuses_bad_arguments_before_launch():
@@ -361,6 +342,10 @@ def test_groups_with_cfg_scale_match_per_group_passes():
 
 
 def test_one_group_without_mask_matches_step():
+    """step() is step_groups() with one group of weight 1.  In the grouped run the last call is a step(): it replays the graphs
+    step_groups() captured for that layout instead of capturing its own.  The first loss is computed from equal parameters and
+    must be equal bit for bit; after that the LoRA weight gradients (summed with fp32 atomics) differ in their last bits between
+    any two runs, the same path twice included, so parameters, moments and later losses are compared with tolerances."""
     spec = U.TINY
     results = []
     for grouped in (False, True):
@@ -370,17 +355,20 @@ def test_one_group_without_mask_matches_step():
         losses = []
         for it in range(3):
             lat, noise, t, ehs = U.synthetic_batch(4, spec, seed=500 + it)
-            if grouped:
-                losses.append(float(step.step_groups([{"latents": lat, "noise": noise, "t": t, "ehs": ehs}])[0].cpu()))
+            if grouped and it < 2:
+                losses.append(step.step_groups([{"latents": lat, "noise": noise, "t": t, "ehs": ehs}]).cpu())
+                graph = step._graph_fb
             else:
-                losses.append(float(step.step(lat, noise, t, ehs).cpu()))
-        results.append((losses, step.flat.data.clone(), step.m.clone()))
+                losses.append(step.step(lat, noise, t, ehs).cpu())
+        if grouped:
+            assert step._graph_fb is graph
+        results.append((torch.cat(losses), step.flat.data.clone(), step.m.clone()))
     (l0, p0, m0), (l1, p1, m1) = results
-    assert all(abs(a - b) <= 1e-4 * abs(a) for a, b in zip(l0, l1)), (l0, l1)
+    assert torch.equal(l0[0], l1[0]) and torch.allclose(l0, l1, rtol=1e-4, atol=0), (l0, l1)
     assert rel_l2(p1, p0) <= 1e-4 and rel_l2(m1, m0) <= 1e-3
 
 
-def test_step_groups_refusals():
+def test_step_groups_refusals_and_layout_check():
     spec = U.TINY
     sd = U.init_params(spec)
     unet, groups, _, _ = lora_unet(spec, sd)
@@ -399,7 +387,7 @@ def test_step_groups_refusals():
         step.step_groups([bad_mask, ok[1]])
     assert step._static is None                                  # nothing was captured by the refused calls
     step.step_groups(ok)
-    with pytest.raises(RuntimeError, match="step_groups"):
+    with pytest.raises(ValueError, match=re.escape("((2, 1), (1.0, 0.5), True)") + ".*" + re.escape("((2,), (1.0,), False)")):
         b = ok[0]
         step.step(b["latents"], b["noise"], b["t"], b["ehs"])
 

@@ -333,7 +333,7 @@ def test_null_scheduler_step_is_unchanged_and_cfg_scale_runs():
         assert step.pyramid is None
         lat, nz, t, ehs = U.synthetic_batch(2, spec, seed=77)
         results.append((float(step.step(lat, nz, t, ehs).cpu()), step.flat.data.clone(), step.acp.clone()))
-    # the same kernels on the same table; the MSE loss sums its blocks with atomics, so runs agree to rounding, not bit for bit
+    # the same kernels on the same table
     assert torch.equal(results[0][2], results[1][2])
     assert abs(results[0][0] - results[1][0]) <= 1e-6 * abs(results[0][0])
     assert float((results[0][1] - results[1][1]).norm() / results[0][1].norm()) <= 1e-5

@@ -64,29 +64,39 @@ def build(spec, sd, cfg_lora, lora_oracle):
 # ----------------------------------------------------------------------------------------------------------------------
 # flat kernels vs torch / the pinned step oracle on equal inputs
 # ----------------------------------------------------------------------------------------------------------------------
-def test_add_noise_and_losses_match_oracle(golden_dir):
+def test_add_noise_and_eps_loss_match_oracle(golden_dir):
     fx = torch.load(os.path.join(golden_dir, "ref_step.pt"))["loss"]
     acp = U.ddpm_alphas_cumprod()
     pred, target, t = fx["pred"].to(DEV), fx["target"].to(DEV), fx["t"].to(DEV)
-    B, per = pred.shape[0], pred[0].numel()
-    # add_noise (reference make_noise / DDPMScheduler.add_noise, train_ac.py:437-447)
+    B, C, HW = pred.shape[0], pred.shape[1], pred[0, 0].numel()
+    # add_noise (reference make_noise / DDPMScheduler.add_noise, train_ac.py:437-447): the scaled kernel with 1/std = 1, one group
     xt = torch.empty_like(pred)
-    call("hcp_add_noise", pred.data_ptr(), target.data_ptr(), t.data_ptr(), acp.to(DEV).data_ptr(), B, per, xt.data_ptr(), stream_ptr())
+    inv_std, group_start = torch.ones(1, device=DEV), torch.tensor([0, B], dtype=torch.int32, device=DEV)
+    call("hcp_add_noise_scaled", pred.data_ptr(), target.data_ptr(), t.data_ptr(), acp.to(DEV).data_ptr(), inv_std.data_ptr(),
+         group_start.data_ptr(), 1, B, C * HW, xt.data_ptr(), stream_ptr())
     assert rel_l2(xt, U.add_noise(fx["pred"], fx["target"], fx["t"], acp)) < 1e-6
+    # the eps loss as the step runs it: one group of weight 1, no mask
+    scale = torch.full((B,), 1.0 / pred.numel(), device=DEV)
+    group = torch.zeros(B, dtype=torch.int32, device=DEV)
+    ws = torch.zeros((_lib.lib().hcp_eps_loss_grouped_workspace_bytes(B, C * HW) + 3) // 4, device=DEV)
+    loss, dpred = torch.zeros(1, device=DEV), torch.empty_like(pred)
+
+    def eps_loss(mode, gamma, grad_scale):
+        loss.zero_()
+        call("hcp_eps_loss_grouped", pred.data_ptr(), target.data_ptr(), t.data_ptr(), acp.to(DEV).data_ptr(), None, scale.data_ptr(),
+             group.data_ptr(), 1, mode, gamma, B, C, HW, grad_scale, loss.data_ptr(), dpred.data_ptr(), ws.data_ptr(), ws.numel() * 4,
+             stream_ptr())
     # plain MSE (nn.MSELoss(reduction='none').mean()) incl. the accumulation scale on the gradient only
     p = fx["pred"].clone().requires_grad_(True)
     ref = S.eps_loss(p, fx["target"], fx["t"], acp)
     ref.backward()
-    loss, dpred = torch.zeros(1, device=DEV), torch.empty_like(pred)
-    call("hcp_mse_loss", pred.data_ptr(), target.data_ptr(), pred.numel(), 0.5, loss.data_ptr(), dpred.data_ptr(), stream_ptr())
+    eps_loss(-1, 1.0, 0.5)
     assert abs(float(loss) - float(ref)) < 1e-5 * float(ref) and rel_l2(dpred, 0.5 * p.grad) < 1e-5
     # the four SNR-weighted criteria against the REAL reference classes' outputs
     for key, want in fx["out"].items():
         kind, gamma = key.split(":")
         mode = {"MinSNRLoss": 0, "SoftMinSNRLoss": 1, "KDiffMinSNRLoss": 2, "EDMLoss": 3}[kind]
-        loss.zero_()
-        call("hcp_snr_mse_loss", pred.data_ptr(), target.data_ptr(), t.data_ptr(), acp.to(DEV).data_ptr(), float(gamma), mode, per, pred.numel(), 1.0,
-             loss.data_ptr(), dpred.data_ptr(), stream_ptr())
+        eps_loss(mode, float(gamma), 1.0)
         assert abs(float(loss) - float(want["loss"])) < 2e-5 * abs(float(want["loss"])), key
         assert rel_l2(dpred, want["dpred"]) < 2e-5, key
 

@@ -148,6 +148,12 @@ def test_engine_refusals():
         step.step(lat, noise, t, ids, {"time_ids": torch.zeros(2, 6), "text_embeds": torch.zeros(2, 64)})
     with pytest.raises(ValueError, match="time_ids"):
         step.step(lat, noise, t, ids, None)
+    # step_groups() checks every group the same way, before anything runs
+    good = {"latents": lat, "noise": noise, "t": t, "ehs": ids, "added_cond_kwargs": {"time_ids": torch.zeros(2, 6)}}
+    with pytest.raises(ValueError, match="group 1: .*time_ids"):
+        step.step_groups([good, {k: v for k, v in good.items() if k != "added_cond_kwargs"}])
+    with pytest.raises(ValueError, match="group 1: text_embeds is computed"):
+        step.step_groups([good, dict(good, added_cond_kwargs={"time_ids": torch.zeros(2, 6), "text_embeds": torch.zeros(2, 64)})])
 
 
 def test_train_ac_builds_the_sdxl_pair_for_a_text_time_unet(tmp_path):

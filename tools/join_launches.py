@@ -31,6 +31,7 @@ SEQ = {
     "hcp_adamw_flat": [("incr_step", 0, 1), ("adamw", 1, 1)],
     "hcp_adamw_flat_dev": [("incr_step", 1, 1), ("adamw_flat_dev", 1, 1)],
     "hcp_lion_flat_dev": [("lion_flat_dev", 1, 1)],
+    "hcp_eps_loss_grouped": [("eps_loss_grouped", 1, 1), ("eps_loss_reduce", 1, 1)],
 }
 
 
